@@ -11,7 +11,7 @@ tracked by git):
                           utils.py, nn/*.py) + its two native backends built from the reference's own
                           sources with the reference's own flags (setup.py:147-182):
         cpu.so            sige/cpu/*.cpp + sige/common.cpp              (-g -O3 -fopenmp)
-        cuda.so           sige/cuda/*.{cpp,cu} + sige/common.cpp        (nvcc -O3, TORCH_CUDA_ARCH_LIST=10.0a;
+        cuda.so           sige/cuda/*.{cpp,cu} + sige/common.cpp        (nvcc -O3, TORCH_CUDA_ARCH_LIST=9.0a;
                           the reference's setup.py only builds it when a GPU is visible at build time
                           (setup.py:164) and passes no arch flags; nvcc cross-compiles it here)
     diffusion/            models/ (the DDPM / PD U-Nets: the north-star model file
@@ -23,7 +23,7 @@ tracked by git):
                           no network; SURVEY.md Appendix D) — only so that the model files import
 
 Used by: bench.py --impl reference (the reference's python + sige.cpu + oneDNN on the host cores),
-bench.py --impl reference-cuda (the reference's python + sige.cuda + cuDNN on the same B200),
+bench.py --impl reference-cuda (the reference's python + sige.cuda + cuDNN on the same H100),
 tests/test_gpu_reference_model.py (the reference's unmodified model file on THIS repo's sige.nn) and
 tests/test_gpu_vs_reference_cuda.py (ours vs the reference's own CUDA path).
 """
@@ -111,7 +111,7 @@ def _build_ext(name: str, sources, with_cuda: bool, verbose: bool) -> str:
     os.environ["CXX"] = "/usr/bin/g++"      # the image's /opt/gcc wrapper cannot find libgomp.spec (SURVEY Appendix D)
     os.environ["CC"] = "/usr/bin/gcc"
     if with_cuda:
-        os.environ["TORCH_CUDA_ARCH_LIST"] = "10.0a"
+        os.environ["TORCH_CUDA_ARCH_LIST"] = "9.0a"
     from torch.utils.cpp_extension import load
 
     build_dir = os.path.join(OUT, "_build_" + name)

@@ -5,7 +5,7 @@
         python baseline/run_reference.py --backend cuda|cpu [--steps K --warmup W --ratio r --threads n --dump out.npz]
 
 BENCH / TEST INFRASTRUCTURE.  Everything on the timed path is the reference's: ``sige.nn`` / ``sige.utils`` from
-/root/reference (verbatim copy), ``sige.cuda`` (its five CUDA kernels recompiled for sm_100a) or ``sige.cpu`` (its
+the reference tree (verbatim copy), ``sige.cuda`` (its five CUDA kernels recompiled for sm_90a) or ``sige.cpu`` (its
 OpenMP kernels), its model file diffusion/models/ddpm_arch/sige_fused_unet.py, and PyTorch's conv (cuDNN / oneDNN) —
 fp32, NCHW, stock backend flags, as the reference runs it.  This repository only contributes the deterministic
 weights and synthetic inputs (sige_b200.workloads.ddpm.init_deterministic / synthetic_inputs — numpy-seeded, no

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — DDPM 256x256 denoising steps/sec @ 1.2 % edit (BASELINE.json metric), B200.
+"""bench.py — DDPM 256x256 denoising steps/sec @ 1.2 % edit (BASELINE.json metric), H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference|reference-cuda] [--ratio 0.012]
                     [--path fused|modules] [--no-flush]
@@ -27,7 +27,7 @@ not travel, the in-tree restatement of the same architecture (sige_b200.workload
 --impl reference: the reference itself — its python package, its sige.cpu OpenMP kernels + oneDNN conv — on this
 box's host cores (baseline/run_reference.py in a child process), rank 0 only.
 --impl reference-cuda: the reference itself on the SAME GPU — its python package, its sige.cuda kernels recompiled for
-sm_100a + cuDNN, fp32 — i.e. what a user of the reference gets on a B200 today.
+sm_90a + cuDNN, fp32 — i.e. what a user of the reference gets on an H100 today.
 """
 from __future__ import annotations
 
@@ -80,12 +80,15 @@ def parse():
                     help="reference = the reference's unmodified model file from baseline/_ref on this repo's sige.nn; "
                          "intree = sige_b200.workloads.ddpm (same architecture, same weights)")
     ap.add_argument("--no-flush", action="store_true", help="do not flush L2 between timed steps")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step returned to the caller as DIR/<name>.npy (float32; "
+                         "a fixed seeded sample if it exceeds 64 MB) so that two builds can be compared output for output")
     ap.add_argument("--cpu-steps", type=int, default=20, help="timed steps of the cpu_baseline leg")
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--no-reference-cuda", action="store_true", help="skip the reference's own CUDA path (sige.cuda for sm_100a + cuDNN) timed beside ours on GPU 0")
+    ap.add_argument("--no-reference-cuda", action="store_true", help="skip the reference's own CUDA path (sige.cuda for sm_90a + cuDNN) timed beside ours on GPU 0")
     ap.add_argument("--threads", type=int, default=0, help="(reference arm) torch/OpenMP threads; 0 = sweep")
     ap.add_argument("--_cpu-child", dest="_cpu_child", action="store_true", help=argparse.SUPPRESS)
-    ap.add_argument("--no-tc5", action="store_true", help="engine: use the mma.sync kernel everywhere (default: tcgen05/TMEM/TMA kernel where the geometry allows)")
+    ap.add_argument("--no-tc5", action="store_true", help="engine: use the mma.sync kernel everywhere (default: wgmma/TMA kernel where the geometry allows)")
     ap.add_argument("--no-producer-preop", action="store_true", help="engine: apply GroupNorm affine + SiLU in every gather (reference order) instead of once in the producer's epilogue")
     ap.add_argument("--dense-stem", action="store_true", help="engine: evaluate conv_in on the whole image even when only the active tiles are read")
     ap.add_argument("--no-fused-attention", action="store_true", help="engine: torch matmul/softmax instead of the fused attention-core kernel")
@@ -158,6 +161,27 @@ class ClockSampler:
 # ------------------------------------------------------------------------------------------
 # reference arm / cpu baseline (oracle/ is imported ONLY here)
 # ------------------------------------------------------------------------------------------
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """arrays {name: tensor} -> out_dir/<name>.npy in float32 (float64 stays float64).  Above DUMP_LIMIT_BYTES in all, each
+    array is reduced to a fixed, seeded sample of its flattened elements (the same indices on every run)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    host = {k: v.detach().cpu().numpy() for k, v in arrays.items()}
+    host = {k: v.astype(np.float64 if v.dtype == np.float64 else np.float32) for k, v in host.items()}
+    total = sum(v.nbytes for v in host.values())
+    for k, v in host.items():
+        if total > DUMP_LIMIT_BYTES:
+            n = max(1, int(v.size * DUMP_LIMIT_BYTES // (2 * total)))
+            idx = np.sort(np.random.default_rng(0).choice(v.size, n, replace=False)).astype(np.int64)
+            v = v.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, k + ".npy"), v)
+    log("outputs of the last timed step written to %s (%s)" % (out_dir, ", ".join(sorted(host))))
+
+
 def host_cores() -> int:
     try:
         return len(os.sched_getaffinity(0))
@@ -263,8 +287,8 @@ def run_reference(args):
     if args._cpu_child:
         print(json.dumps(cpu_reference_legacy(args.ratio, max(1, args.steps), max(1, args.warmup), args.threads)), flush=True)
         return
-    steps = max(1, min(args.steps, 40))          # each step is a bounded sample: the whole arm ends within a few minutes
-    warm = max(1, min(args.warmup, 5))
+    steps = max(1, args.steps)
+    warm = max(1, args.warmup)
     r = cpu_reference_subprocess(args.ratio, steps, warm, threads=args.threads)
     line = {
         "impl": "reference", "metric": "DDPM 256x256 denoising steps/sec @1.2% edit", "value": r["value"], "unit": "steps/s",
@@ -280,7 +304,7 @@ def run_reference(args):
 
 
 def run_reference_cuda(args):
-    """The reference's own CUDA path (sige.cuda for sm_100a + cuDNN, fp32, its unmodified python) on GPU 0 of this box."""
+    """The reference's own CUDA path (sige.cuda for sm_90a + cuDNN, fp32, its unmodified python) on GPU 0 of this box."""
     rank = _env_int("RANK", 0)
     if rank != 0:
         return
@@ -296,7 +320,7 @@ def run_reference_cuda(args):
         "impl": "reference-cuda", "metric": "DDPM 256x256 denoising steps/sec @1.2% edit", "value": r["steps_per_s"], "unit": "steps/s",
         "n_gpus": 1, "steps": r["steps"], "warmup": r["warmup"], "ms_per_step": r["ms_per_step"], "device_ms_per_step": r["device_ms_per_step"],
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32 (cuDNN TF32 allowed: %s — torch default)" % r["tf32"], "data": "synthetic",
-        "config": {"workload": workload_name(args.ratio), "device": r["gpu"], "path": "reference sige.nn + sige.cuda (sm_100a rebuild) + cuDNN, eager, NCHW",
+        "config": {"workload": workload_name(args.ratio), "device": r["gpu"], "path": "reference sige.nn + sige.cuda (sm_90a rebuild) + cuDNN, eager, NCHW",
                    "timing": "the reference's Runner.profile protocol: synchronize after every forward, wall clock"},
         "e2e": {"value": r["steps_per_s"], "unit": "steps/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
     }
@@ -496,6 +520,9 @@ def run_ours(args):
     ms = region(args.steps, False)
     ms_e2e = region(args.steps, True)
     clocks = sampler.stop()
+    if args.dump_outputs:
+        # out_host holds the result of the last timed step (the end-to-end region ends with a synchronize)
+        dump_outputs(args.dump_outputs, {"eps" if world == 1 else "eps_rank%d" % rank: out_host})
 
     value = world * n_edits * args.steps / (ms / 1e3)            # denoising steps of ONE edit per second, summed over edits and GPUs
     e2e_value = world * n_edits * args.steps / (ms_e2e / 1e3)
@@ -529,7 +556,7 @@ def run_ours(args):
                 if loader.available(cuda=True):
                     r = _reference_child("cuda", args.ratio, 50, 10, 0, 300)
                     ref_cuda = {"value": r["steps_per_s"], "unit": "steps/s", "ms_per_step": r["ms_per_step"], "steps": r["steps"], "warmup": r["warmup"],
-                                "what": "the reference's unmodified python + sige.cuda (its kernels rebuilt for sm_100a) + cuDNN, fp32 (TF32 convs: torch default), "
+                                "what": "the reference's unmodified python + sige.cuda (its kernels rebuilt for sm_90a) + cuDNN, fp32 (TF32 convs: torch default), "
                                         "eager, its Runner.profile protocol (synchronize after every forward)",
                                 "speedup_of_this_line": value / r["steps_per_s"]}
                 else:
@@ -588,7 +615,7 @@ def run_consumer(args):
     ref = None
     if loader.available(cuda=True):
         dump = os.path.join(tempfile.mkdtemp(prefix="sige_ref_"), "ref.npz")
-        r = _reference_child("cuda", args.ratio, max(1, min(args.steps, 20)), 3, 0, 900, extra=["--workload", args.workload])      # stock settings (TF32 convs): the timing
+        r = _reference_child("cuda", args.ratio, max(1, args.steps), 3, 0, 900, extra=["--workload", args.workload])      # stock settings (TF32 convs): the timing
         _reference_child("cuda", args.ratio, 1, 1, 0, 900, extra=["--workload", args.workload, "--no-tf32", "--dump", dump])         # exact fp32: the parity target
         ref = (r, np.load(dump))
         log("reference CUDA path: %.2f ms/step" % r["ms_per_step"])
@@ -611,7 +638,7 @@ def run_consumer(args):
         return sum(a.elapsed_time(b) for a, b in evs) / k, out
 
     timed(3)
-    ms_mod, out_mod = timed(max(3, min(args.steps, 20)))
+    ms_mod, out_mod = timed(max(1, args.steps))
     net.set_fused(True, dtype=dtype)
     t0 = time.time()
     with torch.no_grad():
@@ -619,7 +646,9 @@ def run_consumer(args):
     compile_s = time.time() - t0
     step = net.fused_step
     timed(3)
-    ms_fused, out_fused = timed(max(5, min(args.steps, 50)))
+    ms_fused, out_fused = timed(max(1, args.steps))
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"out": out_fused})       # what the last timed fused call returned
 
     def rel(a, b):
         return float(np.abs(a - b).max() / np.abs(b).max())
@@ -651,6 +680,8 @@ def run_consumer(args):
 
 def main():
     args = parse()
+    if args.dump_outputs and args.impl != "ours":
+        raise SystemExit("--dump-outputs: the reference arms run in child processes and return timings only; use it with --impl ours")
     if args.workload != "ddpm" and args.impl == "ours":
         run_consumer(args)
         return

@@ -1,5 +1,5 @@
 /*
- * sige_b200.h — C-ABI of the B200-native SIGE tile-sparse hot path.
+ * sige_b200.h — C-ABI of the H100-native SIGE tile-sparse hot path.
  *
  * This is the drop-in boundary: plain pointers, sizes and a cudaStream_t; no torch
  * types.  It replaces the reference's pybind surface `sige.cuda`
@@ -60,7 +60,7 @@ typedef struct {
 /* ------------------------------------------------------------------------- */
 const char *sige_last_error(void);
 int sige_abi_version(void);
-/* "sm_100a" etc. — the architecture the kernels in this library were built for. */
+/* "sm_90a" etc. — the architecture the kernels in this library were built for. */
 const char *sige_built_arch(void);
 /* reference sige/common.cpp:17-23: "identity" / "swish" -> sige_act_t, -1 if unknown
  * (the reference has undefined behaviour for unknown names). */
@@ -207,7 +207,7 @@ typedef struct {
     /* ---- optional extra destinations ---- */
     int n_aux;              /* 0, 1 or 2 */
     sige_conv_aux_t aux[2];
-    /* ---- optional fused 1x1 shortcut (tcgen05 path, 3x3 main conv only) ----
+    /* ---- optional fused 1x1 shortcut (wgmma path, 3x3 main conv only) ----
      * out += conv1x1(src2) + bias2 on the main tiles whose sc_flags byte is non-zero (sc_flags == NULL: all); on the
      * other tiles `residual` (the CACHED shortcut output) is added instead.  This is the reference's
      * ScatterWithBlockResidual (sige/cuda/scatter_kernel.cu:46-74,119-146) folded into conv2's launch: the shortcut's
@@ -229,7 +229,7 @@ typedef struct {
 /* Launch with programmatic dependent launch: the kernel prefetches its weights while the previous kernel
  * of the stream drains, and waits (griddepcontrol.wait) before touching activations. */
 #define SIGE_CONV_PDL 1
-/* Use the tcgen05 / TMEM / TMA kernel when the geometry allows (3x3 s1 on 6x6 tiles, 1x1 on 4x4 tiles,
+/* Use the wgmma / TMA kernel when the geometry allows (3x3 s1 on 6x6 tiles, 1x1 on 4x4 tiles,
  * Cout % 64 == 0); otherwise the mma.sync kernel runs. */
 #define SIGE_CONV_TC5 2
 /* `idx` is a fixed-capacity list (B == 1): real tiles packed at the front, SIGE_TILE_NONE entries behind them, possibly whole
@@ -265,7 +265,7 @@ int sige_tile_conv_generic(const void *x, const void *w, const void *bias, void 
 /* Launch plan sige_tile_conv would use for a descriptor: pure host logic (no pointer is dereferenced, nothing is
  * launched) — exported so that the tile-width / split-K / ring heuristics can be tested without a GPU. */
 typedef struct {
-    int path;      /* 1 = tcgen05 kernel, 0 = mma.sync kernel (the fields below are then 0) */
+    int path;      /* 1 = wgmma kernel, 0 = mma.sync kernel (the fields below are then 0) */
     int bn;        /* output channels per CTA (64 or 128) */
     int ksplit;    /* K slices = thread-block cluster size (1, 2, 4, 8) */
     int deep_ring; /* 1 = one halo buffer + five weight stages (split-K launches of the narrow 3x3 configuration) */
@@ -340,9 +340,10 @@ int sige_spade_modulate(const void *x, long long x_pixel_stride, const void *gam
 /* ------------------------------------------------------------------------- */
 /* diagnostics                                                                */
 /* ------------------------------------------------------------------------- */
-/* In-kernel timeline: while `buf` (device int64, 16 slots per CTA of the NEXT sige_tile_conv launch that takes the tcgen05
+/* In-kernel timeline: while `buf` (device int64, 16 slots per CTA of the NEXT sige_tile_conv launch that takes the wgmma
  * path) is set, that launch stamps %globaltimer per CTA — slot 0 entry, 3 dependency released + loads issued, 4 halo stored,
- * 5/6 MMA issue begin/end, 7 accumulator ready, 8/9 exchange, 10 stored, 11 exit.  The pointer is baked into the launch's
+ * 5/6 MMA issue begin/end, 7 accumulators out of registers, 8/9 every partial row present (split-K: exchange landed),
+ * 10 stores of thread 0 issued, 11 exit (every thread's stores issued).  The pointer is baked into the launch's
  * kernel parameters (so it survives CUDA-graph capture); call again (NULL to stop) before the next launch.  bench.py derives
  * the in-step roofline from these stamps; returns 0. */
 int sige_debug_set_trace(void *buf);

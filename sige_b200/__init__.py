@@ -1,4 +1,4 @@
-"""sige_b200 — B200-native (sm_100a) implementation of SIGE's tile-sparse
+"""sige_b200 — H100-native (sm_90a) implementation of SIGE's tile-sparse
 gather -> conv -> scatter hot path behind the reference's operator surface.
 
     sige_b200.nn       SIGEModel / SIGEModule / SIGEConv2d / Gather / Scatter /

@@ -131,7 +131,7 @@ def lib() -> ctypes.CDLL:
         if not os.path.isfile(LIB_PATH):
             raise SigeLibraryMissing(
                 "sige_b200: %s not found. Build it with `python -m sige_b200.build` "
-                "(needs nvcc; targets sm_100a). There is no CPU or PyTorch fallback." % LIB_PATH
+                "(needs nvcc; targets sm_90a). There is no CPU or PyTorch fallback." % LIB_PATH
             )
         handle = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in PROTOTYPES.items():

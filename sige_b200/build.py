@@ -1,11 +1,11 @@
-"""Build the C-ABI shared library (include/sige_b200.h) for sm_100a, in-tree.
+"""Build the C-ABI shared library (include/sige_b200.h) for sm_90a (H100), in-tree.
 
     python -m sige_b200.build [--force] [--verbose]
 
 Produces sige_b200/lib/libsige_b200.so with plain `nvcc` (no torch, no cmake): the
 library has no dependency on libtorch — PyTorch only supplies device memory and
 streams on the Python side.  Replaces reference setup.py:147-182 (which has no arch
-flags at all); this build targets exactly one architecture, sm_100a.
+flags at all); this build targets exactly one architecture, sm_90a.
 """
 from __future__ import annotations
 
@@ -22,10 +22,10 @@ LIB_PATH = os.path.join(LIB_DIR, "libsige_b200.so")
 OBJ_DIR = os.path.join(HERE, "lib", "_obj")
 STAMP = os.path.join(LIB_DIR, "build.stamp")
 
-ARCH = "sm_100a"
+ARCH = "sm_90a"
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "--expt-relaxed-constexpr",
     "-Xcompiler", "-fPIC",
@@ -77,7 +77,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
         objs = list(ex.map(compile_one, sources()))
-    cmd = [NVCC, "-shared", "-o", LIB_PATH, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
+    cmd = [NVCC, "-shared", "-o", LIB_PATH, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-lcudart_static", "-ldl", "-lrt", "-lpthread"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

@@ -1,4 +1,4 @@
-// common.cuh — shared device helpers for the sm_100a SIGE kernels.
+// common.cuh — shared device helpers for the sm_90a SIGE kernels.
 //
 // Replaces reference sige/common.cpp (enums, broadcastable) and
 // sige/cuda/common_cuda.cu (binary_op_array_cuda, activation_cuda).
@@ -11,6 +11,27 @@
 #include "../../include/sige_b200.h"
 
 namespace sige {
+
+// Streaming multiprocessors of the current device, queried once per device; 132 (H100 SXM) where no device can be queried
+// (host-only planning on a machine without a GPU).
+constexpr int kDefaultSMs = 132;
+inline int sm_count() {
+    static int cache[64] = {0};
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) {
+        (void)cudaGetLastError();
+        return kDefaultSMs;
+    }
+    if (cache[dev] == 0) {
+        int n = 0;
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
+            (void)cudaGetLastError();
+            return kDefaultSMs;
+        }
+        cache[dev] = n;
+    }
+    return cache[dev];
+}
 
 // ----------------------------------------------------------------------------
 // error plumbing (host)

@@ -3,7 +3,7 @@
 //   GroupNorm statistics of the final activation, folded to per-channel (scale, shift)
 //   conv_out  SiLU(x*scale+shift) -> 3x3, C -> 3 channels   (reference sige_fused_unet.py:431-433)
 // The reference leaves these to cuDNN / ATen; at a 1.2 % edit they are ~20 % of the step
-// (profiles/r01a_launches_engine_step.csv: 244 us for the channels-last GroupNorm alone), and
+// (the channels-last GroupNorm alone was one of the longest launches of the step), and
 // they are pure HBM streams: 16.8 MB written (conv_in) or read (stats, conv_out) at 256x256x128.
 //
 // All three are deterministic (fixed reduction order), stream-ordered and allocation-free.
@@ -506,7 +506,7 @@ int sige_conv_in_nhwc(const void *x, const void *w, const void *bias, void *out,
     const long long total = (long long)B * H * (W / 4) * (Cout / 8);
     SIGE_REQUIRE(total * 4 < 2147483647LL, "sige_conv_in_nhwc: tensor too large");
     const long long want_blocks = (total + 255) / 256;
-    const int grid = (int)(want_blocks < 148LL * 2 ? want_blocks : 148LL * 2);   // persistent: the weight staging is paid once per CTA
+    const int grid = (int)(want_blocks < 2LL * sm_count() ? want_blocks : 2LL * sm_count());   // persistent: the weight staging is paid once per CTA
     cudaStream_t st = (cudaStream_t)stream;
     SIGE_REQUIRE(n_aux >= 0 && n_aux <= 2 && (n_aux == 0 || aux), "sige_conv_in_nhwc: n_aux must be 0..2");
     InAux ia[2] = {{nullptr, nullptr, nullptr, 0}, {nullptr, nullptr, nullptr, 0}};
@@ -536,7 +536,7 @@ int sige_conv_in_nhwc_tiles(const void *x, const void *w, const void *bias, void
     const long long total = (long long)NT * R * S * (Cout / 8);
     SIGE_REQUIRE(total < 2147483647LL && (long long)B * H * W * Cout < 2147483647LL * 8, "sige_conv_in_nhwc_tiles: tensor too large");
     const long long want_blocks = (total + 255) / 256;
-    const int grid = (int)(want_blocks < 148LL * 4 ? want_blocks : 148LL * 4);
+    const int grid = (int)(want_blocks < 4LL * sm_count() ? want_blocks : 4LL * sm_count());
     cudaStream_t st = (cudaStream_t)stream;
     SIGE_REQUIRE(n_aux >= 0 && n_aux <= 2 && (n_aux == 0 || aux), "sige_conv_in_nhwc_tiles: n_aux must be 0..2");
     InAux ia[2] = {{nullptr, nullptr, nullptr, 0}, {nullptr, nullptr, nullptr, 0}};
@@ -552,7 +552,11 @@ int sige_conv_in_nhwc_tiles(const void *x, const void *w, const void *bias, void
     return check_launch("sige_conv_in_nhwc_tiles");
 }
 
-int sige_group_norm_fold_workspace(int B, int C) { return B * 296 * C * 2; }
+// partial-sum blocks of the GroupNorm reduction: two per SM of the current device (the workspace query and the call must see
+// the same device)
+static int gn_partial_blocks() { return 2 * sm_count(); }
+
+int sige_group_norm_fold_workspace(int B, int C) { return B * gn_partial_blocks() * C * 2; }
 
 int sige_group_norm_fold(const void *x, int dtype, int B, int H, int W, int C, int groups, float eps, const void *gamma, const void *beta,
                          float *scale, float *shift, float *workspace, int workspace_floats, sige_stream_t stream) {
@@ -560,7 +564,7 @@ int sige_group_norm_fold(const void *x, int dtype, int B, int H, int W, int C, i
     SIGE_REQUIRE(B > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && C <= 1024 && groups > 0 && C % groups == 0, "sige_group_norm_fold: bad shape (C %% 8, C <= 1024)");
     SIGE_REQUIRE(((uintptr_t)x & 15) == 0, "sige_group_norm_fold: input not 16-byte aligned");
     const int HW = H * W;
-    int nblk = min(296, max(1, HW / 64));
+    int nblk = min(gn_partial_blocks(), max(1, HW / 64));
     SIGE_REQUIRE(workspace_floats >= B * nblk * C * 2, "sige_group_norm_fold: workspace too small (%d floats, need %d)", workspace_floats, B * nblk * C * 2);
     const int CV = C / 8;
     SIGE_REQUIRE(CV <= 256, "sige_group_norm_fold: too many channels");

@@ -39,7 +39,7 @@ template <typename T>
 static int launch_spade(const void *x, long long xs, const void *g, long long gs, const void *b, long long bs, void *out, long long os, long long pixels,
                         int C, float slope, cudaStream_t st) {
     const long long items = pixels * (C / DT<T>::vec);
-    const int blocks = (int)(items + 255 < 148LL * 16 * 256 ? (items + 255) / 256 : 148LL * 16);
+    const int blocks = (int)(items + 255 < 16LL * sm_count() * 256 ? (items + 255) / 256 : 16LL * sm_count());
     spade_modulate_kernel<T><<<blocks, 256, 0, st>>>((const T *)x, xs, (const T *)g, gs, (const T *)b, bs, (T *)out, os, pixels, C, slope);
     return check_launch("sige_spade_modulate");
 }

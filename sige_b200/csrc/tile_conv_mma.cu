@@ -18,7 +18,7 @@
 // fp32 accumulators in shared memory and writes 16-byte channel vectors straight into the
 // destination tensor (coalesced 128-byte lines per pixel), adding bias and the residual.
 //
-// Tensor-core instruction: mma.sync.m16n8k16 (HMMA on sm_100a).  The tcgen05/TMEM variant
+// Tensor-core instruction: mma.sync.m16n8k16 (HMMA on sm_90a).  The wgmma/TMA variant
 // for large edit ratios lives in tile_conv_tc5.cu (when built); this kernel is the latency-
 // oriented path used when the GEMM M dimension is a few hundred rows.
 #include <cooperative_groups.h>
@@ -444,7 +444,7 @@ static int launch_cfg(ConvParams &p, cudaStream_t st) {
     if (p.ksplit <= 0) {
         // auto split-K: aim for ~2 CTAs per SM, keep >= 4 K steps per slice, cluster size <= 8 (portable limit)
         int ks = 1;
-        while (ks < 8 && base * (ks * 2) <= 2 * 148 && J / (ks * 2) >= 4) ks *= 2;
+        while (ks < 8 && base * (ks * 2) <= 2 * sm_count() && J / (ks * 2) >= 4) ks *= 2;
         p.ksplit = ks;
     }
     if (p.ksplit > J) p.ksplit = 1;
@@ -496,8 +496,9 @@ template <typename T> static int launch_tile_conv(ConvParams &p, cudaStream_t st
     const long long cL = ctas_for(p.NT, p.P, p.RS, p.Cout, 128, 128, 288);
     const long long cM = ctas_for(p.NT, p.P, p.RS, p.Cout, 64, 64, 144);
     const long long cS = ctas_for(p.NT, p.P, p.RS, p.Cout, 32, 64, 72);
-    if (cL >= 296) return launch_cfg<T, 2, 8, 4, 2, 288, 5>(p, st);
-    if (cM >= 148 || cS < 0) {
+    const int sms = sm_count();
+    if (cL >= 2 * sms) return launch_cfg<T, 2, 8, 4, 2, 288, 5>(p, st);
+    if (cM >= sms || cS < 0) {
         if (cM > 0) return launch_cfg<T, 2, 4, 2, 2, 144, 8>(p, st);
         return launch_cfg<T, 2, 8, 4, 2, 288, 5>(p, st);
     }
@@ -567,10 +568,10 @@ extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) {
         }
         SIGE_REQUIRE(c2 == a->Cin2 && a->w2_packed && ((uintptr_t)a->w2_packed & 15) == 0, "sige_tile_conv: shortcut channels/weights mismatch");
         SIGE_REQUIRE(!a->src_is_stack && !a->dst_is_stack, "sige_tile_conv: the fused shortcut needs full-tensor source and destination");
-        SIGE_REQUIRE((a->flags & SIGE_CONV_TC5) && tc5_supported(a), "sige_tile_conv: the fused shortcut is implemented by the tcgen05 kernel only (3x3 stride-1 on 6x6 tiles, SIGE_CONV_TC5)");
+        SIGE_REQUIRE((a->flags & SIGE_CONV_TC5) && tc5_supported(a), "sige_tile_conv: the fused shortcut is implemented by the wgmma kernel only (3x3 stride-1 on 6x6 tiles, SIGE_CONV_TC5)");
         SIGE_REQUIRE(a->sc_flags == nullptr || a->residual != nullptr, "sige_tile_conv: sc_flags given without the cached shortcut (residual)");
     }
-    // Blackwell-native path (tcgen05 + TMEM + TMA, tile_conv_tc5.cu) when requested and the geometry fits
+    // Hopper-native path (wgmma + TMA, tile_conv_tc5.cu) when requested and the geometry fits
     if ((a->flags & SIGE_CONV_TC5) && tc5_supported(a)) return tc5_launch(a, (cudaStream_t)stream);
 
     ConvParams p;

@@ -166,7 +166,7 @@ static int launch_depthwise(const SimtParams &p, const void *x, const void *w, c
     const bool vec = p.nhwc && p.Cin % DT<T>::vec == 0 && ((uintptr_t)x % 16 == 0) && ((uintptr_t)out % 16 == 0);
     q.nhwc = p.nhwc ? (vec ? 1 : 2) : 0;          // 1 = NHWC with 16-byte channel vectors, 2 = NHWC scalar, 0 = NCHW scalar
     const long long items = vec ? (long long)p.M * p.P * (p.Cin / DT<T>::vec) : (long long)p.M * p.Cin * p.P;
-    const int blocks = (int)std::min<long long>((items + 255) / 256, 148LL * 16);
+    const int blocks = (int)std::min<long long>((items + 255) / 256, 16LL * sm_count());
     tile_conv_depthwise_kernel<T><<<blocks, 256, 0, st>>>(q, (const T *)x, (const T *)w, (const T *)bias, (T *)out);
     return check_launch("sige_tile_conv_generic(depthwise)");
 }

@@ -1,17 +1,18 @@
-// tile_conv_tc5.cu — Blackwell-native fused gather -> (affine + SiLU) -> tile conv -> (+bias, +residual)
-// -> scatter: tcgen05.mma with the accumulator in TMEM, weights staged by TMA
-// (cp.async.bulk.tensor, 128-byte swizzle), warp-specialised producer / MMA / epilogue roles,
-// mbarrier pipelines, split-K over a thread-block cluster with a distributed-shared-memory reduction.
+// tile_conv_tc5.cu — Hopper-native fused gather -> (affine + SiLU) -> tile conv -> (+bias, +residual)
+// -> scatter: wgmma with register accumulators, weights staged by TMA (cp.async.bulk.tensor, 128-byte
+// swizzle), warp-specialised producer / MMA-consumer roles, mbarrier pipelines, split-K over a
+// thread-block cluster with a distributed-shared-memory reduction.
 //
 // Same contract as tile_conv_mma.cu (one launch == the reference's Gather -> SIGEConv2d -> Scatter
 // triple, reference sige/nn/gather.py:76-89, base.py:88-89, scatter.py:41-60); this file covers the
-// two geometries that make up >90 % of a DDPM step: 3x3 stride-1 on 6x6 halo tiles and 1x1 on 4x4
-// tiles.  Everything else stays on the mma.sync kernel.
+// geometries that make up >90 % of a DDPM step: 3x3 stride-1 on 6x6 halo tiles, 1x1 on 4x4 tiles and
+// 3x3 stride-2 on 5x5 tiles.  Everything else stays on the mma.sync kernel.
 //
-// GEMM view per CTA: D[128 x BN] += A[128 x K] * B[K x BN], K = taps * Cin, UMMA 128 x BN x 16.
+// GEMM view per CTA: D[128 x BN] += A[128 x K] * B[K x BN], K = taps * Cin.  Two consumer warpgroups
+// each own 64 rows and issue wgmma.m64nBNk16 with both operands in shared memory.
 //   * 128 rows = 8 active tiles x 16 output pixels.  For the 3x3 case the row order is
 //     m = oy*32 + tile*4 + ox and the A operand of tap (ky,kx) must be a plainly strided
-//     [128 rows x 64 ch] K-major matrix (UMMA descriptors cannot express a gather).  Trick: keep
+//     [128 rows x 64 ch] K-major matrix (wgmma descriptors cannot express a gather).  Trick: keep
 //     THREE column-shifted copies of the halo tiles in shared memory, copy kx laid out as
 //     [y = 0..5][tile = 0..7][x' = 0..3] rows of 128 bytes holding halo pixel (y, kx + x').  Then
 //     tap (ky,kx) is copy kx shifted by ky*32 rows: row m of the MMA reads row m + 32*ky — a pure
@@ -19,8 +20,9 @@
 //     Cost: each gathered pixel is stored ~2x instead of the 9x of an im2col.
 //   * B (weights, pre-packed [tap][Cin/64][Cout][64]) is a 2-D tensor map {64, taps*Cin/64*Cout}; one TMA
 //     box {64, BN} (a contiguous BN*128-byte run) per (tap, 64-channel chunk) lands in a 128B-swizzled stage of an mbarrier ring.
-//   * one elected thread issues tcgen05.mma; tcgen05.commit releases weight stages / halo buffers and
-//     finally signals the epilogue, which pulls the fp32 accumulator out of TMEM with tcgen05.ld.
+//   * the consumers release weight stages and halo buffers once wgmma.wait_group has retired the MMAs that
+//     read them; the fp32 accumulators are staged through shared memory so that the epilogue writes whole
+//     16-byte runs of each NHWC pixel.
 #include <cooperative_groups.h>
 #include <cuda.h>
 
@@ -36,9 +38,12 @@ namespace tc5 {
 
 constexpr int KC = 64;                 // channels per K chunk = one 128-byte swizzle row
 constexpr int TILES = 8;               // tiles per CTA  (8 x 16 output pixels = 128 GEMM rows)
-constexpr int NPROD_WARPS = 8;         // A-operand producer warps (also the epilogue warps)
-constexpr int NTHREADS = 32 * (2 + NPROD_WARPS);
+constexpr int NCONS_WARPS = 8;         // two MMA-consumer warpgroups (64 GEMM rows each; they also own the accumulators)
+constexpr int NCONS = 32 * NCONS_WARPS;
+constexpr int NPROD_WARPS = 8;         // A-operand producer warps
 constexpr int NPROD = 32 * NPROD_WARPS;
+constexpr int TMA_WARP = NCONS_WARPS + NPROD_WARPS;     // weight loads
+constexpr int NTHREADS = 32 * (TMA_WARP + 1);
 constexpr int A_COPY_BYTES = 6 * TILES * 4 * 128;        // one kx-copy: [6][8][4] rows x 128 B = 24576
 constexpr int A_BUF_BYTES = 3 * A_COPY_BYTES;            // 73728 per 64-channel chunk
 constexpr int EPI_PAD = 4;
@@ -95,7 +100,6 @@ struct Params {
     int ksplit;
     int pdl;
     int push_async;            // split-K exchange: 1 = st.async + per-owner mbarrier, 0 = plain remote stores + cluster barrier
-    int dealloc_late;          // split-K: free TMEM after the reduction instead of before it
     int is_bf16;
     long long *trace;          // development aid: per-CTA clock stamps (16 slots), or nullptr
 };
@@ -186,11 +190,11 @@ __device__ __forceinline__ uint32_t map_rank(uint32_t addr, uint32_t rank) {
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(r) : "r"(addr), "r"(rank));
     return r;
 }
-// 16-byte store into a peer's shared memory that reports its bytes to an mbarrier of that peer: the receiver learns
+// 8-byte store into a peer's shared memory that reports its bytes to an mbarrier of that peer: the receiver learns
 // that the data has landed from its own barrier — no fence and no cluster-wide barrier on the sender's side
-__device__ __forceinline__ void st_async16(uint32_t remote_addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t remote_bar) {
-    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];\n" ::"r"(remote_addr), "r"(a),
-                 "r"(b), "r"(c), "r"(d), "r"(remote_bar)
+__device__ __forceinline__ void st_async8(uint32_t remote_addr, uint32_t a, uint32_t b, uint32_t remote_bar) {
+    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v2.b32 [%0], {%1, %2}, [%3];\n" ::"r"(remote_addr), "r"(a),
+                 "r"(b), "r"(remote_bar)
                  : "memory");
 }
 // 16-byte asynchronous copy global -> shared (LDGSTS): no register staging, so several chunks can be in flight per CTA;
@@ -204,92 +208,135 @@ __device__ __forceinline__ void cp_async_arrive(uint32_t bar) {
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
-
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *tmap, int x, int y, uint32_t bar) {
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];\n" ::"r"(dst),
         "l"(tmap), "r"(x), "r"(y), "r"(bar)
         : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(dst_smem), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
+// wgmma shared-memory descriptor, K-major, 128-byte swizzle (given as (lo, hi) words):
+//   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (= 1, unused for swizzled K-major)
+//   [32,46) stride byte offset >> 4 (= 1024 B between 8-row groups) | [49,52) base offset = 0 (all operand bases are
+//   1024-byte aligned) | [62,64) layout = 1 (SWIZZLE_128B)
+// The issuing warpgroup's instruction stream is the critical path of a latency-bound layer, so per-MMA descriptor
+// arithmetic is one 32-bit add on the low word (start address in 16-byte units; every operand base is below 256 KB,
+// so the 14-bit field never overflows into its neighbours).
+constexpr uint32_t DESC_HI = (1024u >> 4) | (1u << 30);
+__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr) { return (smem_addr >> 4) | (1u << 16); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs that own those registers
+template <int N> __device__ __forceinline__ void fence_acc(float (&d)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Same instruction with the descriptors given as (lo, hi) words: the single issuing thread is the critical path of a
-// latency-bound layer, so per-MMA descriptor arithmetic is reduced to one 32-bit add on the low word (start address
-// in 16-byte units; every operand base is below 256 KB, so the 14-bit field never overflows into its neighbours).
-__device__ __forceinline__ void umma_f16_lohi(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t idesc, uint32_t accumulate) {
+// D[64 x N] (+)= A[64 x 16] * B[16 x N]; fp32 accumulator fragment of thread t of the warpgroup: d[4i + {0,1}] =
+// row 16*(t/32) + (t%32)/4, columns 8i + 2*(t%4) + {0,1}; d[4i + {2,3}] = the same columns, 8 rows further down.
+__device__ __forceinline__ void wgmma_m64n64_f16(float (&d)[32], uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t scale_d) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
         ".reg .b64 da, db;\n"
-        "setp.ne.b32 p, %5, 0;\n"
-        "mov.b64 da, {%1, %3};\n"
-        "mov.b64 db, {%2, %3};\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "r"(a_lo), "r"(b_lo), "r"(hi), "r"(idesc), "r"(accumulate)
+        "setp.ne.b32 p, %35, 0;\n"
+        "mov.b64 da, {%32, %34};\n"
+        "mov.b64 db, {%33, %34};\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{" 
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, da, db, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a_lo), "r"(b_lo), "r"(hi), "r"(scale_d)
         : "memory");
 }
-// true in exactly one (converged) lane of the warp
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
+__device__ __forceinline__ void wgmma_m64n64_bf16(float (&d)[32], uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t scale_d) {
     asm volatile(
         "{\n"
         ".reg .pred p;\n"
-        "elect.sync _|p, 0xffffffff;\n"
-        "selp.u32 %0, 1, 0, p;\n"
+        ".reg .b64 da, db;\n"
+        "setp.ne.b32 p, %35, 0;\n"
+        "mov.b64 da, {%32, %34};\n"
+        "mov.b64 db, {%33, %34};\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{" 
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+        "}, da, db, p, 1, 1, 0, 0;\n"
         "}\n"
-        : "=r"(pred));
-    return pred != 0;
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a_lo), "r"(b_lo), "r"(hi), "r"(scale_d)
+        : "memory");
 }
-constexpr uint32_t DESC_HI = (1024u >> 4) | (1u << 14) | (2u << 29);      // see make_desc
-__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr) { return (smem_addr >> 4) | (1u << 16); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+__device__ __forceinline__ void wgmma_m64n128_f16(float (&d)[64], uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t scale_d) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
+        "{\n"
+        ".reg .pred p;\n"
+        ".reg .b64 da, db;\n"
+        "setp.ne.b32 p, %67, 0;\n"
+        "mov.b64 da, {%64, %66};\n"
+        "mov.b64 db, {%65, %66};\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{" 
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, da, db, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a_lo), "r"(b_lo), "r"(hi), "r"(scale_d)
+        : "memory");
+}
+__device__ __forceinline__ void wgmma_m64n128_bf16(float (&d)[64], uint32_t a_lo, uint32_t b_lo, uint32_t hi, uint32_t scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        ".reg .b64 da, db;\n"
+        "setp.ne.b32 p, %67, 0;\n"
+        "mov.b64 da, {%64, %66};\n"
+        "mov.b64 db, {%65, %66};\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{" 
+        "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+        "}, da, db, p, 1, 1, 0, 0;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a_lo), "r"(b_lo), "r"(hi), "r"(scale_d)
+        : "memory");
 }
 
-// UMMA shared-memory descriptor, K-major, 128-byte swizzle (cute::UMMA::SmemDescriptor):
-//   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (= 1, unused for swizzled K-major)
-//   [32,46) stride byte offset >> 4 (= 1024 B between 8-row groups) | [46,48) version = 1
-//   [49,52) base offset = 0 (all operand bases are 1024-byte aligned) | [61,64) layout = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-    const uint32_t lo = ((smem_addr >> 4) & 0x3FFF) | (1u << 16);
-    const uint32_t hi = (1024u >> 4) | (1u << 14) | (2u << 29);
-    return ((uint64_t)hi << 32) | lo;
-}
-// UMMA instruction descriptor (cute::UMMA::InstrDescriptor), kind::f16, fp32 accumulate, K-major A and B:
-//   [4,6) c_format = 1 (F32) | [7,10) a_format | [10,13) b_format (0 = F16, 1 = BF16)
-//   [15] a_major = 0 | [16] b_major = 0 | [17,23) N >> 3 | [24,29) M >> 4
-__device__ __forceinline__ uint32_t make_idesc(int bn, int bf16) {
-    return (1u << 4) | ((uint32_t)bf16 << 7) | ((uint32_t)bf16 << 10) | ((uint32_t)(bn >> 3) << 17) | ((128u >> 4) << 24);
+template <typename T, int BN>
+__device__ __forceinline__ void wgmma_step(float (&d)[BN / 2], uint32_t a_lo, uint32_t b_lo, uint32_t scale_d) {
+    if constexpr (std::is_same<T, __half>::value) {
+        if constexpr (BN == 64) wgmma_m64n64_f16(d, a_lo, b_lo, DESC_HI, scale_d); else wgmma_m64n128_f16(d, a_lo, b_lo, DESC_HI, scale_d);
+    } else {
+        if constexpr (BN == 64) wgmma_m64n64_bf16(d, a_lo, b_lo, DESC_HI, scale_d); else wgmma_m64n128_bf16(d, a_lo, b_lo, DESC_HI, scale_d);
+    }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -324,15 +371,13 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
     unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     const uint32_t sbase = s32(smem);
     const uint32_t bar0 = sbase + C::OFF_BAR;
-    // barrier layout (8 bytes each): b_full[NSTB] | b_empty[NSTB] | a_full[2] | a_empty[2] | acc_full | tmem slot
+    // barrier layout (8 bytes each): b_full[NSTB] | b_empty[NSTB] | a_full[2] | a_empty[2] | red_full
     auto B_FULL = [&](int s) { return bar0 + 8 * s; };
     auto B_EMPTY = [&](int s) { return bar0 + 8 * (NSTB + s); };
     auto A_FULL = [&](int b) { return bar0 + 8 * (2 * NSTB + b); };
     auto A_EMPTY = [&](int b) { return bar0 + 8 * (2 * NSTB + 2 + b); };
-    const uint32_t ACC_FULL = bar0 + 8 * (2 * NSTB + 4);
-    const uint32_t RED_FULL = bar0 + 8 * (2 * NSTB + 5);     // split-K: all partial rows of the other ranks have landed
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(smem + C::OFF_BAR + 8 * (2 * NSTB + 6));
-    static_assert(8 * (2 * NSTB + 7) <= 256, "barrier block");
+    const uint32_t RED_FULL = bar0 + 8 * (2 * NSTB + 4);     // split-K: all partial rows of the other ranks have landed
+    static_assert(8 * (2 * NSTB + 5) <= 256, "barrier block");
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int tile0 = blockIdx.x * TILES;
@@ -359,14 +404,11 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
     if (warp == 0) {
         if (lane == 0) {
             asm volatile("prefetch.tensormap [%0];\n" ::"l"(&wmap) : "memory");
-            for (int s = 0; s < NSTB; ++s) { mbar_init(B_FULL(s), 1); mbar_init(B_EMPTY(s), 1); }
-            for (int b = 0; b < 2; ++b) { mbar_init(A_FULL(b), NPROD); mbar_init(A_EMPTY(b), 1); }
-            mbar_init(ACC_FULL, 1);
+            for (int s = 0; s < NSTB; ++s) { mbar_init(B_FULL(s), 1); mbar_init(B_EMPTY(s), NCONS_WARPS); }
+            for (int b = 0; b < 2; ++b) { mbar_init(A_FULL(b), NPROD); mbar_init(A_EMPTY(b), NCONS_WARPS); }
             mbar_init(RED_FULL, 1);
             fence_barrier_init();
         }
-        __syncwarp();
-        tmem_alloc(s32(tmem_slot), BN);     // BN fp32 accumulator columns (power of two >= 32)
     } else if (warp == 2) {
         // this CTA's tile origins (constant since set_masks): one global round trip here instead of one per gather thread
         if (S2) {
@@ -392,10 +434,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
         const float dflt = (which == 1 || which == 3) ? 1.f : 0.f;
         for (int e = lane; e < BN; e += 32) s_const[which * BN + e] = (on && src && n0 + e < p.Cout) ? __ldg(src + n0 + e) : dflt;
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     if (p.ksplit > 1) {
         // the receiver's side of the split-K exchange: (ksplit - 1) peers x its share of rows x BN floats will arrive
         if (tid == 0 && p.push_async) mbar_expect_tx(RED_FULL, (uint32_t)(p.ksplit - 1) * (128 / p.ksplit) * BN * 4);
@@ -428,21 +467,11 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
         return ((long long)img * p.dH + hh) * p.dW + ww;
     };
 
-    // destination pixels of this thread's share of the epilogue, resolved here in the prologue (it overlaps the previous
-    // layer): [0] = its GEMM row in the direct path; [0], [1] = its (at most two) items of the split-K reduction
-    int epix[2] = {-1, -1};          // (pixel indices fit 32 bits: checked on the host)
-    if (p.ksplit == 1) {
-        if (warp >= 2) epix[0] = (int)pixel_of((warp & 3) * 32 + lane);
-    } else {
-        const int per = 128 / p.ksplit;
+    float acc[BN / 2];                                 // consumers: this thread's share of its warpgroup's 64 x BN accumulator
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            const int q = tid + i * NTHREADS;
-            if (q < per * (BN / 8)) epix[i] = (int)pixel_of(kr * per + q / (BN / 8));
-        }
-    }
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
 
-    if (warp == 0) {
+    if (warp == TMA_WARP) {
         // ================= TMA producer: weights =================
         if (lane == 0) {
             int s = 0, k = 0;                                          // ring stage and lap
@@ -464,72 +493,82 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
             }
         }
         __syncwarp();
-    } else if (warp == 1) {
-        // ================= MMA issuer =================
-        // One thread issues everything, and in a latency-bound layer its instruction stream IS the critical path (the
-        // first version spent ~17 dependent uniform-datapath instructions per MMA rebuilding both descriptors: ~140
-        // cycles per 128x64x16 MMA against a 32-cycle tensor-core floor).  Descriptor low words are now advanced by
-        // compile-time constants from per-step bases.
-        // The whole warp walks the loop converged; an elected lane issues.
-        const uint32_t d_tmem = __shfl_sync(0xffffffffu, tmem_base, 0);
-        {
-            const uint32_t idesc = make_idesc(BN, p.is_bf16);
-            const uint32_t a_lo0 = desc_lo(sbase + C::OFF_A), b_lo0 = desc_lo(sbase + C::OFF_B);
-            uint32_t accum = 0;
-            int ab = 0, ause = 0;             // halo buffer index and how many times it has been used
-            int st = (j_begin < J_main) ? j_begin % SPC : 0, s = 0, k = 0;
-            for (int j = j_begin; j < j_end; ++j) {
-                const bool is_sc = j >= J_main;
-                if (is_sc) st = 0;
-                if (j == j_begin || st == 0) {                        // a new chunk starts: wait for its halo buffer
-                    mbar_wait(A_FULL(ab), (ause / NAB) & 1);
-                    if (ASYNC) fence_proxy_async();      // cp.async (generic proxy) writes -> visible to the tensor core's async proxy
-                    if (j == j_begin && lane == 0) SIGE_TRACE(5);
-                }
-                mbar_wait(B_FULL(s), k & 1);
-                tc_fence_after();
-                const uint32_t b_step = b_lo0 + s * (C::B_STAGE_BYTES >> 4);
-                uint32_t a_step = a_lo0 + ab * (A_BUF_BYTES >> 4);
-                if (S2) {
-                    a_step += (st == 0 ? 0 : (st == 1 ? 3 : 1)) * ((64 * 128) >> 4);               // ky = st: planes {0,2,4 | 1,3} start at {0, 3, 1}
-                } else if (TAPS == 9) {
-                    if (is_sc) a_step += (A_COPY_BYTES + 32 * 128) >> 4;                           // tap (1,1)
-                    else if (TPS == 3) a_step += st * ((32 * 128) >> 4);                           // ky = st, kx = t
-                    else { const int ky = st / 3; a_step += ky * ((32 * 128) >> 4) + (st - 3 * ky) * (A_COPY_BYTES >> 4); }
-                }
-                const bool chunk_done = is_sc || st == SPC - 1 || j == j_end - 1;
-                if (elect_one()) {
-#pragma unroll
-                    for (int t = 0; t < TPS; ++t) {
-                        if (is_sc && t > 0) break;                    // the shortcut is a single tap: the centre of the 3x3 frame
-#pragma unroll
-                        for (int kk = 0; kk < KC / 16; ++kk)
-                            umma_f16_lohi(d_tmem, a_step + t * (A_COPY_BYTES >> 4) + kk * 2, b_step + t * (C::B_TILE_BYTES >> 4) + kk * 2, DESC_HI, idesc,
-                                          (accum | t | kk) ? 1u : 0u);
-                    }
-                    umma_commit(B_EMPTY(s));                          // weight stage free once these MMAs retire
-                    if (chunk_done) umma_commit(A_EMPTY(ab));         // halo buffer free
-                    if (j == j_end - 1) umma_commit(ACC_FULL);
-                }
-                __syncwarp();
-                accum = 1;
-                if (chunk_done) { ++ause; ab = ause % NAB; }
-                if (++st == SPC) st = 0;
-                if (++s == NSTB) { s = 0; ++k; }
+    } else if (warp < NCONS_WARPS) {
+        // ================= MMA consumers: warpgroup wg multiplies GEMM rows 64*wg .. 64*wg+63 =================
+        // Descriptor low words are advanced by compile-time constants from per-step bases.  A step's MMAs are one
+        // commit group; the weight stage of step j is released once step j+1 has been issued and step j has retired
+        // (wait_group 1), so that the tensor core always has the next step queued.  At the end of a chunk everything
+        // retires (wait_group 0) before its halo buffer is released: with a single halo buffer the producers cannot
+        // start the next chunk earlier.
+        const int wg = warp >> 2;
+        const uint32_t a_lo0 = desc_lo(sbase + C::OFF_A + wg * (64 * 128)), b_lo0 = desc_lo(sbase + C::OFF_B);
+        uint32_t accum = 0;
+        int ab = 0, ause = 0;             // halo buffer index and how many times it has been used
+        int st = (j_begin < J_main) ? j_begin % SPC : 0, s = 0, k = 0;
+        int pend = -1;                    // weight stage of the previous step, not yet released
+        for (int j = j_begin; j < j_end; ++j) {
+            const bool is_sc = j >= J_main;
+            if (is_sc) st = 0;
+            if (j == j_begin || st == 0) {                        // a new chunk starts: wait for its halo buffer
+                mbar_wait(A_FULL(ab), (ause / NAB) & 1);
+                fence_proxy_async();          // gathered data (generic proxy writes) -> visible to the tensor core's async proxy
+                if (j == j_begin && tid == 0) SIGE_TRACE(5);
             }
-            if (lane == 0) SIGE_TRACE(6);
+            mbar_wait(B_FULL(s), k & 1);
+            const uint32_t b_step = b_lo0 + s * (C::B_STAGE_BYTES >> 4);
+            uint32_t a_step = a_lo0 + ab * (A_BUF_BYTES >> 4);
+            if (S2) {
+                a_step += (st == 0 ? 0 : (st == 1 ? 3 : 1)) * ((64 * 128) >> 4);               // ky = st: planes {0,2,4 | 1,3} start at {0, 3, 1}
+            } else if (TAPS == 9) {
+                if (is_sc) a_step += (A_COPY_BYTES + 32 * 128) >> 4;                           // tap (1,1)
+                else if (TPS == 3) a_step += st * ((32 * 128) >> 4);                           // ky = st, kx = t
+                else { const int ky = st / 3; a_step += ky * ((32 * 128) >> 4) + (st - 3 * ky) * (A_COPY_BYTES >> 4); }
+            }
+            const bool chunk_done = is_sc || st == SPC - 1 || j == j_end - 1;
+            fence_acc(acc);
+            wgmma_fence();
+#pragma unroll
+            for (int t = 0; t < TPS; ++t) {
+                if (is_sc && t > 0) break;                    // the shortcut is a single tap: the centre of the 3x3 frame
+#pragma unroll
+                for (int kk = 0; kk < KC / 16; ++kk)
+                    wgmma_step<T, BN>(acc, a_step + t * (A_COPY_BYTES >> 4) + kk * 2, b_step + t * (C::B_TILE_BYTES >> 4) + kk * 2,
+                                      (accum | t | kk) ? 1u : 0u);
+            }
+            wgmma_commit();
+            if (chunk_done) {
+                wgmma_wait<0>();
+                if (lane == 0) {
+                    if (pend >= 0) mbar_arrive(B_EMPTY(pend));
+                    mbar_arrive(B_EMPTY(s));                          // weight stage free
+                    mbar_arrive(A_EMPTY(ab));                         // halo buffer free
+                }
+                pend = -1;
+            } else {
+                wgmma_wait<1>();
+                if (lane == 0 && pend >= 0) mbar_arrive(B_EMPTY(pend));
+                pend = s;
+            }
+            fence_acc(acc);
+            __syncwarp();
+            accum = 1;
+            if (chunk_done) { ++ause; ab = ause % NAB; }
+            if (++st == SPC) st = 0;
+            if (++s == NSTB) { s = 0; ++k; }
         }
-        __syncwarp();
+        wgmma_wait<0>();
+        fence_acc(acc);
+        if (tid == 0) SIGE_TRACE(6);
     } else {
         // ================= A-operand producers: gather + pre-op + swizzled stores =================
-        const int ptid = tid - 64;
+        const int ptid = tid - NCONS;
         if constexpr (S2) {
             // ---- stride-2 geometry: 32 tiles x 5x5 halo pixels x 8 units = 6400 sixteen-byte copies per chunk, pure copy with
             //      cp.async straight into the plane layout described at S2_TILES.  Thread -> (tile = ptid / 8, unit = ptid % 8), and
             //      it walks the 25 pixels of ITS tile: pixel coordinates, planes and destination rows are compile-time constants of
             //      the unrolled loop, per-thread state is the tile origin and two swizzled row offsets.  (A first version kept 25
             //      resolved source offsets per thread: 92 bytes spilled, re-read through a ~20 KB L1 that the gather itself
-            //      thrashes — 12-15 us per chunk, profiles/r02b_graph_timeline_s2_spill.txt.)
+            //      thrashes.)
             static_assert(NPROD == S2_TILES * 8 && UNITS == NPROD * RS, "one (tile, unit) per producer thread");
             const int tl = ptid >> 3, u = ptid & 7;
             const int t = tile0 + tl;
@@ -855,104 +894,93 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
             *reinterpret_cast<uint4 *>(reinterpret_cast<T *>(A.ptr) + pixel * A.C + A.c0 + n) = oa;
         }
     };
+    // accumulator fragment (see wgmma_m64n64_f16): element 4i + h of consumer thread `tid` is GEMM row frag_row(i, h),
+    // columns frag_col(i) + {0, 1} (h = 0: d[4i], d[4i+1]; h = 1: d[4i+2], d[4i+3])
+    const int frag_m = (warp >> 2) * 64 + (warp & 3) * 16 + (lane >> 2), frag_n = 2 * (lane & 3);
+    // the staging area (the halo buffers) is free once both warpgroups' MMAs have retired
+    if (warp < NCONS_WARPS) asm volatile("bar.sync 1, %0;\n" ::"n"(NCONS) : "memory");
+
     if (p.ksplit == 1) {
-        // ---- no split-K: TMEM -> registers -> global.  Two warps per TMEM lane quarter (warp w and w+4 may both touch
-        //      lanes 32*(w%4)..+31) split the BN columns; a thread's share of its pixel is one contiguous run in NHWC.
-        if (warp >= 2) {
-            const int quarter = warp & 3, halfsel = (warp - 2) >> 2;
-            const int m = quarter * 32 + lane;
-            const long long pixel = epix[0];
-            if (p.pdl) asm volatile("griddepcontrol.wait;\n" ::: "memory");
-            mbar_wait(ACC_FULL, 0);
-            tc_fence_after();
-            if (tid == 64) SIGE_TRACE(7);
+        // ---- no split-K: registers -> shared staging [128][EPI_PITCH] -> global, a thread per (row, 8 channels): one
+        //      contiguous 16-byte run in NHWC, consecutive threads on consecutive runs of the same pixel.
+        if (warp < NCONS_WARPS) {
 #pragma unroll
-            for (int cc = 0; cc < BN / 2; cc += 32) {
-                const int c0 = halfsel * (BN / 2) + cc;
-                uint32_t r[32];
-                tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + c0, r);   // warp-collective: every lane takes part
-                if (pixel >= 0) {
+            for (int i = 0; i < BN / 8; ++i)
 #pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        float v[8];
-#pragma unroll
-                        for (int z = 0; z < 8; ++z) v[z] = __uint_as_float(r[8 * g + z]);
-                        if (n0 + c0 + 8 * g < p.Cout) emit(pixel, tl_of(m), n0 + c0 + 8 * g, v);
-                    }
-                }
-            }
-            tc_fence_before();
+                for (int h = 0; h < 2; ++h)
+                    *reinterpret_cast<float2 *>(cst + (frag_m + 8 * h) * C::EPI_PITCH + 8 * i + frag_n) = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
         }
         __syncthreads();
-        if (tid == 0) SIGE_TRACE(8);
-        if (warp == 0) tmem_dealloc(tmem_base, BN);
-        if (tid == 0) { SIGE_TRACE(9); SIGE_TRACE(10); SIGE_TRACE(11); }
+        if (tid == 0) { SIGE_TRACE(7); SIGE_TRACE(8); SIGE_TRACE(9); }       // (no exchange: staged rows are complete)
+        if (p.pdl) asm volatile("griddepcontrol.wait;\n" ::: "memory");
+        for (int q = tid; q < 128 * (BN / 8); q += NTHREADS) {
+            const int m = q / (BN / 8), nv = q - m * (BN / 8);
+            const int n = n0 + nv * 8;
+            if (n >= p.Cout) continue;
+            const long long pixel = pixel_of(m);
+            if (pixel < 0) continue;
+            float v[8];
+            const float4 c0 = *reinterpret_cast<const float4 *>(cst + m * C::EPI_PITCH + nv * 8), c1 = *reinterpret_cast<const float4 *>(cst + m * C::EPI_PITCH + nv * 8 + 4);
+            v[0] = c0.x; v[1] = c0.y; v[2] = c0.z; v[3] = c0.w; v[4] = c1.x; v[5] = c1.y; v[6] = c1.z; v[7] = c1.w;
+            emit(pixel, tl_of(m), n, v);
+        }
+        if (tid == 0) SIGE_TRACE(10);
+        if (p.trace) {                     // (uniform) CTA exit = every thread's stores issued
+            __syncthreads();
+            if (tid == 0) SIGE_TRACE(11);
+        }
         return;
     }
 
-    // ---- split-K: every CTA PUSHES the rows of its partial tile straight from TMEM into the shared memory of the
-    //      rank that owns them (distributed shared memory stores), one cluster barrier, then each rank sums the ks
-    //      slots it received (local reads, fixed order -> deterministic) and stores.  Slot layout at the owner:
-    //      [source rank][row within the owner's share][EPI_PITCH].  Nobody reads remote memory after the barrier, so
+    // ---- split-K: every CTA PUSHES the rows of its partial tile straight from registers into the shared memory of the
+    //      rank that owns them (distributed shared memory stores), then each rank sums the ks slots it received (local
+    //      reads, fixed order -> deterministic) and stores.  Slot layout at the owner: [source rank][row within the owner's
+    //      share][EPI_PITCH]; a rank's own rows go to its halo buffers.  Nobody reads remote memory after the exchange, so
     //      no exit barrier is needed.
     cg::cluster_group cluster = cg::this_cluster();
     const int per = 128 / p.ksplit;
     cluster.barrier_wait();                // (arrived during setup) every CTA of the cluster is running: remote stores are legal
-    if (warp >= 2) {
-        const int quarter = warp & 3, halfsel = (warp - 2) >> 2;
-        const int m = quarter * 32 + lane;
-        const int owner = m / per, lr = m - owner * per;
-        // own rows: this CTA's halo buffers are free once ITS accumulator is complete; remote rows: the owner's slot region
+    if (warp < NCONS_WARPS) {
         float *rslot = reinterpret_cast<float *>(smem + C::OFF_SLOT);
-        float *slot = owner == kr ? cst + lr * C::EPI_PITCH
-                                  : cluster.map_shared_rank(rslot, owner) + ((kr < owner ? kr : kr - 1) * per + lr) * C::EPI_PITCH;
-        mbar_wait(ACC_FULL, 0);
-        tc_fence_after();
-        if (tid == 64) SIGE_TRACE(7);
 #pragma unroll
-        for (int cc = 0; cc < BN / 2; cc += 32) {
-            const int c0 = halfsel * (BN / 2) + cc;
-            uint32_t r[32];
-            tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + c0, r);
+        for (int h = 0; h < 2; ++h) {
+            const int m = frag_m + 8 * h;
+            const int owner = m / per, lr = m - owner * per;
+            const int row_off = ((kr < owner ? kr : kr - 1) * per + lr) * C::EPI_PITCH;      // in the owner's slot region
             if (p.push_async && owner != kr) {
                 // st.async: the bytes are counted by an mbarrier of the OWNER, which then waits on its own barrier only
-                const uint32_t remote = map_rank(sbase + C::OFF_SLOT + (uint32_t)(((kr < owner ? kr : kr - 1) * per + lr) * C::EPI_PITCH + c0) * 4, owner);
+                const uint32_t remote = map_rank(sbase + C::OFF_SLOT + (uint32_t)(row_off + frag_n) * 4, owner);
                 const uint32_t remote_bar = map_rank(RED_FULL, owner);
 #pragma unroll
-                for (int z = 0; z < 8; ++z) st_async16(remote + 16 * z, r[4 * z], r[4 * z + 1], r[4 * z + 2], r[4 * z + 3], remote_bar);
+                for (int i = 0; i < BN / 8; ++i)
+                    st_async8(remote + 32 * i, __float_as_uint(acc[4 * i + 2 * h]), __float_as_uint(acc[4 * i + 2 * h + 1]), remote_bar);
             } else {
-                float4 *dstv = reinterpret_cast<float4 *>(slot + c0);
+                float *slot = owner == kr ? cst + lr * C::EPI_PITCH : cluster.map_shared_rank(rslot, owner) + row_off;
 #pragma unroll
-                for (int z = 0; z < 8; ++z)
-                    dstv[z] = make_float4(__uint_as_float(r[4 * z]), __uint_as_float(r[4 * z + 1]), __uint_as_float(r[4 * z + 2]),
-                                          __uint_as_float(r[4 * z + 3]));
+                for (int i = 0; i < BN / 8; ++i)
+                    *reinterpret_cast<float2 *>(slot + 8 * i + frag_n) = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
             }
         }
-        tc_fence_before();
     }
+    if (tid == 0) SIGE_TRACE(7);
     if (p.pdl) asm volatile("griddepcontrol.wait;\n" ::: "memory");
     if (p.push_async) {
-        __syncthreads();                   // own rows staged; every tcgen05.ld of this CTA has completed
+        __syncthreads();                   // own rows staged
         mbar_wait_cluster(RED_FULL, 0);    // the rows the other ranks pushed have landed
     } else {
         cluster.sync();                    // all partial rows have landed in their owners' slots
     }
     if (tid == 0) { SIGE_TRACE(8); SIGE_TRACE(9); }
-    if (warp == 0 && !p.dealloc_late) { tc_fence_after(); tmem_dealloc(tmem_base, BN); }
-    static_assert(!C::kSplitOk || 64 * (BN / 8) <= 2 * NTHREADS, "at most two items per thread (ksplit >= 2: <= 64 rows per rank)");
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-        const int q = tid + i * NTHREADS;
-        if (q >= per * (BN / 8)) break;
+    const float *rslot = reinterpret_cast<const float *>(smem + C::OFF_SLOT);
+    for (int q = tid; q < per * (BN / 8); q += NTHREADS) {
         const int lr = q / (BN / 8), nv = q - lr * (BN / 8);
         const int n = n0 + nv * 8;
         if (n >= p.Cout) continue;
-        const long long pixel = epix[i];
+        const long long pixel = pixel_of(kr * per + lr);
         if (pixel < 0) continue;
         float v[8];
 #pragma unroll
         for (int z = 0; z < 8; ++z) v[z] = 0.f;
-        const float *rslot = reinterpret_cast<const float *>(smem + C::OFF_SLOT);
 #pragma unroll
         for (int r = 0; r < 8; ++r) {       // fixed rank order: bitwise-deterministic sum
             if (r < p.ksplit) {
@@ -963,9 +991,11 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
         }
         emit(pixel, tl_of(kr * per + lr), n, v);
     }
-    if (warp == 0 && p.dealloc_late) { tc_fence_after(); tmem_dealloc(tmem_base, BN); }
     if (tid == 0) SIGE_TRACE(10);
-    if (tid == 0) SIGE_TRACE(11);
+    if (p.trace) {                         // (uniform) CTA exit = every thread's stores issued
+        __syncthreads();
+        if (tid == 0) SIGE_TRACE(11);
+    }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -995,14 +1025,64 @@ struct Plan {
     int bn, ksplit, deep;
 };
 
+// What the plan needs to know about the device: SMs, and how many CTAs of this kernel (214 KB of shared memory, one CTA per
+// SM) are co-resident for clusters of 1 / 2 / 4 / 8 — cudaOccupancyMaxActiveClusters x cluster size, queried once per device.
+// Without a device (host-only planning) the values of an H100 80GB HBM3 SXM: 132 / 132 / 120 / 120 (66 x2, 30 x4, 15 x8).
+struct Machine {
+    int sms;
+    int max_ctas[9];
+};
+static Machine machine() {
+    static const Machine kH100 = {kDefaultSMs, {0, kDefaultSMs, kDefaultSMs, 0, 120, 0, 0, 0, 120}};
+    static Machine cache[64];
+    static bool done[64] = {false};
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) {
+        (void)cudaGetLastError();
+        return kH100;
+    }
+    if (!done[dev]) {
+        Machine m = kH100;
+        m.sms = sm_count();
+        for (int cs = 1; cs <= 8; cs *= 2) m.max_ctas[cs] = 0;
+        m.max_ctas[1] = m.max_ctas[2] = m.sms;
+        using C = Cfg<64, 9, true>;
+        auto kern = tile_conv_tc5_kernel<__half, 64, 9, true, true>;
+        bool ok = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES) == cudaSuccess;
+        for (int cs = 2; ok && cs <= 8; cs *= 2) {
+            cudaLaunchConfig_t cfg = {};
+            cfg.gridDim = dim3(1, 1, cs);
+            cfg.blockDim = dim3(NTHREADS);
+            cfg.dynamicSmemBytes = C::SMEM_BYTES;
+            cudaLaunchAttribute attr;
+            attr.id = cudaLaunchAttributeClusterDimension;
+            attr.val.clusterDim.x = 1;
+            attr.val.clusterDim.y = 1;
+            attr.val.clusterDim.z = cs;
+            cfg.attrs = &attr;
+            cfg.numAttrs = 1;
+            int n = 0;
+            ok = cudaOccupancyMaxActiveClusters(&n, kern, &cfg) == cudaSuccess && n > 0;
+            if (ok) m.max_ctas[cs] = n * cs;
+        }
+        (void)cudaGetLastError();
+        if (!ok) m = kH100;
+        cache[dev] = m;
+        done[dev] = true;
+    }
+    return cache[dev];
+}
+
 static Plan decide(long long NT, int Cin, int Cout, int taps, int Cin2, int ksplit_req, bool s2 = false) {
     Plan pl;
     const long long m_blocks = ceil_div(NT, s2 ? S2_TILES : TILES);
-    // BN = 128 when that still fills the machine — or when the narrow tiling would need more waves of 148 one-per-SM CTAs
+    // BN = 128 when that still fills the machine — or when the narrow tiling would need more waves of one-per-SM CTAs
     // than the wide one (a batch of edits: 64 row blocks x Cout 256 is 256 narrow CTAs = 2 waves, 128 wide CTAs = 1 wave,
     // and a CTA's gather — the long pole — is the same either way); small problems want more, narrower CTAs
     const long long narrow_ctas = m_blocks * (Cout / 64), wide_ctas = m_blocks * (Cout / 128);
-    const bool wide = !s2 && (Cout % 128 == 0) && (wide_ctas >= 148 || (narrow_ctas > 148 && ceil_div(wide_ctas, 148) < ceil_div(narrow_ctas, 148)));
+    const Machine mc = machine();
+    const long long sms = mc.sms;
+    const bool wide = !s2 && (Cout % 128 == 0) && (wide_ctas >= sms || (narrow_ctas > sms && ceil_div(wide_ctas, sms) < ceil_div(narrow_ctas, sms)));
     pl.bn = wide ? 128 : 64;
     const bool split_ok = pl.bn == 64;                       // Cfg::kSplitOk
     const int tps = (taps == 9 && pl.bn == 64) ? 3 : 1;     // Cfg::TPS
@@ -1010,25 +1090,22 @@ static Plan decide(long long NT, int Cin, int Cout, int taps, int Cin2, int kspl
     const long long base = m_blocks * (Cout / pl.bn);
     int ks = ksplit_req;
     if (ks <= 0) {
-        // one CTA per SM (214 KB smem): co-resident CTAs are 148 / 148 / 132 / 120 for cluster sizes 1 / 2 / 4 / 8
-        // (ncu 'Max Active Clusters': 74 x2, 15 x8); never spill into a second wave.  Splitting pays while every slice
-        // keeps >= min_taps taps (measured: 3 is best, DESIGN.md section 5b).
-        static const int kMaxCtas[9] = {0, 148, 148, 0, 132, 0, 0, 0, 120};
+        // never spill into a second wave of co-resident CTAs (machine()); splitting pays while every slice keeps >= min_taps taps
+        const int *kMaxCtas = mc.max_ctas;
         static int min_taps = getenv("SIGE_TC5_MIN_TAPS") ? atoi(getenv("SIGE_TC5_MIN_TAPS")) : 3;   // tuning knob (taps per K slice)
         ks = 1;
         while (split_ok && ks < 8 && base * (ks * 2) <= kMaxCtas[ks * 2] && (J * tps) / (ks * 2) >= min_taps) ks *= 2;
     }
     if (ks > J || !split_ok) ks = 1;
     // Two consecutive layers are co-resident under programmatic dependent launch (the successor's prologue overlaps this
-    // layer).  A B200 holds 15 clusters of 8 (ncu: Max Active Clusters) — two layers of 8 clusters each do not fit and the 16th
-    // cluster starts, cold, only when a cluster of the predecessor exits (measured: +3 us on every second layer of the dense
-    // 8x8 / 16x16 blocks, profiles/r02_graph_timeline_spread.txt).  A/B knob: fall back to clusters of 4 (33 fit) there.
+    // layer).  Two layers of 8 clusters of 8 do not fit at once, and a cluster of the successor starts, cold, only when
+    // one of the predecessor exits.  A/B knob: fall back to clusters of 4 there.
     static int pair_fit = getenv("SIGE_TC5_PAIR_FIT") ? atoi(getenv("SIGE_TC5_PAIR_FIT")) : 0;
     if (pair_fit && ksplit_req <= 0 && ks == 8 && base > 7) ks = 4;
     pl.ksplit = ks;
     static int deep_env = getenv("SIGE_TC5_DEEP") ? atoi(getenv("SIGE_TC5_DEEP")) : 1;   // A/B knob
-    // (2 = also for un-split launches: with the cp.async gather a single halo buffer costs 0.65 us of exposed gather per chunk,
-    //  while two weight stages — 48 KB in flight — cap the weight ring at ~1.5 us per chunk; an A/B knob, see DESIGN.md)
+    // (2 = also for un-split launches: a single halo buffer exposes the gather of every chunk, two weight stages cap the
+    //  weight ring; an A/B knob)
     pl.deep = (!s2 && pl.bn == 64 && taps == 9 && (ks > 1 || deep_env >= 2)) ? 1 : 0;       // (split launches: always — Cfg::kUnsplit39)
     return pl;
 }
@@ -1038,7 +1115,7 @@ static int launch_v(Params &p, const void *w_packed, const void *w2_packed, cuda
     using C = Cfg<BN, TAPS, DEEP, S2>;
     EncodeTiledFn enc = encode_fn();
     if (!enc) {
-        set_error("sige_tile_conv(tcgen05): cuTensorMapEncodeTiled is not available from the driver");
+        set_error("sige_tile_conv(wgmma): cuTensorMapEncodeTiled is not available from the driver");
         return 2;
     }
     CUtensorMap wmap;
@@ -1051,7 +1128,7 @@ static int launch_v(Params &p, const void *w_packed, const void *w2_packed, cuda
                      gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {
-        set_error("sige_tile_conv(tcgen05): cuTensorMapEncodeTiled failed with %d", (int)r);
+        set_error("sige_tile_conv(wgmma): cuTensorMapEncodeTiled failed with %d", (int)r);
         return 2;
     }
     CUtensorMap wmap2 = wmap;
@@ -1060,7 +1137,7 @@ static int launch_v(Params &p, const void *w_packed, const void *w2_packed, cuda
         r = enc(&wmap2, p.is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void *>(w2_packed), gdim2, gstr, box,
                 estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         if (r != CUDA_SUCCESS) {
-            set_error("sige_tile_conv(tcgen05): cuTensorMapEncodeTiled (shortcut weights) failed with %d", (int)r);
+            set_error("sige_tile_conv(wgmma): cuTensorMapEncodeTiled (shortcut weights) failed with %d", (int)r);
             return 2;
         }
     }
@@ -1071,7 +1148,7 @@ static int launch_v(Params &p, const void *w_packed, const void *w2_packed, cuda
     if (attr_dev != dev) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES);
         if (e != cudaSuccess) {
-            set_error("sige_tile_conv(tcgen05): cannot reserve %d bytes of shared memory: %s", C::SMEM_BYTES, cudaGetErrorString(e));
+            set_error("sige_tile_conv(wgmma): cannot reserve %d bytes of shared memory: %s", C::SMEM_BYTES, cudaGetErrorString(e));
             return 2;
         }
         attr_dev = dev;
@@ -1099,7 +1176,7 @@ static int launch_v(Params &p, const void *w_packed, const void *w2_packed, cuda
     cfg.numAttrs = na;
     cudaError_t e = cudaLaunchKernelEx(&cfg, kern, p, wmap, wmap2);
     if (e != cudaSuccess) {
-        set_error("sige_tile_conv(tcgen05): launch failed (grid %d x %d x %d): %s", cfg.gridDim.x, cfg.gridDim.y, cfg.gridDim.z,
+        set_error("sige_tile_conv(wgmma): launch failed (grid %d x %d x %d): %s", cfg.gridDim.x, cfg.gridDim.y, cfg.gridDim.z,
                   cudaGetErrorString(e));
         (void)cudaGetLastError();
         return 2;
@@ -1131,7 +1208,7 @@ static bool tc5_is_s2(const sige_tile_conv_t *a) {
            a->shift == nullptr && a->act == SIGE_ACT_IDENTITY;
 }
 
-// Can the tcgen05 kernel take this layer?  (3x3 stride 1 on 6x6 tiles, 1x1 on 4x4 tiles, or 3x3 stride 2 on 5x5 tiles; Cout % 64 == 0)
+// Can the wgmma kernel take this layer?  (3x3 stride 1 on 6x6 tiles, 1x1 on 4x4 tiles, or 3x3 stride 2 on 5x5 tiles; Cout % 64 == 0)
 bool tc5_supported(const sige_tile_conv_t *a) {
     const bool g3 = (a->kH == 3 && a->kW == 3 && a->stride == 1 && a->R == 6 && a->S == 6) || tc5_is_s2(a);
     const bool g1 = a->kH == 1 && a->kW == 1 && a->stride == 1 && a->R == 4 && a->S == 4;
@@ -1182,9 +1259,7 @@ int tc5_launch(const sige_tile_conv_t *a, cudaStream_t st) {
     p.pdl = (a->flags & SIGE_CONV_PDL) ? (trig_env ? 2 : 1) : 0;
     p.is_bf16 = a->dtype == SIGE_BF16;
     static int push_env = getenv("SIGE_TC5_PUSH_ASYNC") ? atoi(getenv("SIGE_TC5_PUSH_ASYNC")) : 1;      // A/B knobs
-    static int late_env = getenv("SIGE_TC5_DEALLOC_LATE") ? atoi(getenv("SIGE_TC5_DEALLOC_LATE")) : 0;
     p.push_async = push_env;
-    p.dealloc_late = late_env;
     p.trace = g_trace;
     const bool s2 = tc5_is_s2(a);
     const tc5::Plan pl = tc5::decide(p.NT, p.Cin, p.Cout, p.taps, p.Cin2, a->ksplit, s2);

@@ -1,5 +1,5 @@
 // tile_ops.cu — the five data-movement ops of the SIGE hot path + mask reduction,
-// written for sm_100a.  HBM-bound byte movers: the design rules that matter are
+// written for sm_90a.  HBM-bound byte movers: the design rules that matter are
 // coalescing and 16-byte vector accesses, not tensor cores.
 //
 // Replaces reference sige/cuda/{gather,scatter,scatter_gather}_kernel.cu.  Unlike the

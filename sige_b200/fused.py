@@ -1,4 +1,4 @@
-"""Fused step: an UNMODIFIED model forward, traced once, executed as one fused sm_100a launch per layer.
+"""Fused step: an UNMODIFIED model forward, traced once, executed as one fused sm_90a launch per layer.
 
 ``FusedStep(model, x, *more)`` runs ``model.forward`` once on lazy handles (``sige_b200.lazy``) in sparse
 mode, lowers the recorded tape to a short program of launches and captures it in a CUDA graph.  The model is
@@ -10,7 +10,7 @@ What the lowering recognises (everything else runs as an eager torch node inside
 traceable forward stays correct):
 
   Gather -> SIGEConv2d / nn.Conv2d -> Scatter          one ``sige_tile_conv`` launch: gather (+GroupNorm affine,
-  (reference sige_fused_unet.py:100-131, 212-248)      +SiLU) -> tcgen05 conv -> (+bias, +residual) -> in-place
+  (reference sige_fused_unet.py:100-131, 212-248)      +SiLU) -> wgmma conv -> (+bias, +residual) -> in-place
                                                         scatter into a persistent NHWC buffer initialised from the
                                                         module's cache (the reference's sparse_update form,
                                                         sige/nn/scatter.py:59-60: no clone)

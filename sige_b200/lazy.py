@@ -6,7 +6,7 @@ The reference's model files call ``Gather`` -> ``SIGEConv2d`` -> ``Scatter`` as 
 :185-199, ``norm_out``/``conv_out`` :431-433).  To run such an UNMODIFIED forward as one fused launch per
 layer, the forward is executed once on ``LazyTensor`` handles (SURVEY.md §7.2): every torch function and
 every operator-module call that sees a handle is RECORDED instead of executed, with output shapes
-inferred on the meta device.  ``sige_b200.fused`` then lowers the tape to fused sm_100a launches and
+inferred on the meta device.  ``sige_b200.fused`` then lowers the tape to fused sm_90a launches and
 replays them (CUDA graph); nothing on the tape is ever executed by this module.
 
 A handle is a real ``torch.Tensor`` subclass (wrapper subclass: shape / dtype / device are genuine, there

@@ -5,7 +5,7 @@ Constructor and forward signatures, the attributes model code reads (``block_siz
 ``mode``, ``cache_id``, ``sparse_update``) and the per-mode behaviour follow the reference
 (sige/nn/base.py:80-92, gather.py:12-108, scatter.py:9-136, scatter_gather.py:10-117) so the
 reference's DDPM / Stable-Diffusion / GauGAN model files import and run unmodified.  The sparse
-branches call the sm_100a library through ``sige_b200.ops`` instead of ``sige.cuda``/cuDNN:
+branches call the sm_90a library through ``sige_b200.ops`` instead of ``sige.cuda``/cuDNN:
 
     Gather            -> sige_gather             (NCHW or channels-last, fp32/fp16/bf16)
     SIGEConv2d        -> sige_tile_conv          (tensor cores; channels % 64 == 0, fp16/bf16)

@@ -71,7 +71,7 @@ class SIGEModule(nn.Module):
     # ---- backend lookup (API-compatible; single backend) ----
     def load_runtime(self, function_name: str, runtime_dict: Dict = None) -> Dict:
         """Reference base.py:35-50 probes sige.cpu / sige.cuda / sige.mps.  Here the only runtime is
-        the sm_100a library; the dict keeps the reference's shape ({device: callable})."""
+        the sm_90a library; the dict keeps the reference's shape ({device: callable})."""
         from .. import ops
 
         if runtime_dict is None:
@@ -116,7 +116,7 @@ class SIGEModel(nn.Module):
     (reference base.py:95-129).
 
     Beyond the reference: in ``sparse`` mode on a CUDA fp16/bf16 input the forward is run as a FUSED STEP
-    (``sige_b200.fused``): traced once on lazy handles, lowered to one fused sm_100a launch per wrapped layer,
+    (``sige_b200.fused``): traced once on lazy handles, lowered to one fused sm_90a launch per wrapped layer,
     captured in a CUDA graph and replayed on every later call — the model file itself is unchanged.  The compiled step
     is keyed on (set_masks call, cache generation, cache_id, argument shapes) and rebuilt when any of them changes;
     ``set_fused(False)`` (or SIGE_FUSED=0) keeps the eager operator modules, which is also what a forward that cannot

@@ -48,7 +48,7 @@ def _require_cuda(*ts) -> None:
     for t in ts:
         if t is not None and not t.is_cuda:
             raise RuntimeError(
-                "sige_b200 runs on CUDA (sm_100a) only; got a tensor on '%s'. "
+                "sige_b200 runs on CUDA (sm_90a) only; got a tensor on '%s'. "
                 "There is no CPU/MPS backend and no fallback." % t.device
             )
 

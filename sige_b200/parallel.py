@@ -1,8 +1,8 @@
 """Multi-GPU plumbing: edits are independent, so the only exchange is ONE broadcast of the cached
 original-image state before the step loop (SURVEY.md §8e).  No collective on the per-step path.
 
-The reference has no distributed code at all (SURVEY.md §2.3); this is the green-field B200 part:
-one process per GPU, NCCL over NVLink 5 / NVSwitch through torch.distributed (gloo in CPU tests).
+The reference has no distributed code at all (SURVEY.md §2.3); this is the green-field multi-GPU part:
+one process per GPU, NCCL over NVLink / NVSwitch through torch.distributed (gloo in CPU tests).
 """
 from __future__ import annotations
 

@@ -5,7 +5,7 @@ CUDA events on the launching stream around each launch (L2 flushed before every 
 Algorithmic bytes of one tile-conv launch (SURVEY.md §8d):
     e * [ M*Cin*R*S (tile read) + kH*kW*Cout*Cin (weights) + M*Cout*Ro*So (write) ],  e = 2 (fp16/bf16)
 and its FLOPs 2*M*Ro*So*Cout*Cin*kH*kW.  Peaks come from MEASURED_PEAKS.json (driver-written),
-else the fallback of /opt/skills/guides/B200_PROFILING.md (6650 GB/s, 1590 TFLOP/s).
+else the H100 SXM data sheet (3350 GB/s HBM3, 989 TFLOP/s dense fp16/bf16; not measured).
 """
 from __future__ import annotations
 
@@ -20,38 +20,13 @@ from .nn import SIGEConv2d
 _REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-TRAFFIC_CAPTURE = "r02b_tileconv_dram_traffic_step.csv"      # ncu --metrics dram__bytes_read.sum,dram__bytes_write.sum of `bench.py --ncu`
-
-
 def peaks():
     p = os.path.join(_REPO, "MEASURED_PEAKS.json")
     try:
         d = json.load(open(p))
-        return {"hbm_gbs": float(d["hbm_gbs"]), "bf16_tflops": float(d.get("bf16_tflops", 1590.0)), "source": "measured (MEASURED_PEAKS.json)"}
+        return {"hbm_gbs": float(d["hbm_gbs"]), "bf16_tflops": float(d.get("bf16_tflops", 989.0)), "source": "measured (MEASURED_PEAKS.json)"}
     except Exception:  # noqa: BLE001
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "source": "fallback (B200_PROFILING.md)"}
-
-
-def profiled_traffic():
-    """DRAM traffic of the dominant kernel from the committed ncu capture (profiles/r01j_tileconv_dram_traffic_step.csv:
-    dram__bytes_read.sum + dram__bytes_write.sum of every fused tile-conv launch of one step), as average bytes per
-    launch; None if the capture is absent."""
-    import csv
-
-    path = os.path.join(_REPO, "profiles", TRAFFIC_CAPTURE)
-    try:
-        rows = [r for r in csv.reader(open(path)) if len(r) > 10]
-        hdr = rows[0]
-        vi, ui, mi, ii = hdr.index("Metric Value"), hdr.index("Metric Unit"), hdr.index("Metric Name"), hdr.index("ID")
-        mult = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-        total, ids = 0.0, set()
-        for r in rows[1:]:
-            if r[mi] in ("dram__bytes_read.sum", "dram__bytes_write.sum") and r[ui] in mult:
-                total += float(r[vi].replace(",", "")) * mult[r[ui]]
-                ids.add(r[ii])
-        return total / max(1, len(ids)) if ids else None
-    except Exception:  # noqa: BLE001
-        return None
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "source": "H100 SXM data sheet (not measured)"}
 
 
 def conv_layers_of_step(model, x, t):
@@ -159,7 +134,7 @@ def measure_engine(engine, flush, reps: int = 5):
     slow = sorted(per, key=lambda r: -r[1])[:5]
     return {
         "bound": "hbm", "achieved": achieved, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": achieved / pk["hbm_gbs"],
-        "traffic": profiled_traffic(), "algorithmic_bytes_per_launch": tot_bytes / max(1, len(per)),
+        "traffic": None, "algorithmic_bytes_per_launch": tot_bytes / max(1, len(per)),
         "kernel": "sige::tc5::tile_conv_tc5_kernel / sige::tile_conv_mma_kernel (all %d fused gather-conv-scatter launches of one step)" % len(per),
         "avg_launch_us": 1e3 * tot_ms / max(1, len(per)), "algorithmic_bytes_per_step": tot_bytes, "peak_source": pk["source"],
         "tensor": {"achieved_tflops": tot_flops / (tot_ms * 1e-3) / 1e12, "peak_tflops": pk["bf16_tflops"],
@@ -170,7 +145,7 @@ def measure_engine(engine, flush, reps: int = 5):
 
 
 def measure_in_graph(model, args, options, flush, reps: int = 5):
-    """IN-STEP roofline of the dominant kernel (tc5::tile_conv_tc5_kernel): a second fused step is built whose tcgen05
+    """IN-STEP roofline of the dominant kernel (tc5::tile_conv_tc5_kernel): a second fused step is built whose wgmma
     launches stamp %globaltimer per CTA into a trace buffer (pointer baked into the captured kernel parameters), the
     CUDA graph is replayed after an L2 flush, and per launch  start = the first CTA whose dependency resolved
     (griddepcontrol.wait returned), end = last CTA's exit.
@@ -233,7 +208,7 @@ def measure_in_graph(model, args, options, flush, reps: int = 5):
                 continue
             t = host[offs[i]:offs[i] + ctas[i] * 16].view(ctas[i], 16)
             # slot 3 = this CTA's dependency has resolved (griddepcontrol.wait returned) and its gather loads are issued: the
-            # prologue before it (barrier init, TMEM alloc, weight prefetch) overlaps the PREDECESSOR under PDL and is not
+            # prologue before it (barrier init, weight prefetch) overlaps the PREDECESSOR under PDL and is not
             # charged; slot 11 = CTA exit
             st, en = t[:, 3][t[:, 3] > 0], t[:, 11][t[:, 11] > 0]
             if st.numel() and en.numel():
@@ -246,16 +221,18 @@ def measure_in_graph(model, args, options, flush, reps: int = 5):
         if iv:
             first_last.append((iv[-1][1] - iv[0][0]) / 1e3)
     traced = [i for i in range(len(ctas)) if ctas[i] > 0 and charged[i] > 0]
+    if not traced:
+        raise RuntimeError("in-graph roofline: none of the %d wgmma launches of the step left an entry (slot 3) and exit (slot 11) "
+                           "stamp in the trace buffer" % sum(1 for c in ctas if c > 0))
     tot_us = sum(charged[i] for i in traced)
     tot_bytes = float(sum(step.fused[i].bytes for i in traced))
     tot_flops = float(sum(step.fused[i].flops for i in traced))
     pk = peaks()
-    achieved = tot_bytes / (tot_us * 1e-6) / 1e9 if tot_us else 0.0
-    traffic = profiled_traffic()
+    achieved = tot_bytes / (tot_us * 1e-6) / 1e9
     slow = sorted(traced, key=lambda i: -charged[i])[:5]
     return {
         "bound": "hbm", "achieved": achieved, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": achieved / pk["hbm_gbs"],
-        "traffic": traffic, "traffic_source": ("profiles/%s (ncu capture of `bench.py --ncu`, same kernel build; not measured in this run)" % TRAFFIC_CAPTURE) if traffic else None,
+        "traffic": None,
         "kernel": "sige::tc5::tile_conv_tc5_kernel (%d of the %d fused gather-conv-scatter launches of one step%s)" % (
             len(traced), len(ctas), "" if len(traced) == len(ctas) else "; the rest run on mma.sync"),
         "launches": len(traced), "avg_launch_us": tot_us / max(1, len(traced)), "sum_in_graph_us": tot_us,

@@ -2,7 +2,7 @@
 
 `-m "not gpu"` tests run in the build container (no GPU): oracle vs golden vectors, host logic,
 and that the C-ABI library loads and exports every declared symbol.  `-m gpu` tests are the
-parity tests proper (CUDA path vs oracle / golden) and run on a B200.
+parity tests proper (CUDA path vs oracle / golden) and run on an H100.
 """
 import os
 import sys
@@ -17,7 +17,7 @@ GOLDEN = os.path.join(REPO, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -31,7 +31,7 @@ def pytest_collection_modifyitems(config, items):
         have_gpu = False
     if have_gpu:
         return
-    skip = pytest.mark.skip(reason="needs a CUDA device (B200) — run on the GPU box: pytest -m gpu")
+    skip = pytest.mark.skip(reason="needs a CUDA device (H100): pytest -m gpu")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

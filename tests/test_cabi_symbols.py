@@ -32,7 +32,7 @@ def test_prototype_table_matches_header(cabi_lib):
     assert set(_cabi.PROTOTYPES) == _declared()
     lib = _cabi.lib()
     assert lib.sige_abi_version() == 2
-    assert lib.sige_built_arch() == b"sm_100a"
+    assert lib.sige_built_arch() == b"sm_90a"
     assert lib.sige_activation_from_name(b"identity") == 0
     assert lib.sige_activation_from_name(b"swish") == 1
     assert lib.sige_activation_from_name(b"gelu") == -1     # the reference has UB here (common.cpp:22)
@@ -118,13 +118,13 @@ def _conv_desc(n_tiles, cin, cout, k, *, stride=1, cin2=0, ksplit=0, res=64):
 
 
 def test_tile_conv_launch_plan_heuristics(cabi_lib):
-    """sige_tile_conv_plan: the host-side choice of tile width, split-K (= cluster size) and ring flavour of the tcgen05
-    kernel, on the layer shapes of a DDPM-256 step.  Invariants: one wave only (148 / 148 / 132 / 120 co-resident CTAs
+    """sige_tile_conv_plan: the host-side choice of tile width, split-K (= cluster size) and ring flavour of the wgmma
+    kernel, on the layer shapes of a DDPM-256 step.  Invariants: one wave only (132 / 132 / 120 / 120 co-resident CTAs on an H100
     for cluster sizes 1 / 2 / 4 / 8), every K slice non-empty, deep ring exactly for split narrow 3x3 launches."""
     from sige_b200 import _cabi
 
     lib = _cabi.lib()
-    cap = {1: 148, 2: 148, 4: 132, 8: 120}
+    cap = {1: 132, 2: 132, 4: 120, 8: 120}
 
     def plan(d):
         p = _cabi.TileConvPlan()
@@ -142,7 +142,7 @@ def test_tile_conv_launch_plan_heuristics(cabi_lib):
     assert (p.bn, p.ksplit, p.deep_ring, p.grid_x) == (128, 1, 0, 162)
     p = plan(_conv_desc(16, 512, 1536, 1))                  # qkv of the 16x16 attention block
     assert p.path == 1 and p.bn == 64 and p.ksplit in (1, 2) and p.deep_ring == 0
-    p = plan(_conv_desc(16, 512, 512, 3, stride=2))                    # stride-2 downsample (5x5 -> 2x2 tiles): tcgen05, 32 tiles per CTA
+    p = plan(_conv_desc(16, 512, 512, 3, stride=2))                    # stride-2 downsample (5x5 -> 2x2 tiles): wgmma kernel, 32 tiles per CTA
     assert (p.path, p.bn, p.deep_ring, p.grid_x, p.grid_y) == (1, 64, 0, 1, 8) and p.ksplit == 8
     assert plan(_conv_desc(64, 256, 256, 3, stride=2)).grid_x == 2
     d2 = _conv_desc(16, 256, 256, 3, stride=2)

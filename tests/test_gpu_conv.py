@@ -237,7 +237,7 @@ def test_linearity_and_dense_equals_sparse_at_full_size(oracle):
 
 
 # ---------------------------------------------------------------------------------------------------
-# Blackwell-native kernel (tcgen05.mma + TMEM + TMA weights), flags = SIGE_CONV_TC5
+# Hopper-native kernel (wgmma + TMA weights + cluster split-K), flags = SIGE_CONV_TC5
 # ---------------------------------------------------------------------------------------------------
 TC5 = 2
 TC5_STACK_CASES = [(64, 128, 128, 6, 3), (8, 64, 64, 6, 3), (1, 64, 64, 6, 3), (13, 128, 192, 6, 3), (32, 384, 128, 6, 3), (16, 512, 256, 6, 3),
@@ -386,7 +386,7 @@ def test_tc5_fused_shortcut_matches_block_residual_semantics(oracle):
             e = rel_err(out, want)
             assert e <= 2e-3, "fused shortcut (%s) ksplit %d: rel err %g" % ((Cm, Cx2, Co, H), ks, e)
         d.flags = 0                                   # the mma.sync kernel does not implement it: loud error, not a wrong result
-        with pytest.raises(Exception, match="tcgen05"):
+        with pytest.raises(Exception, match="wgmma"):
             ops.launch_tile_conv(d, torch.cuda.current_stream().cuda_stream)
 
 
@@ -416,10 +416,10 @@ def test_few_channel_stacks_take_the_tensor_cores(oracle, dtype, cl):
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 def test_tc5_stride2_downsample_vs_oracle(oracle, dtype):
-    """The DDPM Downsample (3x3 stride 2 on 5x5 tiles -> 2x2 outputs, reference sige_fused_unet.py:212-221) on the tcgen05 kernel:
+    """The DDPM Downsample (3x3 stride 2 on 5x5 tiles -> 2x2 outputs, reference sige_fused_unet.py:212-221) on the wgmma kernel:
     32 tiles per CTA, halo rows as even / odd planes.  Pure-copy gather (this geometry has no pre-op in the model), ragged image
     edges (odd extents: tiles overhang), more and fewer tiles than one CTA holds, batch 2, a channel-concatenated source, residual,
-    every split-K factor; and the plan really is the tcgen05 path."""
+    every split-K factor; and the plan really is the wgmma path."""
     from ctypes import byref
 
     from sige_b200 import _cabi, ops

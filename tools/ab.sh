@@ -1,5 +1,5 @@
 #!/bin/bash
-# A/B timing of the working tree against a control build, inside ONE gpurun call (box-to-box variation is ~2 %, the
+# A/B timing of the working tree against a control build, inside ONE run on the GPU (box-to-box variation is ~2 %, the
 # effects being chased are 1-5 %).  Control = a copy of a commit with its own library under _base/ (git-ignored):
 #   rm -rf _base && mkdir _base && git archive HEAD | tar -x -C _base && (cd _base && python -m sige_b200.build)
 # Usage on the GPU box:  bash tools/ab.sh [ENV=VALUE ...]     (the variables go to the NEW arm only, e.g. the

@@ -1,7 +1,7 @@
 """Micro-benchmark of the fused tile-conv kernels (development aid, GPU only).
 
 For a few representative DDPM layer shapes: time N back-to-back launches (warm L2) and N launches with an L2
-flush before each (cold), for the mma.sync and the tcgen05 kernel and every split-K factor."""
+flush before each (cold), for the mma.sync and the wgmma kernel and every split-K factor."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -97,7 +97,7 @@ def main():
     for name, n, H, Cin, Cout, k, allt in shapes:
         d = make(n, H, Cin, Cout, k, allt)
         print("== %s" % name)
-        for flags, kn in ((0, "mma.sync"), (2, "tcgen05 "), (1, "mma+pdl "), (3, "tc5+pdl ")):
+        for flags, kn in ((0, "mma.sync"), (2, "wgmma   "), (1, "mma+pdl "), (3, "tc5+pdl ")):
             row = []
             for ks in (1, 2, 4, 8, 0):
                 d.flags, d.ksplit = flags, ks
@@ -123,7 +123,7 @@ if __name__ == "__main__" and "--trace" not in sys.argv:
 
 
 def trace(name, d, ks, flags=2):
-    """Per-stage timeline (globaltimer, ns) of the tcgen05 kernel: median over CTAs, relative to the first CTA's start."""
+    """Per-stage timeline (globaltimer, ns) of the wgmma kernel: median over CTAs, relative to the first CTA's start."""
     import ctypes
     from sige_b200 import _cabi
     lib = _cabi.lib()
@@ -143,7 +143,7 @@ def trace(name, d, ks, flags=2):
     t0 = t[:, 0].min()
     rel = (t - t0).float()
     rel[t == 0] = float("nan")
-    names = ["start", "setup", "idx", "ldg", "store", "mmaA", "mmaEnd", "accRdy", "tmemLd", "clSync", "stored", "end"]
+    names = ["start", "setup", "idx", "ldg", "store", "mmaA", "mmaEnd", "accOut", "rowsIn", "reduce", "stored", "end"]
     med = [float(torch.nanmedian(rel[:, i])) for i in range(12)]
     mx = [float(rel[:, i][~torch.isnan(rel[:, i])].max()) if (~torch.isnan(rel[:, i])).any() else float("nan") for i in range(12)]
     print("  trace %s ks=%d ctas=%d | " % (name, ks, t.shape[0]) + " ".join("%s %.0f/%.0f" % (n, a, b) for n, a, b in zip(names, med, mx)))

@@ -1,4 +1,4 @@
-"""Stride-2 downsample (3x3 s2 on 5x5 tiles): tcgen05 kernel vs mma.sync kernel as a function of the tile count.
+"""Stride-2 downsample (3x3 s2 on 5x5 tiles): wgmma kernel vs mma.sync kernel as a function of the tile count.
 Device time per launch = 20 PDL-chained launches captured in one CUDA graph, replayed 10 times."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,4 +1,4 @@
-"""Selected columns of an ncu report (`ncu -i X.ncu-rep --page raw --csv`) as a small CSV for profiles/.
+"""Selected columns of an ncu report (`ncu -i X.ncu-rep --page raw --csv`) as a small CSV.
     python tools/ncu_summary.py gpurun_out/X.ncu-rep > profiles/rNN_X_summary.csv"""
 import csv
 import subprocess

@@ -1,7 +1,7 @@
-"""profiles/r02_sass_excerpts.txt: per kernel of libsige_b200.so, counts and first occurrences of the tensor-core / TMA /
-TMEM / cluster SASS mnemonics (the proof that the hot kernels are Blackwell-native, B200_PROFILING.md).
+"""Per kernel of libsige_b200.so, counts and first occurrences of the tensor-core / TMA / cluster SASS mnemonics
+(which instructions the hot kernels really use).
 
-    cuobjdump -sass sige_b200/lib/libsige_b200.so > /tmp/sass.txt && python tools/sass_excerpts.py /tmp/sass.txt > profiles/rNN_sass_excerpts.txt
+    cuobjdump -sass sige_b200/lib/libsige_b200.so > sass.txt && python tools/sass_excerpts.py sass.txt
 """
 import collections
 import re
@@ -9,9 +9,9 @@ import sys
 
 txt = open(sys.argv[1]).read()
 funcs = re.split(r"\n\s*Function : ", txt)[1:]
-print("# SASS evidence: cuobjdump -sass sige_b200/lib/libsige_b200.so (sm_100a), per kernel: instruction counts of the")
-print("# tensor-core / TMA / TMEM / cluster mnemonics and the first occurrence of each.\n")
-pat = re.compile(r"\b(UTCHMMA|UTCQMMA|UTCOMMA|UTCMXQMMA|UTCBAR|UTCATOMSWS|LDTM|STTM|UTMALDG|UTMASTG|UTMAPF|UBLKCP|SYNCS|HMMA|IMMA|LDSM|LDGSTS|UCGABAR|ACQBULK|ELECT|CCTL|REDG|STAS|MEMBAR|ERRBAR)(\.[A-Z0-9_.]+)?")
+print("# SASS evidence: cuobjdump -sass sige_b200/lib/libsige_b200.so (sm_90a), per kernel: instruction counts of the")
+print("# tensor-core / TMA / cluster mnemonics and the first occurrence of each.\n")
+pat = re.compile(r"\b(HGMMA|WARPGROUP|UTMALDG|UTMASTG|UTMAPF|UBLKCP|SYNCS|HMMA|IMMA|LDSM|LDGSTS|UCGABAR|ACQBULK|ELECT|CCTL|REDG|STAS|MEMBAR|ERRBAR)(\.[A-Z0-9_.]+)?")
 for f in funcs:
     name = f.split("\n", 1)[0].strip()
     if "sige" not in name:

@@ -1,4 +1,4 @@
-"""In-graph timeline of the fused DDPM step: every tcgen05 fused launch stamps globaltimer into its own trace
+"""In-graph timeline of the fused DDPM step: every wgmma fused launch stamps globaltimer into its own trace
 buffer (pointer captured with the kernel parameters), the CUDA graph is replayed, and the start/end of each kernel
 plus the gaps between consecutive kernels are printed.  Development aid, GPU only."""
 import ctypes, os, sys, warnings
@@ -79,7 +79,7 @@ for st, en, name, n, gd in rows:
     print("%-28s ctas %3d start %8.2f dur %6.2f gap-from-prev-end %6.2f" % (name, n, (st - t0) / 1e3, (en - st) / 1e3, (st - prev_end) / 1e3))
     busy += en - st
     prev_end = max(prev_end, en)
-stage_names = ["start", "setup", "idx", "ldg", "store", "mmaA", "mmaEnd", "accRdy", "tmemLd", "clSync", "stored", "end"]
+stage_names = ["start", "setup", "idx", "ldg", "store", "mmaA", "mmaEnd", "accOut", "rowsIn", "reduce", "stored", "end"]
 print("--- in-graph stage medians (us after the kernel's own first CTA start) for selected layers")
 for i in sorted(names):
     nm = names[i]
