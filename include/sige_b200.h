@@ -268,7 +268,8 @@ typedef struct {
     int path;      /* 1 = wgmma kernel, 0 = mma.sync kernel (the fields below are then 0) */
     int bn;        /* output channels per CTA (64 or 128) */
     int ksplit;    /* K slices = thread-block cluster size (1, 2, 4, 8) */
-    int deep_ring; /* 1 = one halo buffer + five weight stages (split-K launches of the narrow 3x3 configuration) */
+    int deep_ring; /* 1 = the split-K layout of the narrow 3x3 configuration: one halo buffer + five weight stages when every
+                      K slice needs one halo fill, else two halo buffers + two weight stages fed from L2 */
     int grid_x, grid_y, grid_z;
 } sige_tile_conv_plan_t;
 int sige_tile_conv_plan(const sige_tile_conv_t *desc, sige_tile_conv_plan_t *plan);
@@ -343,10 +344,16 @@ int sige_spade_modulate(const void *x, long long x_pixel_stride, const void *gam
 /* In-kernel timeline: while `buf` (device int64, 16 slots per CTA of the NEXT sige_tile_conv launch that takes the wgmma
  * path) is set, that launch stamps %globaltimer per CTA — slot 0 entry, 3 dependency released + loads issued, 4 halo stored,
  * 5/6 MMA issue begin/end, 7 accumulators out of registers, 8/9 every partial row present (split-K: exchange landed),
- * 10 stores of thread 0 issued, 11 exit (every thread's stores issued).  The pointer is baked into the launch's
+ * 10 stores of thread 0 issued, 11 exit (every thread's stores issued); slot 12 holds the number of halo fills of the
+ * CTA's K slice (a count, not a time).  The pointer is baked into the launch's
  * kernel parameters (so it survives CUDA-graph capture); call again (NULL to stop) before the next launch.  bench.py derives
  * the in-step roofline from these stamps; returns 0. */
 int sige_debug_set_trace(void *buf);
+
+/* Halo buffers of split-K narrow 3x3 wgmma launches from now on: 0 = chosen per launch from its K slices (default), 1 = the
+ * single-buffered layout, 2 = the double-buffered one.  Both compute the same sums in the same order, so the outputs are
+ * bitwise equal; for tests.  Returns 0, or non-zero for any other n. */
+int sige_debug_set_split_halo_buffers(int n);
 
 #ifdef __cplusplus
 }

@@ -120,6 +120,7 @@ PROTOTYPES = {
     "sige_sparse_attention": (_I, [POINTER(SparseAttention), _P]),
     "sige_spade_modulate": (_I, [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, c_int64, _I, ctypes.c_float, _I, _P]),
     "sige_debug_set_trace": (_I, [_P]),
+    "sige_debug_set_split_halo_buffers": (_I, [_I]),
 }
 
 _lib = None

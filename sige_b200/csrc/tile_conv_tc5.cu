@@ -104,17 +104,19 @@ struct Params {
     long long *trace;          // development aid: per-CTA clock stamps (16 slots), or nullptr
 };
 
-template <int BN, int TAPS, bool DEEP = false, bool S2 = false> struct Cfg {
+template <int BN, int TAPS, bool DEEP = false, bool S2 = false, bool DB = false> struct Cfg {
     static_assert(!S2 || (BN == 64 && TAPS == 9 && !DEEP), "stride-2 geometry: narrow 3x3 only");
     static constexpr int CT = S2 ? S2_TILES : TILES;           // tiles per CTA
     static constexpr int A_COPY = S2 ? S2_COPY_BYTES : A_COPY_BYTES;
     static constexpr int A_BUF = S2 ? S2_BUF_BYTES : A_BUF_BYTES;
-    // DEEP (split-K launches of the narrow 3x3 configuration: small, latency-bound problems whose K slices rarely span
-    // more than one or two chunks): ONE halo buffer, and the other 72 KB go to the weight ring — 5 stages = 120 KB in
-    // flight, so a slice's weights are on their way before the previous layer has finished, instead of one L2/HBM
-    // round trip per two ring steps.
+    // DEEP (split-K launches of the narrow 3x3 configuration, with the exchange slots) comes in two layouts of the same size:
+    //  * single-buffered (K slices that need one halo fill): ONE halo buffer, and the other 72 KB go to the weight ring —
+    //    5 stages = 120 KB in flight, so a slice's weights are on their way before the previous layer has finished;
+    //  * double-buffered (DB: K slices that span several chunks): two halo buffers, so the gather of chunk c+1 overlaps
+    //    the MMAs of chunk c, and a two-stage ring fed from L2 (the prologue prefetches the whole weight slice into L2).
     static_assert(!DEEP || (BN == 64 && TAPS == 9), "deep ring: narrow 3x3 only");
-    static constexpr int NAB = (DEEP || S2) ? 1 : 2;
+    static_assert(!DB || DEEP, "double-buffered halo: a split-K layout");
+    static constexpr int NAB = ((DEEP && !DB) || S2) ? 1 : 2;
     // one weight-ring stage = TPS taps (a whole kernel row for the narrow 3x3 configuration): fewer barrier round
     // trips for the single MMA-issuing thread
     static constexpr int TPS = (TAPS == 9 && BN == 64) ? 3 : 1;
@@ -125,7 +127,7 @@ template <int BN, int TAPS, bool DEEP = false, bool S2 = false> struct Cfg {
     // ring), so its split-K exchange slots are never used: their 30 KB hold a third weight stage instead (un-split launches are
     // the ones with long K loops per CTA, i.e. weight-ring bound: 72 KB in flight instead of 48).
     static constexpr bool kUnsplit39 = (BN == 64 && TAPS == 9 && !DEEP && !S2);
-    static constexpr int NSTB = S2 ? 3 : DEEP ? 5 : ((BN == 128) ? 4 : (TPS == 3 ? 3 : 4));   // weight ring depth (72 / 120 / 64 / 72 / 32 KB in flight per CTA)
+    static constexpr int NSTB = S2 ? 3 : DEEP ? (DB ? 2 : 5) : ((BN == 128) ? 4 : (TPS == 3 ? 3 : 4));   // weight ring depth (72 / 48 / 120 / 64 / 72 / 32 KB in flight per CTA)
     static constexpr int EPI_PITCH = BN + EPI_PAD;             // floats
     static constexpr int OFF_A = 0;
     static constexpr int OFF_B = NAB * A_BUF;
@@ -213,6 +215,10 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *tma
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];\n" ::"r"(dst),
         "l"(tmap), "r"(x), "r"(y), "r"(bar)
         : "memory");
+}
+// pull one TMA box into L2 without a shared-memory destination or a barrier
+__device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap *tmap, int x, int y) {
+    asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];\n" ::"l"(tmap), "r"(x), "r"(y) : "memory");
 }
 // wgmma shared-memory descriptor, K-major, 128-byte swizzle (given as (lo, hi) words):
 //   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (= 1, unused for swizzled K-major)
@@ -352,12 +358,17 @@ __device__ __forceinline__ long long gtime() {
         if (p.trace) p.trace[((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 16 + (slot)] = gtime(); \
     } while (0)
 
+// K slice of rank kr of a split-K launch: ring steps [k_slice(J, kr, ks), k_slice(J, kr + 1, ks)), an even split (the host
+// picks the halo layout from the same partition, see split_halo_fills)
+__host__ __device__ __forceinline__ int k_slice(int J, int kr, int ks) { return (int)(((long long)J * kr) / ks); }
+
 // ASYNC: the gather is a pure copy (no pre-op: the producer of the source already applied it) and is done with cp.async.
-template <typename T, int BN, int TAPS, bool DEEP, bool ASYNC, bool S2 = false>
+// DB: the double-buffered split-K layout (Cfg).
+template <typename T, int BN, int TAPS, bool DEEP, bool ASYNC, bool S2 = false, bool DB = false>
 __global__ void __launch_bounds__(NTHREADS, 1)
 tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ CUtensorMap wmap,
                      const __grid_constant__ CUtensorMap wmap2) {
-    using C = Cfg<BN, TAPS, DEEP, S2>;
+    using C = Cfg<BN, TAPS, DEEP, S2, DB>;
     static_assert(!S2 || ASYNC, "stride-2 geometry: pure-copy (cp.async) gather only");
     constexpr int NSTB = C::NSTB, TPS = C::TPS, SPC = C::SPC, NAB = C::NAB;
     constexpr int TILES = C::CT;                      // (shadows the namespace constant: 32 for the stride-2 geometry)
@@ -391,10 +402,11 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
     const int NC2 = (TAPS == 9 && !S2) ? p.Cin2 / KC : 0;  // fused 1x1 shortcut: one step (the centre tap) per chunk of ITS input
     const int J = J_main + NC2;
     const int kr = blockIdx.z;
-    const int j_begin = (int)(((long long)J * kr) / p.ksplit), j_end = (int)(((long long)J * (kr + 1)) / p.ksplit);
+    const int j_begin = k_slice(J, kr, p.ksplit), j_end = k_slice(J, kr + 1, p.ksplit);
     // halo-buffer chunks in processing order: main chunks 0..NC-1, then shortcut chunks NC..NC+NC2-1
     auto chunk_of = [&](int j) { return j < J_main ? j / SPC : NC + (j - J_main); };
     const int c_first = chunk_of(j_begin), c_last = chunk_of(j_end - 1);
+    if (tid == 0 && p.trace) p.trace[((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 16 + 12] = c_last - c_first + 1;   // halo fills
     int32_t *s_idx = reinterpret_cast<int32_t *>(smem + C::OFF_CONST);          // [TILES][2] tile origins of this CTA
     unsigned char *s_flags = smem + C::OFF_FLAGS;                               // [TILES] 1 = evaluate the fused shortcut on this tile
     float *s_const = reinterpret_cast<float *>(smem + C::OFF_VEC);              // bias | aux0 scale | aux0 shift | aux1 scale | aux1 shift | bias2
@@ -477,6 +489,19 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
             int s = 0, k = 0;                                          // ring stage and lap
             int c = j_begin < J_main ? j_begin / SPC : 0, st = j_begin < J_main ? j_begin - c * SPC : 0;
             for (int j = j_begin; j < j_end; ++j) {
+                if (DB && j == j_begin + NSTB) {
+                    // the ring is full: pull the rest of the slice into L2 now (this overlaps the previous layer under PDL),
+                    // so that a two-stage ring refills from L2 rather than HBM
+                    for (int jj = j; jj < j_end; ++jj) {
+                        if (jj < J_main) {
+                            const int cj = jj / SPC, row0 = ((jj - cj * SPC) * TPS * NC + cj) * p.Cout + n0;
+#pragma unroll
+                            for (int t = 0; t < TPS; ++t) tma_prefetch_l2_2d(&wmap, 0, row0 + t * NC * p.Cout);
+                        } else {
+                            tma_prefetch_l2_2d(&wmap2, 0, (jj - J_main) * p.Cout + n0);
+                        }
+                    }
+                }
                 mbar_wait(B_EMPTY(s), (k & 1) ^ 1);
                 const uint32_t dst = sbase + C::OFF_B + s * C::B_STAGE_BYTES;
                 if (j < J_main) {
@@ -499,7 +524,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
         // commit group; the weight stage of step j is released once step j+1 has been issued and step j has retired
         // (wait_group 1), so that the tensor core always has the next step queued.  At the end of a chunk everything
         // retires (wait_group 0) before its halo buffer is released: with a single halo buffer the producers cannot
-        // start the next chunk earlier.
+        // start the next chunk earlier; with two they are already filling the other one.
         const int wg = warp >> 2;
         const uint32_t a_lo0 = desc_lo(sbase + C::OFF_A + wg * (64 * 128)), b_lo0 = desc_lo(sbase + C::OFF_B);
         uint32_t accum = 0;
@@ -1110,9 +1135,9 @@ static Plan decide(long long NT, int Cin, int Cout, int taps, int Cin2, int kspl
     return pl;
 }
 
-template <typename T, int BN, int TAPS, bool DEEP, bool ASYNC, bool S2 = false>
+template <typename T, int BN, int TAPS, bool DEEP, bool ASYNC, bool S2 = false, bool DB = false>
 static int launch_v(Params &p, const void *w_packed, const void *w2_packed, cudaStream_t st) {
-    using C = Cfg<BN, TAPS, DEEP, S2>;
+    using C = Cfg<BN, TAPS, DEEP, S2, DB>;
     EncodeTiledFn enc = encode_fn();
     if (!enc) {
         set_error("sige_tile_conv(wgmma): cuTensorMapEncodeTiled is not available from the driver");
@@ -1141,7 +1166,7 @@ static int launch_v(Params &p, const void *w_packed, const void *w2_packed, cuda
             return 2;
         }
     }
-    auto kern = tile_conv_tc5_kernel<T, BN, TAPS, DEEP, ASYNC, S2>;
+    auto kern = tile_conv_tc5_kernel<T, BN, TAPS, DEEP, ASYNC, S2, DB>;
     static int attr_dev = -1;
     int dev = 0;
     cudaGetDevice(&dev);
@@ -1185,19 +1210,38 @@ static int launch_v(Params &p, const void *w_packed, const void *w2_packed, cuda
 }
 
 // pure-copy gathers (no pre-op in the gather stage) take the cp.async variant
-template <typename T, int BN, int TAPS, bool DEEP = false>
+template <typename T, int BN, int TAPS, bool DEEP = false, bool DB = false>
 static int launch(Params &p, const void *w_packed, const void *w2_packed, cudaStream_t st) {
     static int async_env = getenv("SIGE_TC5_ASYNC_GATHER") ? atoi(getenv("SIGE_TC5_ASYNC_GATHER")) : 1;      // A/B knob
     const bool pure_copy = p.scale == nullptr && p.shift == nullptr && p.act == SIGE_ACT_IDENTITY;
-    if (pure_copy && async_env) return launch_v<T, BN, TAPS, DEEP, true>(p, w_packed, w2_packed, st);
-    return launch_v<T, BN, TAPS, DEEP, false>(p, w_packed, w2_packed, st);
+    if (pure_copy && async_env) return launch_v<T, BN, TAPS, DEEP, true, false, DB>(p, w_packed, w2_packed, st);
+    return launch_v<T, BN, TAPS, DEEP, false, false, DB>(p, w_packed, w2_packed, st);
 }
+
+// Halo fills of the longest K slice of a split narrow 3x3 launch (the kernel's partition: k_slice, chunk_of).  One fill: the
+// single-buffered layout (its deep weight ring has the whole slice in flight); more: the double-buffered one.
+static int split_halo_fills(int Cin, int Cin2, int ks) {
+    const int NC = Cin / KC, J_main = NC * 3, J = J_main + Cin2 / KC;
+    auto chunk_of = [&](int j) { return j < J_main ? j / 3 : NC + (j - J_main); };
+    int most = 0;
+    for (int kr = 0; kr < ks; ++kr) {
+        const int b = k_slice(J, kr, ks), e = k_slice(J, kr + 1, ks);
+        if (e > b && chunk_of(e - 1) - chunk_of(b) + 1 > most) most = chunk_of(e - 1) - chunk_of(b) + 1;
+    }
+    return most;
+}
+static int g_split_halo_buffers = 0;     // sige_debug_set_split_halo_buffers
 
 }  // namespace tc5
 
 static long long *g_trace = nullptr;
 extern "C" int sige_debug_set_trace(void *buf) {
     g_trace = reinterpret_cast<long long *>(buf);
+    return 0;
+}
+extern "C" int sige_debug_set_split_halo_buffers(int n) {
+    SIGE_REQUIRE(n >= 0 && n <= 2, "sige_debug_set_split_halo_buffers: n must be 0, 1 or 2 (got %d)", n);
+    tc5::g_split_halo_buffers = n;
     return 0;
 }
 
@@ -1269,9 +1313,12 @@ int tc5_launch(const sige_tile_conv_t *a, cudaStream_t st) {
         return tc5::launch_v<__nv_bfloat16, 64, 9, false, true, true>(p, a->w_packed, a->w2_packed, st);
     }
     const bool wide = pl.bn == 128, three = p.taps == 9;
+    const int nab = tc5::g_split_halo_buffers ? tc5::g_split_halo_buffers : (tc5::split_halo_fills(p.Cin, p.Cin2, p.ksplit) > 1 ? 2 : 1);
+    const bool db = pl.deep && nab == 2;
 #define SIGE_TC5(T)                                                                              \
     (wide ? (three ? tc5::launch<T, 128, 9>(p, a->w_packed, a->w2_packed, st) : tc5::launch<T, 128, 1>(p, a->w_packed, a->w2_packed, st)) \
-          : (three ? (pl.deep ? tc5::launch<T, 64, 9, true>(p, a->w_packed, a->w2_packed, st) : tc5::launch<T, 64, 9>(p, a->w_packed, a->w2_packed, st)) \
+          : (three ? (pl.deep ? (db ? tc5::launch<T, 64, 9, true, true>(p, a->w_packed, a->w2_packed, st) : tc5::launch<T, 64, 9, true>(p, a->w_packed, a->w2_packed, st)) \
+                            : tc5::launch<T, 64, 9>(p, a->w_packed, a->w2_packed, st)) \
                    : tc5::launch<T, 64, 1>(p, a->w_packed, a->w2_packed, st)))
     if (a->dtype == SIGE_F16) return SIGE_TC5(__half);
     return SIGE_TC5(__nv_bfloat16);

@@ -144,14 +144,9 @@ def measure_engine(engine, flush, reps: int = 5):
     }
 
 
-def measure_in_graph(model, args, options, flush, reps: int = 5):
-    """IN-STEP roofline of the dominant kernel (tc5::tile_conv_tc5_kernel): a second fused step is built whose wgmma
-    launches stamp %globaltimer per CTA into a trace buffer (pointer baked into the captured kernel parameters), the
-    CUDA graph is replayed after an L2 flush, and per launch  start = the first CTA whose dependency resolved
-    (griddepcontrol.wait returned), end = last CTA's exit.
-    Programmatic dependent launch lets a layer's prologue overlap its predecessor, so the time CHARGED to launch i is its
-    exclusive part  end_i - max(start_i, end_{i-1})  — the charges add up to the union of the kernel's intervals, which is
-    <= the step time by construction.  achieved = sum(algorithmic bytes of those launches) / sum(charged time)."""
+def _traced_step(model, args, options):
+    """A fused, graph-captured step whose wgmma launches stamp %globaltimer per CTA (16 slots each) into a device buffer:
+    (step, plans, ctas, offs, buf) with offs[i] the first slot of launch i (ctas[i] == 0: not a wgmma launch)."""
     import ctypes
 
     from . import _cabi
@@ -159,26 +154,26 @@ def measure_in_graph(model, args, options, flush, reps: int = 5):
 
     lib = _cabi.lib()
     dev = args[0].device
-    order, sizes = {}, []
+    order = {}
 
-    def plan_ctas(fc):
+    def plan_of(fc):
         pl = _cabi.TileConvPlan()
         lib.sige_tile_conv_plan(ctypes.byref(fc.desc), ctypes.byref(pl))
-        return pl.grid_x * pl.grid_y * pl.grid_z if pl.path == 1 else 0
+        return pl
 
     # pass 1 (no trace): learn the grids, size the trace buffer
     opts = dict(options)
     opts.pop("use_graph", None)
     with torch.no_grad():
         probe = FusedStep(model, *args, use_graph=False, **opts)
-    ctas = [plan_ctas(f) for f in probe.fused]
+    plans = [plan_of(f) for f in probe.fused]
+    ctas = [pl.grid_x * pl.grid_y * pl.grid_z if pl.path == 1 else 0 for pl in plans]
     offs, tot = [], 0
     for c in ctas:
         offs.append(tot)
         tot += c * 16
     del probe
     buf = torch.zeros(max(tot, 16), dtype=torch.int64, device=dev)
-    state = {"i": 0}
 
     def hook(fc):
         i = order.setdefault(id(fc), len(order))
@@ -192,6 +187,19 @@ def measure_in_graph(model, args, options, flush, reps: int = 5):
         FusedConv.trace_hook = None
         lib.sige_debug_set_trace(None)
     assert len(step.fused) == len(ctas)
+    return step, plans, ctas, offs, buf
+
+
+def measure_in_graph(model, args, options, flush, reps: int = 5):
+    """IN-STEP roofline of the dominant kernel (tc5::tile_conv_tc5_kernel): a second fused step is built whose wgmma
+    launches stamp %globaltimer per CTA into a trace buffer (pointer baked into the captured kernel parameters), the
+    CUDA graph is replayed after an L2 flush, and per launch  start = the first CTA whose dependency resolved
+    (griddepcontrol.wait returned), end = last CTA's exit.
+    Programmatic dependent launch lets a layer's prologue overlap its predecessor, so the time CHARGED to launch i is its
+    exclusive part  end_i - max(start_i, end_{i-1})  — the charges add up to the union of the kernel's intervals, which is
+    <= the step time by construction.  achieved = sum(algorithmic bytes of those launches) / sum(charged time)."""
+    dev = args[0].device
+    step, _, ctas, offs, buf = _traced_step(model, args, options)
     charged = [0.0] * len(ctas)
     first_last = []
     for r in range(reps):
@@ -246,3 +254,48 @@ def measure_in_graph(model, args, options, flush, reps: int = 5):
         "method": "in-graph %%globaltimer stamps (first CTA past its dependency .. last CTA exit per launch), L2 flushed before the replay, "
                   "overlap with the predecessor (PDL prologue) charged once; median-free mean of %d replays" % reps,
     }
+
+
+STAGES = (("dep_to_first_halo", 3, 5), ("mainloop", 5, 6), ("exchange", 6, 9), ("epilogue", 9, 11))
+
+
+def stage_breakdown(model, args, options, flush, reps: int = 5):
+    """Where the time of each wgmma launch of the traced step goes, from the per-CTA %globaltimer stamps of the kernel:
+    for every fused launch the median over CTAs and replays (L2 flushed before each) of
+      dep_to_first_halo  slot 3 -> 5   dependency resolved, gather issued -> first halo buffer full
+      mainloop           slot 5 -> 6   first halo full -> last MMA retired
+      exchange           slot 6 -> 9   split-K partial rows pushed and received (un-split: accumulator staging)
+      epilogue           slot 9 -> 11  bias / residual / stores -> CTA exit
+    in microseconds, with the layer name, the launch plan and the halo fills of each K rank (slot 12: the most
+    fills any CTA of that rank consumed; None when the library does not record it)."""
+    step, plans, ctas, offs, buf = _traced_step(model, args, options)
+    dev = args[0].device
+    samples = [{name: [] for name, _, _ in STAGES} for _ in ctas]
+    fills = [None] * len(ctas)
+    for r in range(reps):
+        buf.zero_()
+        if flush is not None:
+            flush.fill_(r)
+        torch.cuda.synchronize(dev)
+        step.replay()
+        torch.cuda.synchronize(dev)
+        host = buf.cpu()
+        for i, n in enumerate(ctas):
+            if n == 0:
+                continue
+            t = host[offs[i]:offs[i] + n * 16].view(n, 16)
+            live = (t[:, 3] > 0) & (t[:, 11] > 0)          # padding CTAs exit before their first stamp
+            for name, a, b in STAGES:
+                samples[i][name] += ((t[live, b] - t[live, a]).double() / 1e3).tolist()
+            f = t[:, 12].view(plans[i].grid_z, -1).max(dim=1).values
+            if int(f.max()) > 0:
+                fills[i] = [int(v) for v in f]
+    out = []
+    for i, f in enumerate(step.fused):
+        if ctas[i] == 0:
+            continue
+        pl = plans[i]
+        med = {name: (float(torch.tensor(v).median()) if v else None) for name, v in samples[i].items()}
+        out.append({"layer": f.name, "tiles": f.tiles, "bn": pl.bn, "ksplit": pl.ksplit, "deep_ring": pl.deep_ring,
+                    "grid": [pl.grid_x, pl.grid_y, pl.grid_z], "halo_fills_per_rank": fills[i], "us": med})
+    return out
