@@ -338,6 +338,43 @@ int sige_spade_modulate(const void *x, long long x_pixel_stride, const void *gam
                         const void *beta, long long beta_pixel_stride, void *out, long long out_pixel_stride,
                         long long pixels, int C, float negative_slope, int dtype, sige_stream_t stream);
 
+/* Separable convolution of GAN Compression's sub-mobile SPADE on the active tiles, one launch per SPADE layer:
+ *   out_b = conv1x1_b( dwconv3x3_b(x) * scale_b + shift_b ),   b < nbranch (gamma and beta read the same input)
+ * — per branch the depthwise SIGEConv2d (groups = Cin), the folded instance norm and the 1x1 SIGEConv2d of reference
+ * gaugan/models/mobile_modules.py:108-112, and the Scatter / ScatterGather behind them (gaugan/models/sige_normalization.py:157-165):
+ * the 4x4 outputs of every 6x6 halo tile are pasted IN PLACE into the branch's destination.  The affine is folded by the caller:
+ * dw_weight = scale * w, dw_bias = scale * b + shift.
+ * Source: a channel window [src_c0, src_c0 + Cin) of an NHWC buffer [B, H, W, src_C] read through `idx` (zero outside the image;
+ * SIGE_TILE_NONE tiles read zeros and write nothing), or of a tile stack [B*N, 6, 6, src_C] (row b*N + i).  Destination: channels
+ * [dst_c0, dst_c0 + Cout) of an NHWC buffer [B, dH, dW, dst_C] at (idx + off), or a stack [B*N, 4, 4, dst_C].
+ * Cin a multiple of 16 in [16, 256], Cout a multiple of 8 in [8, 1024], f16 / bf16 (sige_separable_conv_supported() tells, k = 3);
+ * channel counts and offsets multiples of 8; buffers 16-byte aligned.  flags: SIGE_CONV_PDL. */
+typedef struct {
+    const float *dw_weight; /* fp32 [Cin][3][3], affine folded */
+    const float *dw_bias;   /* fp32 [Cin] or NULL */
+    const void *pw_weight;  /* [Cout][Cin] in dtype */
+    const float *pw_bias;   /* fp32 [Cout] or NULL */
+    void *dst;
+    int dst_is_stack;
+    int dH, dW, dst_C, dst_c0;
+} sige_separable_branch_t;
+typedef struct {
+    int dtype;
+    const void *src;
+    int src_is_stack;
+    int src_C, src_c0;
+    int B, H, W;            /* source extent (NHWC buffer source) */
+    const int32_t *idx;     /* [N,2] halo-tile origins in the source frame */
+    int N;                  /* tiles per image */
+    int Cin, Cout;
+    int offH, offW;         /* output origin = idx + off */
+    int nbranch;            /* 1 or 2 */
+    sige_separable_branch_t branch[2];
+    int flags;
+} sige_separable_conv_t;
+int sige_separable_conv_supported(int Cin, int Cout, int k, int dtype);
+int sige_separable_conv(const sige_separable_conv_t *p, sige_stream_t stream);
+
 /* ------------------------------------------------------------------------- */
 /* diagnostics                                                                */
 /* ------------------------------------------------------------------------- */

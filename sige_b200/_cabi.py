@@ -58,6 +58,17 @@ class SparseAttention(Structure):
                 ("scale", ctypes.c_float), ("dtype", c_int), ("flags", c_int)]
 
 
+class SeparableBranch(Structure):
+    _fields_ = [("dw_weight", c_void_p), ("dw_bias", c_void_p), ("pw_weight", c_void_p), ("pw_bias", c_void_p), ("dst", c_void_p),
+                ("dst_is_stack", c_int), ("dH", c_int), ("dW", c_int), ("dst_C", c_int), ("dst_c0", c_int)]
+
+
+class SeparableConv(Structure):
+    _fields_ = [("dtype", c_int), ("src", c_void_p), ("src_is_stack", c_int), ("src_C", c_int), ("src_c0", c_int),
+                ("B", c_int), ("H", c_int), ("W", c_int), ("idx", c_void_p), ("N", c_int), ("Cin", c_int), ("Cout", c_int),
+                ("offH", c_int), ("offW", c_int), ("nbranch", c_int), ("branch", SeparableBranch * 2), ("flags", c_int)]
+
+
 class TileConv(Structure):
     _fields_ = [
         ("dtype", c_int),
@@ -119,6 +130,8 @@ PROTOTYPES = {
     "sige_sparse_attention_supported": (_I, [_I, _I]),
     "sige_sparse_attention": (_I, [POINTER(SparseAttention), _P]),
     "sige_spade_modulate": (_I, [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, c_int64, _I, ctypes.c_float, _I, _P]),
+    "sige_separable_conv_supported": (_I, [_I, _I, _I, _I]),
+    "sige_separable_conv": (_I, [POINTER(SeparableConv), _P]),
     "sige_debug_set_trace": (_I, [_P]),
     "sige_debug_set_split_halo_buffers": (_I, [_I]),
 }

@@ -259,6 +259,7 @@ class ConvInRec:
 # weakly and re-checked) + its version counter — never by address: the caching allocator hands a freed model's addresses to
 # the next one.
 _PACKED: Dict = {}
+_SEPARABLE: Dict = {}
 
 
 class CudaExecutor:
@@ -458,6 +459,40 @@ class CudaExecutor:
 
         return run
 
+    def separable_supported(self, cin: int, cout: int) -> bool:
+        return self.ops.separable_conv_supported(cin, cout, self.dtype)
+
+    def _separable_weights(self, dw: "DWConv", pw_w: torch.Tensor, pw_b: Optional[torch.Tensor]):
+        """(depthwise weight, bias with the affine folded in fp32; 1x1 weight in the step's dtype; fp32 1x1 bias), cached by the
+        identity (and version) of the parameters and of the tensors the affine was recorded with."""
+        import weakref
+
+        objs = tuple(o for o in (dw.weight, dw.bias, pw_w, pw_b) + tuple(c._base if c._base is not None else c for c in dw.consts) if o is not None)
+        k = (tuple(id(o) for o in objs), self.dtype)
+        hit = _SEPARABLE.get(k)
+        if hit is not None and all(r() is o for r, o in zip(hit[0], objs)) and hit[1] == tuple(o._version for o in objs) and hit[2][2].device == self.device:
+            return hit[2]
+        w, b = self.ops.separable_fold(dw.weight.to(self.device), None if dw.bias is None else dw.bias.to(self.device), dw.scale, dw.shift)
+        packed = (w, b, pw_w.detach().to(self.device, self.dtype).reshape(pw_w.shape[0], -1).contiguous(),
+                  None if pw_b is None else pw_b.detach().to(self.device).float().contiguous())
+        for dead in [kk for kk, vv in _SEPARABLE.items() if any(r() is None for r in vv[0])]:
+            del _SEPARABLE[dead]
+        _SEPARABLE[k] = (tuple(weakref.ref(o) for o in objs), tuple(o._version for o in objs), packed)
+        return packed
+
+    def prepare_separable(self, rec: "SepLaunch") -> Callable[[int], None]:
+        """One sige_separable_conv launch of a SepLaunch record (gamma and beta of one SPADE layer)."""
+        from ._cabi import CONV_PDL
+
+        branches = [self._separable_weights(dw, pw_w, pw_b) + (dst.raw,) for (dw, pw_w, pw_b, dst) in rec.branches]
+        src = rec.src[:, rec.c0:rec.c0 + rec.Cin]
+        ops, idx, off, stack, batch, flags = self.ops, rec.idx, rec.off, rec.src_stack, rec.batch, (CONV_PDL if rec.pdl else 0)
+
+        def run(_stream):
+            ops.separable_conv(src, branches, idx, src_stack=stack, offset=off, batch=batch, flags=flags)
+
+        return run
+
     def sparse_attention_supported(self, head_dim: int) -> bool:
         return self.ops.sparse_attention_supported(head_dim, self.dtype)
 
@@ -616,6 +651,46 @@ class Spade:
         self.stage, self.gamma, self.x, self.beta, self.slope = stage, gamma, x, beta, slope
 
 
+class DWConv:
+    """Depthwise 3x3 SIGEConv2d (groups = Cin = Cout) on 6x6 halo tiles, with the per-channel affine that follows it in GAN
+    Compression's separable conv (the dense pass's instance norm, reference gaugan/models/mobile_modules.py:108-111).  Speculative:
+    only a 1x1 SIGEConv2d consumes it (as `SepOut`); any other consumer gets the recorded calls evaluated.
+    `src` is a RealStack (NHWC tile stack) or a plain lazy Stack of a buffer; `c0` the start of its channel window."""
+
+    def __init__(self, src, c0: int, weight, bias, scale=None, shift=None, consts: Tuple = ()):
+        self.src, self.c0, self.weight, self.bias, self.scale, self.shift, self.consts = src, c0, weight, bias, scale, shift, consts
+
+    @property
+    def C(self) -> int:
+        return int(self.weight.shape[0])
+
+
+class SepOut:
+    """1x1 conv of a DWConv: a separable conv whose launch waits for its Scatter / ScatterGather (like ConvOut)."""
+
+    def __init__(self, dw: DWConv, weight, bias):
+        self.dw, self.weight, self.bias = dw, weight, bias
+
+
+class SepLaunch:
+    """One `sige_separable_conv` launch: up to two branches (gamma and beta of one SPADE layer) on the same source window and
+    tile list.  Branch = (DWConv, 1x1 weight, 1x1 bias, destination Buf)."""
+
+    def __init__(self, name: str, src: torch.Tensor, src_stack: bool, c0: int, idx: torch.Tensor, off: int, batch: int, slot: int):
+        self.name, self.src, self.src_stack, self.c0, self.idx, self.off, self.batch = name, src, src_stack, c0, idx, off, batch
+        self.slot = slot                      # index of the launch in Lowering.steps
+        self.pdl = False
+        self.branches: List[Tuple[DWConv, torch.Tensor, Optional[torch.Tensor], Buf]] = []
+
+    @property
+    def Cin(self) -> int:
+        return self.branches[0][0].C
+
+    @property
+    def Cout(self) -> int:
+        return int(self.branches[0][1].shape[0])
+
+
 _POINTWISE = {"add", "mul", "sub", "div", "rsub", "neg", "leaky_relu", "relu", "silu", "gelu", "sigmoid", "tanh", "clamp", "clamp_min", "abs"}
 _MATERIAL = (Full, Stack, RealStack, ConvOut, RealT)
 _VIEW_OPS = {"reshape", "view", "permute", "transpose", "chunk", "split", "__getitem__", "unsqueeze", "squeeze", "flatten", "unflatten",
@@ -697,6 +772,8 @@ class Lowering:
         self.sparse_attention_calls = 0
         self.spade = os.environ.get("SIGE_SPADE_FUSE", "1") != "0"       # SPADE modulation as one launch (0: recorded torch calls, for A/B)
         self.spade_calls = 0
+        self.separable: List[SepLaunch] = []
+        self._nhwc_stacks: Dict[int, torch.Tensor] = {}
         self.steps: List[Tuple[str, Callable[[int], None]]] = []
         self.fused: List[FusedConv] = []
         self.conv_ins: List[ConvInRec] = []
@@ -1382,6 +1459,8 @@ class Lowering:
         if isinstance(m.padding, str) or m.padding_mode != "zeros":
             return False
         x = node.args[0]
+        if self._separable_conv(node, m, x):
+            return True
         if not isinstance(self.sym(x), (Stack, RealStack)) and x.dim() == 4:      # SIGEConv2d in sparse mode always sees a tile stack
             t = self.runtime_tensor(x)
             if not t.is_contiguous(memory_format=torch.channels_last):
@@ -1390,6 +1469,127 @@ class Lowering:
                 self.eager_nodes.append("to_nhwc")
             self.env[id(x)] = RealStack(t)
         return self._conv_common(node, node.args[0], m.weight, m.bias, m.stride, 0, m.dilation, m.groups)
+
+    # ---- GAN Compression's separable conv: depthwise 3x3 -> per-channel affine -> 1x1, one launch per SPADE layer
+    def _separable_conv(self, node: Node, m, x) -> bool:
+        """Depthwise 3x3 SIGEConv2d on a tile stack (or a channel window of one) -> DWConv; 1x1 SIGEConv2d on a DWConv -> SepOut."""
+        supported = getattr(self.ex, "separable_supported", None)
+        if supported is None or not isinstance(x, LazyTensor) or _pair(m.stride) != (1, 1) or _pair(m.dilation) != (1, 1):
+            return False
+        w, b = m.weight, m.bias
+        cout, cin_g = int(w.shape[0]), int(w.shape[1])
+        v = self.sym(x)
+        if isinstance(v, DWConv):
+            if (tuple(w.shape[2:]) != (1, 1) or m.groups != 1 or cin_g != v.C or self.n_uses(x) != 1
+                    or not supported(v.C, cout)):
+                return False
+            self.env[id(node.outs[0])] = SepOut(v, w, b)
+            return True
+        cin = int(x.shape[1])
+        if tuple(w.shape[2:]) != (3, 3) or m.groups != cin or cout != cin or cin_g != 1 or tuple(x.shape[2:]) != (6, 6) or not supported(cin, cin):
+            return False
+        src = self._separable_source(x)
+        if src is None:
+            return False
+        self.env[id(node.outs[0])] = DWConv(src[0], src[1], w, b)
+        return True
+
+    def _separable_source(self, x: LazyTensor):
+        """(RealStack with an NHWC tensor | plain lazy Stack, channel offset) of a depthwise conv's input: a 6x6 tile stack or a
+        torch.split channel slice of one (SPADE's actv_0 / actv_1 / actv_s, reference
+        gaugan/models/sub_mobile_spade_generators/sige_fused_sub_mobile_spade_generator.py:158-169); None otherwise.  (A
+        SIGEConv2d in sparse mode only ever reads tile stacks, so a 6x6 "image" here is one.)"""
+        v = self.sym(x)
+        if v is None and x.node is not None:
+            self.runtime_tensor(x)               # a stack from a call the lowering does not know (the eager scatter_gather)
+            v = self.sym(x)
+        if isinstance(v, Stack):
+            g = v.gather
+            if (v.src.single is None or v.scale is not None or v.shift is not None or g.activation_name != "identity"
+                    or tuple(g.block_size) != (6, 6) or getattr(g, "tile_images", None) is not None):
+                return None
+            return v, 0
+        c0 = 0
+        if isinstance(v, ChanSlice):             # torch.split of a stack: the whole stack became one NHWC buffer
+            v.buf.readers.append(None)
+            t, c0 = v.buf.raw, v.c0
+        elif isinstance(v, Full) and v.single is not None:
+            v.single.readers.append(None)
+            t = v.single.raw
+        elif isinstance(v, (RealStack, RealT)):
+            t = v.tensor
+        else:
+            return None
+        if t.dim() != 4 or tuple(t.shape[2:]) != (6, 6) or t.shape[1] % 8 or c0 % 8:
+            return None
+        if not t.is_contiguous(memory_format=torch.channels_last):
+            if id(t) not in self._nhwc_stacks:       # one copy per stack, shared by every slice that reads it
+                nhwc = torch.empty(tuple(t.shape), dtype=self.dtype, device=self.dev, memory_format=torch.channels_last)
+                self.steps.append(("eager", lambda _s, src=t, dst=nhwc: dst.copy_(src)))
+                self.eager_nodes.append("to_nhwc")
+                self._nhwc_stacks[id(t)] = nhwc
+            t = self._nhwc_stacks[id(t)]
+        return RealStack(t), c0
+
+    def _sep_affine(self, node: Node, is_mul: bool) -> bool:
+        """`x * scale` / `x + shift` by a constant per-channel [1, C, 1, 1] (or scalar) tensor on a DWConv."""
+        a, b = node.args[0], node.args[1]
+        x, c = (a, b) if isinstance(a, LazyTensor) else (b, a)
+        v = self.sym(x) if isinstance(x, LazyTensor) else None
+        if not isinstance(v, DWConv) or not _is_const(c) or self.n_uses(x) != 1 or tuple(node.outs[0].shape) != tuple(x.shape):
+            return False
+        if not (c.numel() == 1 or (c.dim() == 4 and tuple(c.shape) == (1, v.C, 1, 1))):
+            return False
+        cv = self.vec(c).expand(v.C) if c.numel() == 1 else self.vec(c)
+        if is_mul:
+            scale = cv if v.scale is None else v.scale * cv
+            shift = None if v.shift is None else v.shift * cv
+        else:
+            scale, shift = v.scale, (cv if v.shift is None else v.shift + cv)
+        self.env[id(node.outs[0])] = DWConv(v.src, v.c0, v.weight, v.bias, scale, shift, v.consts + (c,))
+        return True
+
+    def _sep_stack(self, v) -> bool:
+        """Is `v` the lazy re-gather of a buffer a separable launch writes?"""
+        return isinstance(v, Stack) and v.src.single is not None and any(v.src.single is br[3] for r in self.separable for br in r.branches)
+
+    def _sep_fits(self, so: SepOut, g) -> bool:
+        """Can the launch scatter through Gather `g`'s tile set?"""
+        if getattr(g, "tile_images", None) is not None or tuple(g.block_size) != (6, 6) or tuple(g.offset)[0] != tuple(g.offset)[1]:
+            return False
+        src = so.dw.src
+        if isinstance(src, Stack):
+            return self._same_gather(src.gather, g)
+        return int(src.tensor.shape[0]) % max(1, int(g.active_indices.shape[0])) == 0 and int(g.active_indices.shape[0]) > 0
+
+    def _sep_emit(self, node: Node, so: SepOut, dst: Buf, g) -> None:
+        """Add the branch to the previous launch if that one is the other branch of the same SPADE layer (same source window,
+        same tile set, emitted just before), else open a new launch."""
+        dw = so.dw
+        if isinstance(dw.src, Stack):
+            f = dw.src.src
+            src, src_stack, idx = f.single.raw, False, self.slot(g).buf
+            f.single.readers.append((idx, 6, 0, None))
+        else:
+            src, src_stack, idx = dw.src.tensor, True, g.active_indices.to(self.dev)
+        last = self.separable[-1] if self.separable else None
+        if (last is not None and len(last.branches) == 1 and last.slot == len(self.steps) - 1 and last.src is src and last.c0 == dw.c0
+                and last.idx is idx and last.Cin == dw.C and last.Cout == int(so.weight.shape[0]) and last.batch == dst.shape[0]):
+            last.branches.append((dw, so.weight, so.bias, dst))
+            last.name += "+" + self._module_name(node)
+        else:
+            rec = SepLaunch(self._module_name(node), src, src_stack, dw.c0, idx, int(g.offset[0]), dst.shape[0], len(self.steps))
+            rec.pdl = self.pdl
+            rec.branches.append((dw, so.weight, so.bias, dst))
+            self.separable.append(rec)
+            self.steps.append(("separable", None))
+            ex = self.ex
+
+            def prep(rec=rec):
+                self.steps[rec.slot] = ("separable", ex.prepare_separable(rec))
+
+            self._pending_prepare.append(prep)
+        _ = dst.raw               # written in place every step: the buffer must exist (initialised from the module's cache)
 
     # ---- operator modules
     def _h_sige_gather(self, node: Node):
@@ -1423,6 +1623,14 @@ class Lowering:
         x, residual = node.args
         m = node.module
         co = self.sym(x)
+        if isinstance(co, SepOut):         # the shortcut SPADE's gamma / beta: Scatter, then a Gather of its own geometry
+            g = m.gather.module
+            if residual is not None or self.n_uses(x) != 1 or not self._sep_fits(co, g):
+                return False
+            dst = self.cached(m.original_outputs[m.cache_id], g.num_edits)
+            self._sep_emit(node, co, dst, g)
+            self.env[id(node.outs[0])] = Full([(dst, 0)])
+            return True
         if not (isinstance(co, ConvOut) and co.on_tiles):
             return False
         # (a conv output that is ALSO consumed as a stack — SD's transformer scatters proj_in's tiles and keeps them as
@@ -1451,17 +1659,24 @@ class Lowering:
         x, scale, shift = node.args
         m = node.module
         co = self.sym(x)
-        if not (isinstance(co, ConvOut) and co.on_tiles and self.n_uses(x) == 1):
+        sep = isinstance(co, SepOut)
+        if not ((sep or (isinstance(co, ConvOut) and co.on_tiles)) and self.n_uses(x) == 1):
             return False
         if not (scale is None or _is_const(scale)) or not (shift is None or _is_const(shift)):
             return False
         g = m.gather.module
-        if isinstance(co.src, Stack) and not self._same_gather(co.src.gather, g):
+        if sep:
+            if not self._sep_fits(co, g):
+                return False
+        elif isinstance(co.src, Stack) and not self._same_gather(co.src.gather, g):
             return False
-        if isinstance(co.src, RealStack) and (int(co.src.tensor.shape[2]) != int(g.block_size[0]) or g.block_size[0] != g.block_size[1] or g.tile_images is not None):
+        elif isinstance(co.src, RealStack) and (int(co.src.tensor.shape[2]) != int(g.block_size[0]) or g.block_size[0] != g.block_size[1] or g.tile_images is not None):
             return False          # (a materialised stack — GauGAN's SPADE convs read torch math on the tiles — scatters through g's tile set)
         dst = self.cached(m.original_outputs[m.cache_id], g.num_edits)
-        self._tile_emit(node, co, dst, name=self._module_name(node), gather=g)
+        if sep:
+            self._sep_emit(node, co, dst, g)
+        else:
+            self._tile_emit(node, co, dst, name=self._module_name(node), gather=g)
 
         class _G:        # the second gather re-uses the paired gather's geometry with this module's activation
             pass
@@ -1570,6 +1785,8 @@ class Lowering:
     def _h_mul(self, node: Node):
         a, b = node.args[0], node.args[1]
         out = node.outs[0]
+        if len(node.args) == 2 and not node.kwargs and self._sep_affine(node, True):
+            return True
         sa, sb = (self.sym(a) if isinstance(a, LazyTensor) else None), (self.sym(b) if isinstance(b, LazyTensor) else None)
         # x * sigmoid(x)
         for x, s_ in ((a, sb), (b, sa)):
@@ -1610,10 +1827,14 @@ class Lowering:
         a, b = node.args[0], node.args[1]
         if node.kwargs.get("alpha", 1) != 1 or len(node.args) > 2:
             return False
+        if self._sep_affine(node, False):
+            return True
         out = node.outs[0]
         if self.spade:
-            for t_, c_ in ((a, b), (b, a)):        # 1 + gamma on a value that has no symbolic form (a slice of a tile stack)
-                if (isinstance(t_, LazyTensor) and isinstance(c_, (int, float)) and float(c_) == 1.0 and t_.dim() == 4 and self.sym(t_) is None
+            for t_, c_ in ((a, b), (b, a)):        # 1 + gamma on a value that has no symbolic form (a slice of a tile stack), or on the
+                # re-gathered tiles of a separable launch's destination (the sub-mobile SPADE's gamma)
+                if (isinstance(t_, LazyTensor) and isinstance(c_, (int, float)) and float(c_) == 1.0 and t_.dim() == 4
+                        and (self.sym(t_) is None or self._sep_stack(self.sym(t_)))
                         and tuple(t_.shape) == tuple(out.shape) and t_.dtype.is_floating_point):
                     self.env[id(out)] = Spade(1, t_)
                     return True

@@ -617,3 +617,82 @@ def spade_modulate(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, neg
                                                    float(negative_slope), _dt(x), _stream(x)), "sige_spade_modulate")
     _bump()
     return out
+
+
+def separable_conv_supported(cin: int, cout: int, dtype: torch.dtype) -> bool:
+    code = {torch.float16: _cabi.F16, torch.bfloat16: _cabi.BF16}.get(dtype)
+    return code is not None and bool(_cabi.lib().sige_separable_conv_supported(int(cin), int(cout), 3, code))
+
+
+def separable_fold(dw_weight: torch.Tensor, dw_bias: Optional[torch.Tensor], scale: Optional[torch.Tensor], shift: Optional[torch.Tensor]):
+    """fp32 (weight [C, 9], bias [C]) of a depthwise 3x3 conv followed by the per-channel affine x*scale + shift:
+    weight = scale*w, bias = scale*b + shift (reference gaugan/models/mobile_modules.py:110-111)."""
+    c = int(dw_weight.shape[0])
+    w = dw_weight.detach().float().reshape(c, 9)
+    b = torch.zeros(c, dtype=torch.float32, device=w.device) if dw_bias is None else dw_bias.detach().float().reshape(c)
+    if scale is not None:
+        sc = scale.detach().float().reshape(c).to(w.device)
+        w, b = w * sc.view(c, 1), b * sc
+    if shift is not None:
+        b = b + shift.detach().float().reshape(c).to(w.device)
+    return w.contiguous(), b.contiguous()
+
+
+def separable_conv(x: torch.Tensor, branches, idx: Optional[torch.Tensor] = None, *, src_stack: bool = False, dst_stack: bool = False,
+                   offset: int = 1, batch: int = 1, flags: int = 0) -> None:
+    """Separable 3x3 conv of 6x6 halo tiles -> 4x4 outputs, up to two branches on one input, one launch (sige_separable_conv).
+
+    x: channels-innermost 4-D tensor, possibly a channel slice (torch.split) of a wider one: an NHWC buffer [B, Cin, H, W] read
+    through ``idx`` (int32 [N, 2] halo-tile origins), or a tile stack [B*N, Cin, 6, 6] (``src_stack``).  ``branches``: one or two
+    (dw_weight fp32 [Cin, 9], dw_bias fp32 [Cin], pw_weight [Cout, Cin] in x's dtype, pw_bias fp32 [Cout] or None, out) with the
+    affine folded into the depthwise part (``separable_fold``); ``out`` is a channels-innermost NHWC buffer [B, Cout, dH, dW] whose
+    tiles at ``idx + offset`` are overwritten in place, or a stack [B*N, Cout, 4, 4] (``dst_stack``)."""
+    from ._cabi import SeparableConv
+
+    _require_cuda(x, idx)
+    if not 1 <= len(branches) <= 2:
+        raise ValueError("separable_conv: one or two branches")
+    rx = _pixel_rows(x)
+    if rx is None or x.data_ptr() % 16:
+        raise ValueError("separable_conv: x must be a channels-innermost 4-D tensor with uniformly strided pixels, 16-byte aligned")
+    cin = int(x.shape[1])
+    d = SeparableConv()
+    d.dtype = _dt(x)
+    d.src, d.src_is_stack, d.src_C, d.src_c0 = x.data_ptr(), int(src_stack), rx[2], 0
+    if src_stack:
+        if tuple(x.shape[2:]) != (6, 6) or x.shape[0] % batch:
+            raise ValueError("separable_conv: a stack source is [B*N, Cin, 6, 6]")
+        d.B, d.H, d.W, d.N = int(batch), 6, 6, int(x.shape[0]) // batch
+    else:
+        if idx is None:
+            raise ValueError("separable_conv: a buffer source needs the tile list")
+        d.B, d.H, d.W, d.N = int(x.shape[0]), int(x.shape[2]), int(x.shape[3]), int(idx.shape[0])
+    if idx is not None:
+        idx = _idx(idx)
+        if idx.dim() != 2 or idx.shape[1] != 2 or (src_stack and int(idx.shape[0]) != d.N):
+            raise ValueError("separable_conv: idx must be int32 [N, 2] with one row per tile")
+    elif not dst_stack:
+        raise ValueError("separable_conv: a buffer destination needs the tile list")
+    d.idx = None if idx is None else idx.data_ptr()
+    d.Cin, d.offH, d.offW, d.nbranch, d.flags = cin, int(offset), int(offset), len(branches), int(flags)
+    for i, (dw_w, dw_b, pw_w, pw_b, out) in enumerate(branches):
+        pw_w = pw_w.reshape(pw_w.shape[0], -1)
+        cout = int(pw_w.shape[0])
+        if i == 0:
+            d.Cout = cout
+        if (cout != d.Cout or tuple(pw_w.shape) != (cout, cin) or pw_w.dtype != x.dtype or not pw_w.is_contiguous() or dw_w.dtype != torch.float32
+                or tuple(dw_w.shape) != (cin, 9) or not dw_w.is_contiguous() or (dw_b is not None and (dw_b.dtype != torch.float32 or dw_b.numel() != cin))
+                or (pw_b is not None and (pw_b.dtype != torch.float32 or pw_b.numel() != cout))):
+            raise ValueError("separable_conv: branch %d: weights do not match (dw fp32 [Cin, 9], pw [Cout, Cin] in x's dtype, fp32 biases)" % i)
+        ro = _pixel_rows(out)
+        if ro is None or out.dtype != x.dtype or int(out.shape[1]) != cout or (dst_stack and tuple(out.shape) != (d.B * d.N, cout, 4, 4)) \
+                or (not dst_stack and int(out.shape[0]) != d.B):
+            raise ValueError("separable_conv: branch %d: out must be a channels-innermost %s with Cout channels in x's dtype" % (i, "stack [B*N, Cout, 4, 4]" if dst_stack else "buffer [B, Cout, dH, dW]"))
+        _require_cuda(dw_w, dw_b, pw_w, pw_b, out)
+        br = d.branch[i]
+        br.dw_weight, br.dw_bias = dw_w.data_ptr(), None if dw_b is None else dw_b.data_ptr()
+        br.pw_weight, br.pw_bias = pw_w.data_ptr(), None if pw_b is None else pw_b.data_ptr()
+        br.dst, br.dst_is_stack, br.dH, br.dW, br.dst_C, br.dst_c0 = out.data_ptr(), int(dst_stack), int(out.shape[2]), int(out.shape[3]), ro[2], 0
+    with torch.cuda.device(x.device):
+        _cabi.check(_cabi.lib().sige_separable_conv(byref(d), _stream(x)), "sige_separable_conv")
+    _bump()

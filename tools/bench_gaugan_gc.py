@@ -1,0 +1,107 @@
+"""Time the sparse step of GauGAN compressed with GAN Compression (the sub-mobile SPADE generator) on one GPU.
+
+    python tools/bench_gaugan_gc.py [--steps 50] [--warmup 10] [--dtype fp16|bf16] [--size full|mini] [--dump-outputs DIR]
+
+Workload: sige_b200/workloads/gaugan_gc.py at full size — 512 x 1024 label map, config 32_32_32_48_32_24_24_32 (the published
+GAN Compression Cityscapes sub-network), 5 sparse blocks, the 2.98 % label edit of the full-size GauGAN workload; fp32 model and
+dense pass, sparse step as a fused fp16 step (`set_fused(True, dtype=torch.float16)`) in one CUDA graph.  As bench.py: warm-up,
+per-step CUDA events around `model(x)`, an L2 flush (256 MiB write) between steps outside the events, GPU name / power limit /
+SM clock read in the same run, the launch mix of the compiled step, and --dump-outputs DIR (the last timed step's output as
+float32 .npy).  Prints one JSON line.
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+from collections import Counter
+
+REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+if REPO not in sys.path:
+    sys.path.insert(0, REPO)
+
+
+def gpu_info() -> dict:
+    import torch
+
+    info = {"name": torch.cuda.get_device_name(0)}
+    try:
+        r = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        pl, sm, sm_max = (v.strip() for v in r.stdout.strip().split(","))
+        info.update({"power_limit_w": float(pl), "sm_mhz": float(sm), "sm_max_mhz": float(sm_max)})
+    except Exception as e:  # noqa: BLE001
+        info["nvidia_smi"] = "unavailable: %s" % e
+    return info
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
+    ap.add_argument("--steps", type=int, default=50)
+    ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--dtype", choices=["fp16", "bf16"], default="fp16")
+    ap.add_argument("--size", choices=["full", "mini"], default="full")
+    ap.add_argument("--no-flush", action="store_true", help="do not flush L2 between timed steps")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
+    args = ap.parse_args()
+
+    import numpy as np
+    import torch
+
+    if not torch.cuda.is_available():
+        raise SystemExit("bench_gaugan_gc: needs a CUDA device")
+    from sige.utils import dilate_mask, downsample_mask
+    from sige_b200.workloads import gaugan_gc as G
+
+    dev = torch.device("cuda", 0)
+    torch.cuda.set_device(0)
+    dtype = torch.float16 if args.dtype == "fp16" else torch.bfloat16
+    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+    net = G.build_gaugan_gc(args.size).to(dev)
+    t0 = time.time()
+    G.run_gaugan_gc(net, downsample_mask, dilate_mask, device=dev, size=args.size, fused=lambda n: n.set_fused(True, dtype=dtype))
+    compile_s = time.time() - t0
+    step = net.fused_step
+    x = G.gaugan_gc_inputs(args.size)[1].to(dev)
+    flush = None if args.no_flush else torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+
+    def timed(k):
+        evs = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(k)]
+        out = None
+        with torch.no_grad():
+            for i in range(k):
+                if flush is not None:
+                    flush.fill_(i & 0xFF)
+                evs[i][0].record()
+                out = net(x)
+                evs[i][1].record()
+        torch.cuda.synchronize()
+        return [a.elapsed_time(b) for a, b in evs], out
+
+    timed(max(1, args.warmup))
+    info_before = gpu_info()
+    ms, out = timed(max(1, args.steps))
+    info = gpu_info()
+    if args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "out.npy"), out.float().cpu().numpy())
+    kinds = Counter(k for k, _ in step.steps) if step is not None else Counter()
+    low = step.low if step is not None else None
+    line = {
+        "metric": "gaugan-gc %s sparse step" % args.size, "ms_per_step": float(np.median(ms)), "ms_mean": float(np.mean(ms)),
+        "ms_min": float(np.min(ms)), "ms_max": float(np.max(ms)), "steps": len(ms), "warmup": args.warmup,
+        "dtype": args.dtype, "l2": "not flushed" if flush is None else "flushed (256 MiB write) between timed steps",
+        "gpu": info, "sm_mhz_before_timing": info_before.get("sm_mhz"), "compile_seconds": compile_s,
+        "launches": {"tile_conv": len(step.fused) if step else 0, "separable": kinds.get("separable", 0), "spade": kinds.get("spade", 0),
+                     "eager_nodes": len(step.eager_nodes) if step else None},
+        "eager_node_kinds": dict(Counter(step.eager_nodes).most_common(8)) if step else None,
+        "separable_branches": [len(r.branches) for r in getattr(low, "separable", [])] if low is not None else None,
+    }
+    print(json.dumps(line), flush=True)
+
+
+if __name__ == "__main__":
+    main()
