@@ -36,8 +36,10 @@ extern "C" {
 
 typedef enum { SIGE_F32 = 0, SIGE_F16 = 1, SIGE_BF16 = 2 } sige_dtype_t;
 typedef enum { SIGE_NCHW = 0, SIGE_NHWC = 1 } sige_layout_t;
-/* reference sige/common.cpp:11-23 (ActivationType, getActivationType) */
-typedef enum { SIGE_ACT_IDENTITY = 0, SIGE_ACT_SWISH = 1 } sige_act_t;
+/* reference sige/common.cpp:11-23 (ActivationType, getActivationType).  SIGE_ACT_RELU = max(x, 0) is accepted only as the
+ * activation of a sige_tile_conv aux destination (the fused ReLU epilogue); every other activation argument takes
+ * identity / swish. */
+typedef enum { SIGE_ACT_IDENTITY = 0, SIGE_ACT_SWISH = 1, SIGE_ACT_RELU = 2 } sige_act_t;
 
 typedef void *sige_stream_t; /* cudaStream_t */
 
@@ -151,14 +153,16 @@ int sige_scatter_gather(const void *x, const void *y, int dtype, int layout, int
 
 /* Weight repack for the tensor-core path: OIHW (any dtype) -> [kH*kW][Cin/64][Cout][64]
  * in `dst_dtype` (f16/bf16) — the slab of one (tap, 64-channel chunk, Cout block) is contiguous.
- * Run once per weight.  (Cin not a multiple of 64: plain [kH*kW][Cout][Cin].) */
+ * Run once per weight.  (Cin not a multiple of 64: plain [kH*kW][Cout][Cin].  A sige_tile_conv source of such a
+ * width wants the weight zero-padded along Cin to round_up(Cin, 64) first, then packed.) */
 int sige_pack_conv_weight(const void *w_oihw, int src_dtype, int Cout, int Cin, int kH, int kW,
                           void *w_packed, int dst_dtype, sige_stream_t stream);
 
 /* One source segment of the (virtually concatenated) conv input: NHWC. */
 typedef struct {
     const void *ptr; /* [B, H>>up, W>>up, C] */
-    int C;           /* channels in this segment (multiple of 64 on the tensor-core path) */
+    int C;           /* channels in this segment: a multiple of 64 on the tensor-core path, or a multiple of 8 for the
+                        only segment of a launch (mma.sync kernel; no fused shortcut) */
     int up;          /* 0, or 1 = nearest-neighbour x2 upsample applied on read */
 } sige_conv_src_t;
 
@@ -171,12 +175,16 @@ typedef struct {
     int C, c0;          /* writes channels [c0, c0 + Cout) */
     const float *scale; /* fp32 [Cout] or NULL */
     const float *shift; /* fp32 [Cout] or NULL */
-    int act;            /* sige_act_t */
+    int act;            /* sige_act_t; SIGE_ACT_RELU only on a sige_tile_conv aux (dst = NULL, one aux, no affine:
+                           the launch writes relu(conv + bias [+ residual])) */
 } sige_conv_aux_t;
 
 typedef struct {
     int dtype; /* SIGE_F16 / SIGE_BF16 (tensor cores) */
-    /* ---- source: where halo tiles are gathered from ---- */
+    /* ---- source: where halo tiles are gathered from ----
+     * Every segment's C is a multiple of 64, or n_src == 1 and C is a multiple of 8 (a narrow layer: the last K chunk is
+     * partial and runs on the mma.sync kernel; w_packed is then the weight zero-padded to round_up(Cin, 64) input channels;
+     * no fused shortcut). */
     int n_src;              /* 1 or 2 (channel concat of two tensors, torch.cat dim=1) */
     sige_conv_src_t src[2];
     int B, H, W;            /* logical input extent (after optional upsample) */
@@ -190,7 +198,7 @@ typedef struct {
     int affine_bstride;     /* 0 (shared) or Cin (per batch element) */
     int act;                /* sige_act_t */
     /* ---- conv ---- */
-    const void *w_packed;   /* from sige_pack_conv_weight */
+    const void *w_packed;   /* from sige_pack_conv_weight (of the Cin-padded weight on a narrow source) */
     const float *bias;      /* fp32 [Cout] or NULL */
     int Cin, Cout, kH, kW, stride;
     /* ---- destination ---- */

@@ -19,7 +19,7 @@ LIB_PATH = os.path.join(HERE, "lib", "libsige_b200.so")
 
 F32, F16, BF16 = 0, 1, 2
 NCHW, NHWC = 0, 1
-ACT_IDENTITY, ACT_SWISH = 0, 1
+ACT_IDENTITY, ACT_SWISH, ACT_RELU = 0, 1, 2
 CONV_PDL = 1
 CONV_TC5 = 2
 CONV_PADDED = 4

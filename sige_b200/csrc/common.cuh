@@ -86,8 +86,9 @@ template <bool kFast> __device__ __forceinline__ float swish(float z) {
     if (kFast) return __fdividef(z, 1.0f + __expf(-z));
     return z / (1.0f + expf(-z));
 }
+// SIGE_ACT_RELU is accepted only as the activation of a tile-conv aux destination (the fused ReLU epilogue).
 template <bool kFast> __device__ __forceinline__ float activate(int act, float z) {
-    return act == SIGE_ACT_SWISH ? swish<kFast>(z) : z;
+    return act == SIGE_ACT_SWISH ? swish<kFast>(z) : act == SIGE_ACT_RELU ? fmaxf(z, 0.f) : z;
 }
 
 // ----------------------------------------------------------------------------

@@ -512,6 +512,7 @@ int sige_conv_in_nhwc(const void *x, const void *w, const void *bias, void *out,
     InAux ia[2] = {{nullptr, nullptr, nullptr, 0}, {nullptr, nullptr, nullptr, 0}};
     for (int i = 0; i < n_aux; ++i) {
         SIGE_REQUIRE(aux[i].ptr && aux[i].C == Cout && aux[i].c0 == 0 && ((uintptr_t)aux[i].ptr & 15) == 0, "sige_conv_in_nhwc: bad aux destination %d", i);
+        SIGE_REQUIRE(aux[i].act == SIGE_ACT_IDENTITY || aux[i].act == SIGE_ACT_SWISH, "sige_conv_in_nhwc: aux %d unknown activation %d", i, aux[i].act);
         ia[i] = InAux{aux[i].ptr, aux[i].scale, aux[i].shift, aux[i].act};
     }
     switch (dtype) {
@@ -542,6 +543,7 @@ int sige_conv_in_nhwc_tiles(const void *x, const void *w, const void *bias, void
     InAux ia[2] = {{nullptr, nullptr, nullptr, 0}, {nullptr, nullptr, nullptr, 0}};
     for (int i = 0; i < n_aux; ++i) {
         SIGE_REQUIRE(aux[i].ptr && aux[i].C == Cout && aux[i].c0 == 0 && ((uintptr_t)aux[i].ptr & 15) == 0, "sige_conv_in_nhwc_tiles: bad aux destination %d", i);
+        SIGE_REQUIRE(aux[i].act == SIGE_ACT_IDENTITY || aux[i].act == SIGE_ACT_SWISH, "sige_conv_in_nhwc_tiles: aux %d unknown activation %d", i, aux[i].act);
         ia[i] = InAux{aux[i].ptr, aux[i].scale, aux[i].shift, aux[i].act};
     }
     switch (dtype) {

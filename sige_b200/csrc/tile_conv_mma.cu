@@ -14,7 +14,11 @@
 // pointwise pre-op is applied on the way in; out-of-image pixels are zero AFTER the pre-op,
 // reference gather_kernel.cu:33-42) and re-used by all kH*kW taps: the A fragments of tap
 // (ky,kx) are just ldmatrix row pointers into the halo tile shifted by (ky,kx).  Weights are
-// pre-packed [tap][Cin/64][Cout][64] and streamed through a cp.async ring.  The epilogue stages the
+// pre-packed [tap][ceil(Cin/64)][Cout][64] and streamed through a cp.async ring.
+// A single source whose Cin is a multiple of 8 but not of 64 (the narrow layers of pruned /
+// compressed models) ends in a partial chunk: its channels >= Cin are zero in shared memory
+// (never read from global memory), its weights are zero-padded, and only the k16 steps that
+// hold real channels are issued — the skipped ones would add exact zeros.  The epilogue stages the
 // fp32 accumulators in shared memory and writes 16-byte channel vectors straight into the
 // destination tensor (coalesced 128-byte lines per pixel), adding bias and the residual.
 //
@@ -59,7 +63,7 @@ struct ConvParams {
     const float *scale, *shift;
     int affine_bstride;
     int act;
-    const void *w;          // [taps][Cin/64][Cout][64]
+    const void *w;          // [taps][ceil(Cin/64)][Cout][64], zero-padded along Cin
     const float *bias;
     int Cin, Cout, kH, kW, taps, stride;
     int Ro, So, P;          // output tile extent, pixels per tile
@@ -143,7 +147,7 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
     // fixed-capacity tile lists: a CTA whose first tile is SIGE_TILE_NONE padding has nothing to do (see tile_conv_tc5.cu)
     if (p.padded && __ldg(p.idx + 2 * tile0) <= SIGE_TILE_NONE) return;
     const int ntile = min(p.tpc, p.NT - tile0);    // tiles actually present
-    const int NC = p.Cin / KC;                     // K chunks
+    const int NC = (p.Cin + KC - 1) / KC;          // K chunks (the last one partial on a narrow source)
     const int J = NC * p.taps;                     // (chunk, tap) steps of the whole K loop
     // split-K: the cluster's CTAs (rank = blockIdx.z) each take a contiguous slice of the K loop
     const int kr = blockIdx.z;
@@ -188,9 +192,9 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
 #pragma unroll
         for (int k = 0; k < LOADS; ++k) {
             ld_reg[k] = make_uint4(0, 0, 0, 0);
-            if (ld_smem[k] >= 0 && ld_pix[k] >= 0) {
+            const int u = (tid + k * NTHREADS) & 7;
+            if (ld_smem[k] >= 0 && ld_pix[k] >= 0 && cbase + u * 8 < p.Cin) {   // channels >= Cin: zero
                 const int hh = (ld_pix[k] >> 16) >> seg.up, ww = (ld_pix[k] & 0xffff) >> seg.up;
-                const int u = (tid + k * NTHREADS) & 7;
                 const T *src = reinterpret_cast<const T *>(seg.ptr) +
                                (((long long)ld_img[k] * Hs + hh) * Ws + ww) * seg.C + cl + u * 8;
                 ld_reg[k] = __ldg(reinterpret_cast<const uint4 *>(src));
@@ -203,9 +207,8 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
         for (int k = 0; k < LOADS; ++k) {
             if (ld_smem[k] < 0) continue;
             uint4 v = ld_reg[k];
-            if (pre && ld_pix[k] >= 0) {
-                const int u = (tid + k * NTHREADS) & 7;
-                const int ch = c * KC + u * 8;
+            const int ch = c * KC + ((tid + k * NTHREADS) & 7) * 8;
+            if (pre && ld_pix[k] >= 0 && ch < p.Cin) {   // scale / shift hold Cin entries: padding units stay zero
                 T *e = reinterpret_cast<T *>(&v);
                 float sc[8], sh[8];
 #pragma unroll
@@ -236,7 +239,7 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
         if (j < j_end) {
             const int c = j / p.taps, tap = j - c * p.taps;
             unsigned char *st = bst + ((j - j_begin) % NSTAGE) * Cfg::B_STAGE_BYTES;
-            // packed [tap][Cin/64][Cout][64]: this CTA's slab is one contiguous run of BN*128 bytes
+            // packed [tap][ceil(Cin/64)][Cout][64]: this CTA's slab is one contiguous run of BN*128 bytes
             const T *wbase = reinterpret_cast<const T *>(p.w) + (((long long)tap * NC + c) * p.Cout) * KC;
             for (int q = tid; q < BN * 8; q += NTHREADS) {
                 const int n = q >> 3, u = q & 7;
@@ -293,6 +296,7 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
         __syncthreads();
         b_issue(j + NSTAGE - 1);
         const int ky = tap / p.kW, kx = tap - ky * p.kW;
+        const int ksteps = min(KC / 16, (p.Cin - c * KC + 15) / 16);   // k16 steps holding real channels (4 unless partial)
         const uint32_t bbase = smem_u32(bst + ((j - j_begin) % NSTAGE) * Cfg::B_STAGE_BYTES);
         uint32_t a_addr[WM];
         int a_key[WM];
@@ -303,6 +307,7 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
         }
 #pragma unroll
         for (int kk = 0; kk < KC / 16; ++kk) {
+            if (kk >= ksteps) break;
             uint32_t af[WM][4];
 #pragma unroll
             for (int i = 0; i < WM; ++i)
@@ -439,7 +444,7 @@ static int launch_cfg(ConvParams &p, cudaStream_t st) {
                   p.P, Cfg::BM, HALO_PIX);
         return 1;
     }
-    const int J = (p.Cin / KC) * p.taps;
+    const int J = ceil_div(p.Cin, KC) * p.taps;
     const long long base = (long long)ceil_div(p.NT, p.tpc) * ceil_div(p.Cout, Cfg::BN);
     if (p.ksplit <= 0) {
         // auto split-K: aim for ~2 CTAs per SM, keep >= 4 K steps per slice, cluster size <= 8 (portable limit)
@@ -522,14 +527,18 @@ extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) {
     SIGE_REQUIRE(a->R >= a->kH && a->S >= a->kW, "sige_tile_conv: tile smaller than the kernel");
     if (a->N == 0) return 0;
     int csum = 0;
+    bool narrow = false;   // a source whose channel count is a multiple of 8 but not of 64: partial last K chunk
     for (int s = 0; s < a->n_src; ++s) {
         SIGE_REQUIRE(a->src[s].ptr != nullptr, "sige_tile_conv: source %d is null", s);
-        SIGE_REQUIRE(a->src[s].C > 0 && a->src[s].C % KC == 0, "sige_tile_conv: source %d has %d channels; the tensor-core path needs a multiple of %d", s, a->src[s].C, KC);
+        SIGE_REQUIRE(a->src[s].C > 0 && a->src[s].C % 8 == 0, "sige_tile_conv: source %d has %d channels; the tensor-core path needs a multiple of 8", s, a->src[s].C);
+        narrow = narrow || a->src[s].C % KC != 0;
         SIGE_REQUIRE(a->src[s].up == 0 || a->src[s].up == 1, "sige_tile_conv: bad upsample flag");
         SIGE_REQUIRE(((uintptr_t)a->src[s].ptr & 15) == 0, "sige_tile_conv: source %d is not 16-byte aligned", s);
         csum += a->src[s].C;
     }
     SIGE_REQUIRE(csum == a->Cin, "sige_tile_conv: source channels (%d) != Cin (%d)", csum, a->Cin);
+    SIGE_REQUIRE(!narrow || a->n_src == 1, "sige_tile_conv: a source whose channel count is not a multiple of %d cannot be concatenated with another", KC);
+    SIGE_REQUIRE(!narrow || a->n_src2 == 0, "sige_tile_conv: the fused shortcut needs a main source whose channel count is a multiple of %d (got Cin %d)", KC, a->Cin);
     SIGE_REQUIRE(a->Cout > 0 && a->Cout % 8 == 0, "sige_tile_conv: Cout (%d) must be a multiple of 8", a->Cout);
     SIGE_REQUIRE(a->w_packed && (a->dst || a->n_aux > 0), "sige_tile_conv: null weight/destination");
     SIGE_REQUIRE(a->src_is_stack || a->idx, "sige_tile_conv: index list missing");
@@ -555,7 +564,7 @@ extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) {
         const sige_conv_aux_t &x = a->aux[i];
         SIGE_REQUIRE(x.ptr && ((uintptr_t)x.ptr & 15) == 0 && x.C % 8 == 0 && x.c0 % 8 == 0 && x.c0 + a->Cout <= x.C, "sige_tile_conv: bad aux destination %d", i);
         SIGE_REQUIRE((!x.scale || ((uintptr_t)x.scale & 15) == 0) && (!x.shift || ((uintptr_t)x.shift & 15) == 0), "sige_tile_conv: aux %d affine not 16-byte aligned", i);
-        SIGE_REQUIRE(x.act == SIGE_ACT_IDENTITY || x.act == SIGE_ACT_SWISH, "sige_tile_conv: aux %d unknown activation", i);
+        SIGE_REQUIRE(x.act == SIGE_ACT_IDENTITY || x.act == SIGE_ACT_SWISH || x.act == SIGE_ACT_RELU, "sige_tile_conv: aux %d unknown activation", i);
     }
 
     SIGE_REQUIRE(!a->idx_per_image || (!a->src_is_stack && !a->dst_is_stack), "sige_tile_conv: per-image tile lists need full-tensor source and destination");

@@ -121,6 +121,7 @@ class ConvSpec:
         self.dst_stack: Optional[torch.Tensor] = None        # destination is a tile stack (B*N, Cout, Ro, So) NHWC
         self.residual: Optional[torch.Tensor] = None
         self.aux: List[Tuple[torch.Tensor, Optional[torch.Tensor], Optional[torch.Tensor], str]] = []
+        self.epilogue_act = "identity"                       # "relu": the destination holds relu(conv + bias [+ residual])
         self.shortcut = None                                 # (src tensors, weight fp32 OI11, bias fp32, flags uint8 [N] or None)
         self.shortcut_key = None
         self.pdl = False
@@ -149,7 +150,8 @@ class FusedConv:
         self.keep: List = []
 
     def can_aux(self) -> bool:
-        return len(self.spec.aux) < 2
+        # a ReLU epilogue writes its destination through the launch's aux slot, and a view would see the pre-ReLU value
+        return len(self.spec.aux) < 2 and self.spec.epilogue_act == "identity"
 
     def add_aux(self, view: torch.Tensor, scale, shift, act: str) -> None:
         self.spec.aux.append((view, scale, shift, act))
@@ -272,16 +274,19 @@ class CudaExecutor:
 
         self.ops, self.device, self.dtype = ops, device, dtype
 
-    def _pack(self, w: torch.Tensor, key) -> torch.Tensor:
-        """key: None (do not cache) or (parameter object, tag)."""
+    def _pack(self, w: torch.Tensor, key, pad_cin: int = 0) -> torch.Tensor:
+        """key: None (do not cache) or (parameter object, tag).  pad_cin > Cin: zero input channels appended before packing (the
+        layout of a narrow source's launch)."""
         import weakref
 
         if key is not None:
             param, tag = key
-            k = (id(param), tag, self.dtype)
+            k = (id(param), tag, pad_cin, self.dtype)
             hit = _PACKED.get(k)
             if hit is not None and hit[0]() is param and hit[1] == param._version and hit[2].device == param.device:
                 return hit[2]
+        if pad_cin > w.shape[1]:
+            w = F.pad(w, (0, 0, 0, 0, 0, pad_cin - w.shape[1]))
         wp = self.ops.pack_conv_weight(w.contiguous(), self.dtype)
         if key is not None:
             for dead in [kk for kk, vv in _PACKED.items() if vv[0]() is None]:
@@ -327,7 +332,7 @@ class CudaExecutor:
                 b = b.clone()
                 b[:rows] *= f
             key = None
-        wp = self._pack(w, key)
+        wp = self._pack(w, key, pad_cin=(s.Cin + 63) // 64 * 64 if s.Cin % 64 else 0)
         b32 = None if b is None else b.float().contiguous()
         d = ops.tile_conv_descriptor()
         d.dtype = ops._DTYPES[self.dtype]
@@ -376,6 +381,11 @@ class CudaExecutor:
             a.scale = None if sc is None else sc.data_ptr()
             a.shift = None if sh is None else sh.data_ptr()
             a.act = ops._act(act)
+        if s.epilogue_act == "relu":         # the destination becomes the launch's one aux, with no affine
+            assert not s.aux and d.dst
+            a = d.aux[0]
+            a.ptr, a.C, a.c0, a.scale, a.shift, a.act = d.dst, d.dC, d.dst_c0, None, None, ops._cabi.ACT_RELU
+            d.dst, d.n_aux = None, 1
         d.n_src2 = 0
         if s.shortcut is not None:
             sc_tensors, sc_w, sc_b, sc_flags = s.shortcut
@@ -461,6 +471,11 @@ class CudaExecutor:
 
     def separable_supported(self, cin: int, cout: int) -> bool:
         return self.ops.separable_conv_supported(cin, cout, self.dtype)
+
+    def narrow_conv_supported(self, cin: int, cout: int, k: int, stride: int) -> bool:
+        """Can sige_tile_conv run a conv whose single source has `cin` channels, a multiple of 8 but not of 64 (the mma.sync
+        kernel with a partial last K chunk)?"""
+        return self.ops.tile_conv_narrow_supported(cin, cout, k, stride, self.dtype)
 
     def _separable_weights(self, dw: "DWConv", pw_w: torch.Tensor, pw_b: Optional[torch.Tensor]):
         """(depthwise weight, bias with the affine folded in fp32; 1x1 weight in the step's dtype; fp32 1x1 bias), cached by the
@@ -570,8 +585,10 @@ class RealStack:
 class ConvOut:
     """A conv whose launch has not been emitted yet (its consumer decides destination / residual / shortcut)."""
 
-    def __init__(self, node: Node, src, weight, bias, k: int, stride: int, padding: int):
+    def __init__(self, node: Node, src, weight, bias, k: int, stride: int, padding: int, cin_pad: int = 0, act: Optional[str] = None):
         self.node, self.src, self.weight, self.bias, self.k, self.stride, self.padding = node, src, weight, bias, k, stride, padding
+        self.cin_pad = cin_pad          # zero input channels appended to the weight (the source is a zero-padded label map)
+        self.act = act                  # "relu": epilogue activation of the launch
 
     @property
     def on_tiles(self) -> bool:
@@ -774,6 +791,7 @@ class Lowering:
         self.spade_calls = 0
         self.separable: List[SepLaunch] = []
         self._nhwc_stacks: Dict[int, torch.Tensor] = {}
+        self._padded_maps: Dict[int, Full] = {}
         self.steps: List[Tuple[str, Callable[[int], None]]] = []
         self.fused: List[FusedConv] = []
         self.conv_ins: List[ConvInRec] = []
@@ -898,9 +916,11 @@ class Lowering:
     def emit_conv(self, name: str, segs: Sequence[Tuple[Buf, int]], pre: Optional[Pre], hw: Tuple[int, int], idx: torch.Tensor, block: int,
                   weight: torch.Tensor, bias: Optional[torch.Tensor], stride: int, off: int, dst: Optional[Buf], residual: Optional[Buf] = None,
                   shortcut=None, stack_src: Optional[torch.Tensor] = None, dst_stack: Optional[torch.Tensor] = None,
-                  weight_fold: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, tile_img: Optional[torch.Tensor] = None) -> Optional[FusedConv]:
+                  weight_fold: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, tile_img: Optional[torch.Tensor] = None,
+                  cin_pad: int = 0, epilogue: Optional[str] = None) -> Optional[FusedConv]:
         """Each source is (buffer, upsample flag); `pre` spans the concatenated channels.  An affine source is read from the
-        pre-transformed view its producer maintains, else the gather stage applies the pre-op."""
+        pre-transformed view its producer maintains, else the gather stage applies the pre-op.  `cin_pad` zero input channels
+        are appended to the weight; `epilogue` = "relu" writes relu(out) to the destination."""
         if stack_src is not None:            # rows are b*N + i (reference sige/cuda/gather_kernel.cu:30)
             B = dst.shape[0] if (dst is not None and idx is not None) else 1
             n = int(stack_src.shape[0]) // B
@@ -921,7 +941,10 @@ class Lowering:
                 w32 = w32 * f_scale.to(w32.device).view(1, -1, 1, 1)
             key = None                      # folded with per-image statistics: never cached
             self._keepalive.append(weight_fold)
+        if cin_pad:
+            w32 = F.pad(w32, (0, 0, 0, 0, 0, cin_pad))
         s.weight, s.bias, s.weight_key = w32, b32, key
+        s.epilogue_act = epilogue or "identity"
         s.k, s.stride, s.off, s.block = int(weight.shape[2]), stride, off, block
         s.B, s.H, s.W = B, hw[0], hw[1]
         s.idx, s.N, s.tile_img = idx, n, tile_img
@@ -1203,6 +1226,8 @@ class Lowering:
 
         self.steps.append(("eager", run))
         self.eager_nodes.append("gather(n%d)" % lt.node.index)
+        if out.shape[1] != lt.shape[1]:          # a zero-padded label map: the recorded channels only
+            out = out[:, :lt.shape[1]]
         self.env[id(lt)] = RealStack(out)
         return out
 
@@ -1221,7 +1246,8 @@ class Lowering:
         B = 1 if stack_src is not None else segs[0][0].shape[0]
         ro = (block - co.k) // co.stride + 1
         out = torch.empty((B * n, int(co.weight.shape[0]), ro, ro), dtype=self.dtype, device=self.dev, memory_format=torch.channels_last)
-        self.emit_conv("n%d.conv_stack" % co.node.index, segs, pre, hw, idx, block, co.weight, co.bias, co.stride, off, None, stack_src=stack_src, dst_stack=out)
+        self.emit_conv("n%d.conv_stack" % co.node.index, segs, pre, hw, idx, block, co.weight, co.bias, co.stride, off, None, stack_src=stack_src, dst_stack=out,
+                       cin_pad=co.cin_pad, epilogue=co.act)
         self.env[id(lt)] = RealStack(out)
         return out
 
@@ -1405,7 +1431,9 @@ class Lowering:
                 return True
             return False
         if isinstance(v, (Stack, RealStack)):
-            if p != 0 or cin % 64 != 0 or cout % 8 != 0:
+            src_c = v.src.C if isinstance(v, Stack) else int(v.tensor.shape[1])
+            nsegs = len(v.src.segs) if isinstance(v, Stack) else 1
+            if p != 0 or cout % 8 != 0 or not (cin % 64 == 0 or self._narrow(cin, src_c, nsegs, cout, k, s)):
                 return False
             if isinstance(v, Stack) and (v.gather.activation_first and v.gather.activation_name != "identity"):
                 return False
@@ -1414,7 +1442,7 @@ class Lowering:
                 return False
             if block < k or (block - k) % s != 0:
                 return False
-            self.env[id(out)] = ConvOut(node, v, weight, bias, k, s, 0)
+            self.env[id(out)] = ConvOut(node, v, weight, bias, k, s, 0, cin_pad=src_c - cin)
             return True
         if isinstance(v, RealT) and v.tensor.dim() == 4 and cin <= 4 and k == 3 and s == 1 and p == 1 and cout % 8 == 0 and v.tensor.shape[1] == cin:
             t = v.tensor
@@ -1434,7 +1462,9 @@ class Lowering:
             self.env[id(out)] = Full([(dst, 0)])
             return True
         f = self.as_full(x)
-        if f is None or cin % 64 != 0 or cout % 8 != 0 or len(f.segs) > 2 or any(b.shape[1] % 64 for b, _ in f.segs):
+        if f is None or cout % 8 != 0 or len(f.segs) > 2:
+            return False
+        if (cin % 64 != 0 or any(b.shape[1] % 64 for b, _ in f.segs)) and not (f.C == cin and self._narrow(cin, cin, len(f.segs), cout, k, s)):
             return False
         h, w = f.HW
         if h % 4 or w % 4:
@@ -1448,6 +1478,37 @@ class Lowering:
             return False
         self.env[id(out)] = ConvOut(node, f, weight, bias, k, s, p)
         return True
+
+    def _narrow(self, cin: int, src_c: int, nsegs: int, cout: int, k: int, stride: int) -> bool:
+        """A conv whose input width is a multiple of 8 but not of 64 (the narrow layers of pruned / compressed models) is one
+        tile-conv launch on a single source when the executor runs such launches.  src_c > cin: the source is a label map
+        zero-padded to round_up(cin, 8) channels, and the weight is padded to match."""
+        ok = getattr(self.ex, "narrow_conv_supported", None)
+        return (ok is not None and nsegs == 1 and src_c % 8 == 0 and src_c in (cin, (cin + 7) // 8 * 8)
+                and ok(src_c, cout, k, stride))
+
+    @staticmethod
+    def _narrow_dense(v) -> bool:
+        """A dense conv of a narrow input (the dense sub-mobile SPADE's 1x1 gamma conv): SPADE's modulation reads its buffer, as it
+        read the result of the eager conv before such convs were lowered."""
+        return isinstance(v, ConvOut) and not v.on_tiles and int(v.weight.shape[1]) % 64 != 0
+
+    def _padded_map(self, x) -> Optional[Full]:
+        """A map whose channel count is not a multiple of 8 (GauGAN's 36-channel label map), for a Gather when the executor runs
+        narrow tile convs: written once per step into a channels-last buffer of round_up(C, 8) channels in the step's dtype, the
+        channels behind C zero.  That copy is the layout copy the map needs anyway."""
+        if (getattr(self.ex, "narrow_conv_supported", None) is None or not isinstance(x, LazyTensor) or x.dim() != 4 or x.shape[1] % 8 == 0
+                or not x.dtype.is_floating_point):
+            return None
+        if id(x) not in self._padded_maps:
+            src = self.runtime_tensor(x)
+            B, C, H, W = (int(d) for d in src.shape)
+            t = self.empty(B, (C + 7) // 8 * 8, H, W)
+            t.zero_()
+            self.steps.append(("eager", lambda _s, src=src, dst=t[:, :C]: dst.copy_(src)))
+            self.eager_nodes.append("to_nhwc")
+            self._padded_maps[id(x)] = Full([(Buf(self, t.shape, raw=t), 0)])
+        return self._padded_maps[id(x)]
 
     def _h_conv2d(self, node: Node):
         a = self._bind(node, ("input", "weight", "bias", "stride", "padding", "dilation", "groups"),
@@ -1500,16 +1561,23 @@ class Lowering:
         gaugan/models/sub_mobile_spade_generators/sige_fused_sub_mobile_spade_generator.py:158-169); None otherwise.  (A
         SIGEConv2d in sparse mode only ever reads tile stacks, so a 6x6 "image" here is one.)"""
         v = self.sym(x)
+        c0 = 0
+        if v is None and x.node is not None and x.node.name == "split":
+            # torch.split of the lazy re-gather of a buffer a fused launch wrote (actvs after a fused mlp_shared): the window is
+            # read in place through the tile list
+            a = self._bind(x.node, ("tensor", "split_size_or_sections", "dim"), {"dim": 0})
+            st = self.sym(a["tensor"]) if isinstance(a["tensor"], LazyTensor) else None
+            if isinstance(st, Stack) and a["dim"] == 1 and isinstance(a["split_size_or_sections"], int):
+                v, c0 = st, x.slot * a["split_size_or_sections"]
         if v is None and x.node is not None:
             self.runtime_tensor(x)               # a stack from a call the lowering does not know (the eager scatter_gather)
             v = self.sym(x)
         if isinstance(v, Stack):
             g = v.gather
             if (v.src.single is None or v.scale is not None or v.shift is not None or g.activation_name != "identity"
-                    or tuple(g.block_size) != (6, 6) or getattr(g, "tile_images", None) is not None):
+                    or tuple(g.block_size) != (6, 6) or getattr(g, "tile_images", None) is not None or c0 % 8):
                 return None
-            return v, 0
-        c0 = 0
+            return v, c0
         if isinstance(v, ChanSlice):             # torch.split of a stack: the whole stack became one NHWC buffer
             v.buf.readers.append(None)
             t, c0 = v.buf.raw, v.c0
@@ -1598,6 +1666,8 @@ class Lowering:
         if not (scale is None or _is_const(scale)) or not (shift is None or _is_const(shift)):
             return False
         f = self.as_full(x)
+        if f is None and scale is None and shift is None and g.activation_name == "identity":
+            f = self._padded_map(x)
         if f is None or f.pre is not None or f.pad is not None:
             return False
         self.env[id(node.outs[0])] = Stack(f, g, scale, shift)
@@ -1608,7 +1678,7 @@ class Lowering:
         if stack_src is not None and gather is not None:      # a materialised stack scattered through `gather`'s tile set
             idx, off = gather.active_indices.to(self.dev), int(gather.offset[0])
         self.emit_conv(name or ("n%d" % node.index), segs, pre, hw, idx, block, co.weight, co.bias, co.stride, off, dst, residual=residual,
-                       shortcut=shortcut, stack_src=stack_src, tile_img=timg)
+                       shortcut=shortcut, stack_src=stack_src, tile_img=timg, cin_pad=co.cin_pad, epilogue=co.act)
 
     def _module_name(self, node: Node) -> str:
         return self.module_names.get(id(node.module), "n%d" % node.index)
@@ -1642,7 +1712,7 @@ class Lowering:
             return False
         res_buf = None
         if residual is not None:
-            if _is_const(residual):
+            if _is_const(residual) or co.act is not None:      # (the model adds the residual AFTER the activation)
                 return False
             res_buf = self.plain_buf(residual)
             if res_buf is None:
@@ -1692,7 +1762,8 @@ class Lowering:
         x, residual = node.args
         m = node.module
         co, sc = self.sym(x), self.sym(residual)
-        if not (isinstance(co, ConvOut) and isinstance(sc, ConvOut) and co.on_tiles and sc.on_tiles and self.n_uses(x) == 1 and self.n_uses(residual) == 1):
+        if not (isinstance(co, ConvOut) and isinstance(sc, ConvOut) and co.on_tiles and sc.on_tiles and self.n_uses(x) == 1 and self.n_uses(residual) == 1
+                and co.act is None and sc.act is None):
             return False
         # sources: lazy gathers (DDPM) or materialised stacks (GauGAN: SPADE's torch math sits between the Gather and the conv —
         # reference gaugan/models/spade_generators/sige_fused_spade_generator.py:160-198 — such a launch scatters through the
@@ -1731,7 +1802,7 @@ class Lowering:
             and int(sg.block_size[0]) == 4 and int(mg.block_size[0]) == 6
         fuse = (not main_real and not sc_real and self.fuse_shortcut and self.tc5 and self.producer_preop and subset and co.k == 3 and co.stride == 1
                 and all(up == 0 for _, up in sc_full.segs) and len(sc_full.segs) <= 2 and sc_full.plain
-                and int(sc.weight.shape[1]) % 64 == 0)
+                and int(sc.weight.shape[1]) % 64 == 0 and int(co.weight.shape[1]) % 64 == 0)
         name = self._module_name(node)
         if fuse:
             flags = torch.isin(main_key, sc_key).to(torch.uint8).contiguous()
@@ -1834,7 +1905,7 @@ class Lowering:
             for t_, c_ in ((a, b), (b, a)):        # 1 + gamma on a value that has no symbolic form (a slice of a tile stack), or on the
                 # re-gathered tiles of a separable launch's destination (the sub-mobile SPADE's gamma)
                 if (isinstance(t_, LazyTensor) and isinstance(c_, (int, float)) and float(c_) == 1.0 and t_.dim() == 4
-                        and (self.sym(t_) is None or self._sep_stack(self.sym(t_)))
+                        and (self.sym(t_) is None or self._sep_stack(self.sym(t_)) or self._narrow_dense(self.sym(t_)))
                         and tuple(t_.shape) == tuple(out.shape) and t_.dtype.is_floating_point):
                     self.env[id(out)] = Spade(1, t_)
                     return True
@@ -1855,7 +1926,8 @@ class Lowering:
                 res_buf = None
                 if (isinstance(ro, ConvOut) and not ro.on_tiles and ro.k == 1 and self.n_uses(r) == 1 and co.k == 3 and co.stride == 1
                         and self.fuse_shortcut and self.tc5 and self.producer_preop and ro.src.plain and all(up == 0 for _, up in ro.src.segs) and len(ro.src.segs) <= 2
-                        and ro.src.HW == src.HW and int(ro.weight.shape[0]) == int(co.weight.shape[0]) and int(ro.weight.shape[1]) % 64 == 0):
+                        and ro.src.HW == src.HW and int(ro.weight.shape[0]) == int(co.weight.shape[0]) and int(ro.weight.shape[1]) % 64 == 0
+                        and int(co.weight.shape[1]) % 64 == 0):
                     shortcut = ([b_ for b_, _ in ro.src.segs], ro.weight, ro.bias, None)     # dense block: the 1x1 shortcut on every tile
                 else:
                     res_buf = self.plain_buf(r)
@@ -1884,6 +1956,17 @@ class Lowering:
             self.env[id(node.outs[0])] = Spade(3, v.gamma, x=v.x, beta=v.beta, slope=float(a["negative_slope"]))
             return True
         return False
+
+    def _h_relu(self, node: Node):
+        """ReLU of a conv on tiles that nothing else reads (GauGAN's mlp_shared = conv -> nn.ReLU): the launch's epilogue."""
+        a = self._bind(node, ("input", "inplace"), {"inplace": False})
+        x = a["input"]
+        co = self.sym(x) if isinstance(x, LazyTensor) else None
+        if (getattr(self.ex, "narrow_conv_supported", None) is None or a["inplace"] or not isinstance(co, ConvOut) or not co.on_tiles
+                or co.act is not None or self.n_uses(x) != 1):
+            return False
+        self.env[id(node.outs[0])] = ConvOut(co.node, co.src, co.weight, co.bias, co.k, co.stride, co.padding, cin_pad=co.cin_pad, act="relu")
+        return True
 
     def _h_sigmoid(self, node: Node):
         x = node.args[0]

@@ -337,6 +337,13 @@ def tile_conv_tc_supported(x: torch.Tensor, weight: torch.Tensor, stride, dilati
     )
 
 
+def tile_conv_narrow_supported(cin: int, cout: int, k: int, stride: int, dtype: torch.dtype) -> bool:
+    """Does ``sige_tile_conv`` take a single source of `cin` channels, a multiple of 8 but not of 64?  (The mma.sync kernel with a
+    partial last K chunk; the weight is packed zero-padded to round_up(cin, 64) input channels.)"""
+    return dtype in (torch.float16, torch.bfloat16) and cin > 0 and cin % 8 == 0 and cin % 64 != 0 and cout > 0 and cout % 8 == 0 \
+        and k >= 1 and stride >= 1
+
+
 def tile_conv_descriptor() -> TileConv:
     return TileConv()
 
