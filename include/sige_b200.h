@@ -250,6 +250,29 @@ typedef struct {
 /* Fused gather -> (affine+SiLU) -> conv (+bias) -> (+residual) -> scatter, one launch. */
 int sige_tile_conv(const sige_tile_conv_t *p, sige_stream_t stream);
 
+/* SPADE's modulation applied in the gather stage of a tile conv (sige_tile_conv_modulated): for channel c < Cin of an in-image
+ * halo pixel the conv reads
+ *   a = leaky((x*scale[c] + shift[c]) * (1 + gamma[c]) + beta[c], negative_slope)      (fp32, rounded once to the dtype)
+ * — reference gaugan/models/sige_normalization.py:84-86 plus the block's F.leaky_relu(., 0.2) on the three stacks its Gather /
+ * ScatterGather modules cut, without materialising them.  gamma and beta are NHWC [B, H, W, C] at the source's LOGICAL extent
+ * (B, H, W of the descriptor; the source itself may be read through x2 up-sampling), each read from channels
+ * [c0, c0 + Cin) of its C.  Pixels outside the image and SIGE_TILE_NONE tiles read zero; on a narrow source gamma and beta are
+ * never read at or past Cin. */
+typedef struct {
+    const void *gamma;
+    int gamma_C, gamma_c0;
+    const void *beta;
+    int beta_C, beta_c0;
+    float negative_slope;   /* 1 = no activation (the shortcut SPADE) */
+} sige_conv_modulation_t;
+/* Host-only: does sige_tile_conv_modulated take a conv of Cin -> Cout, k x k, this stride, in `dtype`? */
+int sige_tile_conv_modulated_supported(int Cin, int Cout, int k, int stride, int dtype);
+/* sige_tile_conv whose pre-op is followed by the modulation above; always the mma.sync kernel (SIGE_CONV_TC5 is ignored).
+ * Refused before any CUDA call: n_src != 1, a stack source, act != SIGE_ACT_IDENTITY (negative_slope is the activation), a fused
+ * shortcut, idx_per_image, gamma / beta windows that overrun their buffer or are not multiples of 8 elements, pointers that are
+ * not 16-byte aligned, a non-finite slope.  Everything else is sige_tile_conv's contract; N == 0 is a no-op. */
+int sige_tile_conv_modulated(const sige_tile_conv_t *p, const sige_conv_modulation_t *m, sige_stream_t stream);
+
 /* Residual block: conv1 -> conv2 of one block (reference diffusion/models/ddpm_arch/sige_fused_unet.py:100-131: main_gather ->
  * conv1 -> scatter_gather -> conv2 -> scatter[_with_block_residual]) as ONE call.  `conv2` gathers from the buffer `conv1`
  * scatters into (conv1->dst or one of its aux views must be conv2's source); its fused 1x1 shortcut / residual fields carry

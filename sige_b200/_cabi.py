@@ -46,6 +46,11 @@ class ConvAux(Structure):
     _fields_ = [("ptr", c_void_p), ("C", c_int), ("c0", c_int), ("scale", c_void_p), ("shift", c_void_p), ("act", c_int)]
 
 
+class ConvModulation(Structure):
+    _fields_ = [("gamma", c_void_p), ("gamma_C", c_int), ("gamma_c0", c_int), ("beta", c_void_p), ("beta_C", c_int), ("beta_c0", c_int),
+                ("negative_slope", ctypes.c_float)]
+
+
 class TileConvPlan(ctypes.Structure):
     _fields_ = [("path", ctypes.c_int), ("bn", ctypes.c_int), ("ksplit", ctypes.c_int), ("deep_ring", ctypes.c_int),
                 ("grid_x", ctypes.c_int), ("grid_y", ctypes.c_int), ("grid_z", ctypes.c_int)]
@@ -117,6 +122,8 @@ PROTOTYPES = {
     "sige_scatter_gather": (_I, [_P, _P] + [_I] * 10 + [_P, _I, _P, _BP, _BP, _I, _I, _P, _P]),
     "sige_pack_conv_weight": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _P]),
     "sige_tile_conv": (_I, [POINTER(TileConv), _P]),
+    "sige_tile_conv_modulated_supported": (_I, [_I] * 5),
+    "sige_tile_conv_modulated": (_I, [POINTER(TileConv), POINTER(ConvModulation), _P]),
     "sige_resblock": (_I, [POINTER(TileConv), POINTER(TileConv), _P]),
     "sige_tile_conv_generic": (_I, [_P, _P, _P, _P] + [_I] * 14 + [_P]),
     "sige_tile_conv_plan": (_I, [_P, _P]),

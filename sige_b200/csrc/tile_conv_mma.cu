@@ -21,12 +21,16 @@
 // hold real channels are issued — the skipped ones would add exact zeros.  The epilogue stages the
 // fp32 accumulators in shared memory and writes 16-byte channel vectors straight into the
 // destination tensor (coalesced 128-byte lines per pixel), adding bias and the residual.
+// The MOD instantiations (sige_tile_conv_modulated) apply SPADE's modulation in the same register-staged
+// halo path: leaky((x*scale + shift) * (1 + gamma) + beta) with gamma / beta read at the halo pixel, so
+// the modulated tile stack the reference gathers and modulates with pointwise torch calls never exists.
 //
 // Tensor-core instruction: mma.sync.m16n8k16 (HMMA on sm_90a).  The wgmma/TMA variant
 // for large edit ratios lives in tile_conv_tc5.cu (when built); this kernel is the latency-
 // oriented path used when the GEMM M dimension is a few hundred rows.
 #include <cooperative_groups.h>
 
+#include <cmath>
 #include <type_traits>
 
 #include "common.cuh"
@@ -78,6 +82,11 @@ struct ConvParams {
     int rC, res_c0;
     int n_aux;
     AuxDst aux[2];
+    // SPADE modulation in the gather stage (MOD instantiations only): gamma / beta are NHWC [B, H, W, gC / bC] at the logical
+    // source extent, read from channels [g_c0 / b_c0 + c]
+    const void *gamma, *beta;
+    int gC, g_c0, bC, b_c0;
+    float slope;
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) {
@@ -131,7 +140,7 @@ struct ConvCfg {
     static constexpr int LOADS = (HALO_UNITS + NTHREADS - 1) / NTHREADS;
 };
 
-template <typename T, int WM, int WN, int WARPS_M, int WARPS_N, int HALO_PIX, int NSTAGE>
+template <typename T, int WM, int WN, int WARPS_M, int WARPS_N, int HALO_PIX, int NSTAGE, bool MOD>
 __global__ void __launch_bounds__(32 * WARPS_M * WARPS_N)
 tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
     using Cfg = ConvCfg<T, WM, WN, WARPS_M, WARPS_N, HALO_PIX, NSTAGE>;
@@ -201,8 +210,8 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
             }
         }
     };
-    auto halo_store = [&](int c, unsigned char *buf) {   // registers -> pre-op -> shared
-        const bool pre = (p.scale != nullptr) || (p.shift != nullptr) || (p.act != SIGE_ACT_IDENTITY);
+    auto halo_store = [&](int c, unsigned char *buf) {   // registers -> pre-op [-> modulation] -> shared
+        const bool pre = MOD || (p.scale != nullptr) || (p.shift != nullptr) || (p.act != SIGE_ACT_IDENTITY);
 #pragma unroll
         for (int k = 0; k < LOADS; ++k) {
             if (ld_smem[k] < 0) continue;
@@ -223,11 +232,26 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
                     const float4 a = __ldg(s4), b = __ldg(s4 + 1);
                     sh[0] = a.x; sh[1] = a.y; sh[2] = a.z; sh[3] = a.w; sh[4] = b.x; sh[5] = b.y; sh[6] = b.z; sh[7] = b.w;
                 }
+                if constexpr (MOD) {
+                    // leaky((x*scale + shift) * (1 + gamma) + beta) at the same (logical) pixel, rounded once; gamma / beta are
+                    // only read where x is (in the image, channel < Cin)
+                    const long long px = ((long long)ld_img[k] * p.H + (ld_pix[k] >> 16)) * p.W + (ld_pix[k] & 0xffff);
+                    const uint4 gr = __ldg(reinterpret_cast<const uint4 *>(reinterpret_cast<const T *>(p.gamma) + px * p.gC + p.g_c0 + ch));
+                    const uint4 br = __ldg(reinterpret_cast<const uint4 *>(reinterpret_cast<const T *>(p.beta) + px * p.bC + p.b_c0 + ch));
+                    const T *ge = reinterpret_cast<const T *>(&gr), *be = reinterpret_cast<const T *>(&br);
 #pragma unroll
-                for (int z = 0; z < 8; ++z) {
-                    float f = fmaf(DT<T>::to_f(e[z]), sc[z], sh[z]);
-                    f = activate<true>(p.act, f);
-                    e[z] = DT<T>::from_f(f);
+                    for (int z = 0; z < 8; ++z) {
+                        float f = fmaf(DT<T>::to_f(e[z]), sc[z], sh[z]);
+                        f = fmaf(f, 1.f + DT<T>::to_f(ge[z]), DT<T>::to_f(be[z]));
+                        e[z] = DT<T>::from_f(f < 0.f ? f * p.slope : f);
+                    }
+                } else {
+#pragma unroll
+                    for (int z = 0; z < 8; ++z) {
+                        float f = fmaf(DT<T>::to_f(e[z]), sc[z], sh[z]);
+                        f = activate<true>(p.act, f);
+                        e[z] = DT<T>::from_f(f);
+                    }
                 }
             }
             *reinterpret_cast<uint4 *>(buf + ld_smem[k]) = v;
@@ -423,10 +447,10 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
     if (p.ksplit > 1) cg::this_cluster().sync();   // nobody leaves while a peer still reads its partial tile
 }
 
-template <typename T, int WM, int WN, int WARPS_M, int WARPS_N, int HALO_PIX, int NSTAGE>
+template <typename T, int WM, int WN, int WARPS_M, int WARPS_N, int HALO_PIX, int NSTAGE, bool MOD>
 static int launch_cfg(ConvParams &p, cudaStream_t st) {
     using Cfg = ConvCfg<T, WM, WN, WARPS_M, WARPS_N, HALO_PIX, NSTAGE>;
-    auto kern = tile_conv_mma_kernel<T, WM, WN, WARPS_M, WARPS_N, HALO_PIX, NSTAGE>;
+    auto kern = tile_conv_mma_kernel<T, WM, WN, WARPS_M, WARPS_N, HALO_PIX, NSTAGE, MOD>;
     static int attr_dev = -1;   // per instantiation; one process drives one GPU, but stay correct if not
     int dev = 0;
     cudaGetDevice(&dev);
@@ -495,29 +519,26 @@ static inline long long ctas_for(int NT, int P, int RS, int Cout, int BM, int BN
     return (long long)ceil_div(NT, tpc) * ceil_div(Cout, BN);
 }
 
-template <typename T> static int launch_tile_conv(ConvParams &p, cudaStream_t st) {
+template <typename T, bool MOD> static int launch_tile_conv(ConvParams &p, cudaStream_t st) {
     // L: 128x128 CTA tile, 8 warps, 5-stage weight ring; M: 64x64, 4 warps, 8 stages; S: 32x64, 4 warps, 8 stages.
     // Prefer the largest tile that still fills the machine; below that, the smallest tile plus split-K.
     const long long cL = ctas_for(p.NT, p.P, p.RS, p.Cout, 128, 128, 288);
     const long long cM = ctas_for(p.NT, p.P, p.RS, p.Cout, 64, 64, 144);
     const long long cS = ctas_for(p.NT, p.P, p.RS, p.Cout, 32, 64, 72);
     const int sms = sm_count();
-    if (cL >= 2 * sms) return launch_cfg<T, 2, 8, 4, 2, 288, 5>(p, st);
+    if (cL >= 2 * sms) return launch_cfg<T, 2, 8, 4, 2, 288, 5, MOD>(p, st);
     if (cM >= sms || cS < 0) {
-        if (cM > 0) return launch_cfg<T, 2, 4, 2, 2, 144, 8>(p, st);
-        return launch_cfg<T, 2, 8, 4, 2, 288, 5>(p, st);
+        if (cM > 0) return launch_cfg<T, 2, 4, 2, 2, 144, 8, MOD>(p, st);
+        return launch_cfg<T, 2, 8, 4, 2, 288, 5, MOD>(p, st);
     }
-    return launch_cfg<T, 2, 2, 1, 4, 72, 8>(p, st);
+    return launch_cfg<T, 2, 2, 1, 4, 72, 8, MOD>(p, st);
 }
 
 bool tc5_supported(const sige_tile_conv_t *a);
 int tc5_launch(const sige_tile_conv_t *a, cudaStream_t st);
 
-}  // namespace sige
-
-using namespace sige;
-
-extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) {
+// Argument checks and launch of sige_tile_conv; m != nullptr: sige_tile_conv_modulated (whose own refusals come first).
+static int tile_conv(const sige_tile_conv_t *a, const sige_conv_modulation_t *m, sige_stream_t stream) {
     SIGE_REQUIRE(a != nullptr, "sige_tile_conv: null descriptor");
     SIGE_REQUIRE(a->dtype == SIGE_F16 || a->dtype == SIGE_BF16,
                  "sige_tile_conv: tensor-core path needs f16/bf16 (got dtype %d); use sige_tile_conv_generic", a->dtype);
@@ -526,6 +547,15 @@ extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) {
                  "sige_tile_conv: bad geometry");
     SIGE_REQUIRE(a->R >= a->kH && a->S >= a->kW, "sige_tile_conv: tile smaller than the kernel");
     if (a->N == 0) return 0;
+    if (m) {
+        const int cin = a->Cin;
+        SIGE_REQUIRE(m->gamma && m->beta, "sige_tile_conv_modulated: null gamma / beta");
+        SIGE_REQUIRE(((uintptr_t)m->gamma & 15) == 0 && ((uintptr_t)m->beta & 15) == 0, "sige_tile_conv_modulated: gamma / beta not 16-byte aligned");
+        SIGE_REQUIRE(m->gamma_C % 8 == 0 && m->gamma_c0 % 8 == 0 && m->gamma_c0 >= 0 && m->gamma_c0 + cin <= m->gamma_C,
+                     "sige_tile_conv_modulated: gamma channel window [%d, %d) of %d channels (multiples of 8 within the buffer)", m->gamma_c0, m->gamma_c0 + cin, m->gamma_C);
+        SIGE_REQUIRE(m->beta_C % 8 == 0 && m->beta_c0 % 8 == 0 && m->beta_c0 >= 0 && m->beta_c0 + cin <= m->beta_C,
+                     "sige_tile_conv_modulated: beta channel window [%d, %d) of %d channels (multiples of 8 within the buffer)", m->beta_c0, m->beta_c0 + cin, m->beta_C);
+    }
     int csum = 0;
     bool narrow = false;   // a source whose channel count is a multiple of 8 but not of 64: partial last K chunk
     for (int s = 0; s < a->n_src; ++s) {
@@ -581,7 +611,7 @@ extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) {
         SIGE_REQUIRE(a->sc_flags == nullptr || a->residual != nullptr, "sige_tile_conv: sc_flags given without the cached shortcut (residual)");
     }
     // Hopper-native path (wgmma + TMA, tile_conv_tc5.cu) when requested and the geometry fits
-    if ((a->flags & SIGE_CONV_TC5) && tc5_supported(a)) return tc5_launch(a, (cudaStream_t)stream);
+    if (!m && (a->flags & SIGE_CONV_TC5) && tc5_supported(a)) return tc5_launch(a, (cudaStream_t)stream);
 
     ConvParams p;
     p.seg[0] = ConvSeg{a->src[0].ptr, a->src[0].C, a->src[0].up};
@@ -613,8 +643,39 @@ extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) {
     p.tpc = 1;
     p.ksplit = a->ksplit;
     p.pdl = (a->flags & SIGE_CONV_PDL) ? 1 : 0;
-    if (a->dtype == SIGE_F16) return launch_tile_conv<__half>(p, (cudaStream_t)stream);
-    return launch_tile_conv<__nv_bfloat16>(p, (cudaStream_t)stream);
+    p.gamma = p.beta = nullptr;
+    p.gC = p.g_c0 = p.bC = p.b_c0 = 0;
+    p.slope = 1.f;
+    if (m) {
+        p.gamma = m->gamma; p.gC = m->gamma_C; p.g_c0 = m->gamma_c0;
+        p.beta = m->beta; p.bC = m->beta_C; p.b_c0 = m->beta_c0;
+        p.slope = m->negative_slope;
+        if (a->dtype == SIGE_F16) return launch_tile_conv<__half, true>(p, (cudaStream_t)stream);
+        return launch_tile_conv<__nv_bfloat16, true>(p, (cudaStream_t)stream);
+    }
+    if (a->dtype == SIGE_F16) return launch_tile_conv<__half, false>(p, (cudaStream_t)stream);
+    return launch_tile_conv<__nv_bfloat16, false>(p, (cudaStream_t)stream);
+}
+
+}  // namespace sige
+
+using namespace sige;
+
+extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) { return tile_conv(a, nullptr, stream); }
+
+extern "C" int sige_tile_conv_modulated_supported(int Cin, int Cout, int k, int stride, int dtype) {
+    return (dtype == SIGE_F16 || dtype == SIGE_BF16) && Cin > 0 && Cin % 8 == 0 && Cout > 0 && Cout % 8 == 0 && k >= 1 && stride >= 1 ? 1 : 0;
+}
+
+extern "C" int sige_tile_conv_modulated(const sige_tile_conv_t *a, const sige_conv_modulation_t *m, sige_stream_t stream) {
+    SIGE_REQUIRE(a != nullptr && m != nullptr, "sige_tile_conv_modulated: null descriptor");
+    SIGE_REQUIRE(a->n_src == 1, "sige_tile_conv_modulated: one source segment (got n_src %d)", a->n_src);
+    SIGE_REQUIRE(!a->src_is_stack, "sige_tile_conv_modulated: the source must be a full tensor read through the tile list, not a stack");
+    SIGE_REQUIRE(a->act == SIGE_ACT_IDENTITY, "sige_tile_conv_modulated: act must be identity (negative_slope is the activation)");
+    SIGE_REQUIRE(a->n_src2 == 0, "sige_tile_conv_modulated: no fused shortcut");
+    SIGE_REQUIRE(!a->idx_per_image, "sige_tile_conv_modulated: per-image tile lists are not supported");
+    SIGE_REQUIRE(isfinite(m->negative_slope), "sige_tile_conv_modulated: negative_slope must be finite");
+    return tile_conv(a, m, stream);
 }
 
 // conv1 -> conv2 of one residual block as one call (see include/sige_b200.h).

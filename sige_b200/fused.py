@@ -122,6 +122,7 @@ class ConvSpec:
         self.residual: Optional[torch.Tensor] = None
         self.aux: List[Tuple[torch.Tensor, Optional[torch.Tensor], Optional[torch.Tensor], str]] = []
         self.epilogue_act = "identity"                       # "relu": the destination holds relu(conv + bias [+ residual])
+        self.modulation = None                               # (gamma, beta, slope): SPADE's modulation in the gather stage
         self.shortcut = None                                 # (src tensors, weight fp32 OI11, bias fp32, flags uint8 [N] or None)
         self.shortcut_key = None
         self.pdl = False
@@ -184,6 +185,8 @@ class FusedConv:
         if s.shortcut is not None:
             c2 = int(s.shortcut[1].shape[1])
             b += 2 * (n * c2 * 16 + s.Cout * c2)
+        if s.modulation is not None:
+            b += 2 * 2 * n * s.Cin * s.block * s.block
         return b
 
     @property
@@ -387,6 +390,12 @@ class CudaExecutor:
             a.ptr, a.C, a.c0, a.scale, a.shift, a.act = d.dst, d.dC, d.dst_c0, None, None, ops._cabi.ACT_RELU
             d.dst, d.n_aux = None, 1
         d.n_src2 = 0
+        if s.modulation is not None:       # the mma.sync kernel with SPADE's modulation in its gather stage
+            gamma, beta, slope = s.modulation
+            mod = ops.conv_modulation(gamma, beta, slope)
+            fc.desc, fc.keep = d, keep + [idx_t, mod]
+            fc.launch_fn = lambda stream, d=d, mod=mod: ops.launch_tile_conv_modulated(d, mod, stream)
+            return
         if s.shortcut is not None:
             sc_tensors, sc_w, sc_b, sc_flags = s.shortcut
             w2 = self._pack(sc_w, s.shortcut_key)
@@ -477,6 +486,10 @@ class CudaExecutor:
         kernel with a partial last K chunk)?"""
         return self.ops.tile_conv_narrow_supported(cin, cout, k, stride, self.dtype)
 
+    def modulated_conv_supported(self, cin: int, cout: int, k: int, stride: int) -> bool:
+        """Can sige_tile_conv_modulated run a conv whose source is SPADE's modulation of `cin` channels?"""
+        return self.ops.tile_conv_modulated_supported(cin, cout, k, stride, self.dtype)
+
     def _separable_weights(self, dw: "DWConv", pw_w: torch.Tensor, pw_b: Optional[torch.Tensor]):
         """(depthwise weight, bias with the affine folded in fp32; 1x1 weight in the step's dtype; fp32 1x1 bias), cached by the
         identity (and version) of the parameters and of the tensors the affine was recorded with."""
@@ -531,10 +544,11 @@ class CudaExecutor:
 # symbolic values of the lowering
 # =====================================================================================================================
 class Pre:
-    """Pending per-channel pointwise op act(x*scale+shift); scale/shift are fp32 [C] or [B, C] tensors or None."""
+    """Pending per-channel pointwise op act(x*scale+shift); scale/shift are fp32 [C] or [B, C] tensors or None.  `mod` = (gamma Buf,
+    beta Buf, slope): SPADE's modulation leaky((x*scale+shift) * (1 + gamma) + beta) after it (a ModStack's gather stage)."""
 
-    def __init__(self, scale=None, shift=None, act: Optional[str] = None):
-        self.scale, self.shift, self.act = scale, shift, act
+    def __init__(self, scale=None, shift=None, act: Optional[str] = None, mod=None):
+        self.scale, self.shift, self.act, self.mod = scale, shift, act, mod
 
     def copy(self) -> "Pre":
         return Pre(self.scale, self.shift, self.act)
@@ -573,6 +587,16 @@ class Stack:
 
     def __init__(self, src: Full, gather, scale, shift):
         self.src, self.gather, self.scale, self.shift = src, gather, scale, shift
+
+
+class ModStack(Stack):
+    """SPADE's modulation of three lazy Stacks cut with one tile list: the tiles of `src` (with the Gather's scale / shift) times
+    (1 + the same tiles of `gamma`) plus those of `beta`, then leaky_relu(slope).  Only ever the source of a ConvOut: the conv's
+    launch applies it in its gather stage (sige_tile_conv_modulated), so none of the stacks is materialised."""
+
+    def __init__(self, x: Stack, gamma: "Buf", beta: "Buf", slope: float):
+        super().__init__(x.src, x.gather, x.scale, x.shift)
+        self.gamma, self.beta, self.slope = gamma, beta, slope
 
 
 class RealStack:
@@ -957,7 +981,16 @@ class Lowering:
         else:
             tensors: List[torch.Tensor] = []
             gather_side = False
-            if pre is not None and (pre.scale is not None or pre.shift is not None or pre.act):
+            if pre is not None and pre.mod is not None:        # modulated gather: raw x, its affine applied before the modulation
+                tensors = [b_.raw for (b_, _) in segs]
+                s.scale = None if pre.scale is None else pre.scale.contiguous()
+                s.shift = None if pre.shift is None else pre.shift.contiguous()
+                s.per_sample_affine = self._per_sample(pre)
+                gamma, beta, slope = pre.mod
+                for b_ in (gamma, beta):
+                    b_.readers.append((idx, block, 0, tile_img))
+                s.modulation = (gamma.raw, beta.raw, slope)
+            elif pre is not None and (pre.scale is not None or pre.shift is not None or pre.act):
                 per_sample = (pre.scale is not None and pre.scale.dim() == 2) or (pre.shift is not None and pre.shift.dim() == 2)
                 views, c0 = [], 0
                 if not per_sample:
@@ -1085,6 +1118,9 @@ class Lowering:
         pre = None
         if st.scale is not None or st.shift is not None or g.activation_name != "identity":
             pre = Pre(self._chan_vec(st.scale, st.src), self._chan_vec(st.shift, st.src), None if g.activation_name == "identity" else g.activation_name)
+        if isinstance(st, ModStack):
+            pre = pre or Pre()
+            pre.mod = (st.gamma, st.beta, st.slope)
         timg = getattr(g, "tile_images", None)
         if timg is None and int(g.active_indices.shape[0]) > 0 and not exact:
             idx = self.slot(g).buf            # fixed capacity, padded with SIGE_TILE_NONE (see IdxSlot)
@@ -1404,7 +1440,8 @@ class Lowering:
         return vals
 
     # ---- convolutions
-    def _conv_common(self, node: Node, x, weight, bias, stride, padding, dilation, groups) -> bool:
+    def _conv_common(self, node: Node, x, weight, bias, stride, padding, dilation, groups, src: Optional[Stack] = None) -> bool:
+        """`src`: the conv's source when it is not x's symbolic value (a ModStack)."""
         if not (_is_const(weight) and (bias is None or _is_const(bias))) or weight.dim() != 4:
             return False
         k, s, p = _pair(weight.shape[2:]), _pair(stride), (_pair(padding) if not isinstance(padding, str) else None)
@@ -1413,7 +1450,7 @@ class Lowering:
         k, s, p = k[0], s[0], p[0]
         cout, cin = int(weight.shape[0]), int(weight.shape[1])
         out = node.outs[0]
-        v = self.sym(x)
+        v = self.sym(x) if src is None else src
         if isinstance(v, GNVal):
             if k == 3 and s == 1 and p == 1 and cout <= 8 and cin % 16 == 0 and v.act in (None, "swish") and self.ex.tail_supported(cin, cout):
                 res = torch.empty((v.src.shape[0], cout, v.src.shape[2], v.src.shape[3]), dtype=self.dtype, device=self.dev)
@@ -1522,14 +1559,41 @@ class Lowering:
         x = node.args[0]
         if self._separable_conv(node, m, x):
             return True
-        if not isinstance(self.sym(x), (Stack, RealStack)) and x.dim() == 4:      # SIGEConv2d in sparse mode always sees a tile stack
+        mod = self._modulated(x, m.weight, m.stride)
+        if mod is None and not isinstance(self.sym(x), (Stack, RealStack)) and x.dim() == 4:      # SIGEConv2d in sparse mode always sees a tile stack
             t = self.runtime_tensor(x)
             if not t.is_contiguous(memory_format=torch.channels_last):
                 src, t = t, torch.empty(tuple(t.shape), dtype=self.dtype, device=self.dev, memory_format=torch.channels_last)
                 self.steps.append(("eager", lambda _s, src=src, t=t: t.copy_(src)))
                 self.eager_nodes.append("to_nhwc")
             self.env[id(x)] = RealStack(t)
-        return self._conv_common(node, node.args[0], m.weight, m.bias, m.stride, 0, m.dilation, m.groups)
+        return self._conv_common(node, node.args[0], m.weight, m.bias, m.stride, 0, m.dilation, m.groups, src=mod)
+
+    def _modulated(self, x, weight, stride) -> Optional[ModStack]:
+        """The source of a conv that reads SPADE's modulation `leaky((x*scale+shift) * (1 + gamma) + beta)` (Spade stage 3) of three lazy
+        Stacks of single buffers cut with ONE tile list (reference gaugan/models/sige_normalization.py:84-86: x from the block's
+        Gather with the batch norm folded in, gamma / beta re-gathered from the separable launches' buffers), when the executor
+        runs such launches; None otherwise (the modulation is then evaluated on its own)."""
+        ok = getattr(self.ex, "modulated_conv_supported", None)
+        v = self.sym(x) if isinstance(x, LazyTensor) else None
+        if ok is None or not isinstance(v, Spade) or v.stage != 3 or (v.slope is not None and not math.isfinite(v.slope)):
+            return None
+        sx, sg, sb = self.sym(v.x), self.sym(v.gamma), self.sym(v.beta)
+        if not all(isinstance(t, Stack) and not isinstance(t, ModStack) for t in (sx, sg, sb)):
+            return None
+        g, f = sx.gather, sx.src
+        if (getattr(g, "tile_images", None) is not None or g.activation_name != "identity" or g.block_size[0] != g.block_size[1]
+                or int(g.active_indices.shape[0]) == 0 or not f.plain or len(f.segs) != 1):
+            return None
+        shape = (f.B, f.C, *f.HW)
+        for t in (sg, sb):
+            if (t.src.single is None or t.scale is not None or t.shift is not None or t.gather.activation_name != "identity"
+                    or not self._same_gather(t.gather, g) or t.src.single.shape != shape):
+                return None
+        k, s = _pair(weight.shape[2:]), _pair(stride)
+        if k[0] != k[1] or s[0] != s[1] or not ok(f.C, int(weight.shape[0]), k[0], s[0]):
+            return None
+        return ModStack(sx, sg.src.single, sb.src.single, 1.0 if v.slope is None else float(v.slope))
 
     # ---- GAN Compression's separable conv: depthwise 3x3 -> per-channel affine -> 1x1, one launch per SPADE layer
     def _separable_conv(self, node: Node, m, x) -> bool:
@@ -1769,6 +1833,7 @@ class Lowering:
         # reference gaugan/models/spade_generators/sige_fused_spade_generator.py:160-198 — such a launch scatters through the
         # module's own tile sets and always takes the un-fused form below)
         main_real, sc_real = isinstance(co.src, RealStack), isinstance(sc.src, RealStack)
+        modulated = isinstance(co.src, ModStack) or isinstance(sc.src, ModStack)     # (the fused shortcut reads its source raw)
         if not ((isinstance(co.src, Stack) or main_real) and (isinstance(sc.src, Stack) or sc_real)):
             return False
         mg, sg = m.main_gather.module, m.shortcut_gather.module
@@ -1781,7 +1846,8 @@ class Lowering:
         if sc_real:
             if not real_ok(sc, sg):
                 return False
-        elif sc.src.gather is not sg or sc.k != 1 or sc.src.scale is not None or sc.src.shift is not None or sg.activation_name != "identity":
+        elif sc.src.gather is not sg or sc.k != 1 or ((sc.src.scale is not None or sc.src.shift is not None) and not isinstance(sc.src, ModStack)) \
+                or sg.activation_name != "identity":
             return False
         cid = m.cache_id
         dst = self.cached(m.original_outputs[cid], mg.num_edits)
@@ -1800,7 +1866,7 @@ class Lowering:
             sc_key = sc_key + sg.tile_images.to(self.dev).long() * (width * width)
         subset = bool(torch.isin(sc_key, main_key).all()) and tuple(mg.block_stride) == tuple(sg.block_stride) == (4, 4) \
             and int(sg.block_size[0]) == 4 and int(mg.block_size[0]) == 6
-        fuse = (not main_real and not sc_real and self.fuse_shortcut and self.tc5 and self.producer_preop and subset and co.k == 3 and co.stride == 1
+        fuse = (not main_real and not sc_real and not modulated and self.fuse_shortcut and self.tc5 and self.producer_preop and subset and co.k == 3 and co.stride == 1
                 and all(up == 0 for _, up in sc_full.segs) and len(sc_full.segs) <= 2 and sc_full.plain
                 and int(sc.weight.shape[1]) % 64 == 0 and int(co.weight.shape[1]) % 64 == 0)
         name = self._module_name(node)

@@ -344,12 +344,35 @@ def tile_conv_narrow_supported(cin: int, cout: int, k: int, stride: int, dtype: 
         and k >= 1 and stride >= 1
 
 
+def tile_conv_modulated_supported(cin: int, cout: int, k: int, stride: int, dtype: torch.dtype) -> bool:
+    """Does ``sige_tile_conv_modulated`` (SPADE's modulation in the gather stage, mma.sync kernel) take this conv?"""
+    code = {torch.float16: _cabi.F16, torch.bfloat16: _cabi.BF16}.get(dtype)
+    return code is not None and bool(_cabi.lib().sige_tile_conv_modulated_supported(int(cin), int(cout), int(k), int(stride), code))
+
+
 def tile_conv_descriptor() -> TileConv:
     return TileConv()
 
 
 def launch_tile_conv(desc: TileConv, stream: int) -> None:
     _cabi.check(_cabi.lib().sige_tile_conv(byref(desc), stream), "sige_tile_conv")
+    _bump()
+
+
+def conv_modulation(gamma: torch.Tensor, beta: torch.Tensor, negative_slope: float, gamma_c0: int = 0, beta_c0: int = 0) -> "_cabi.ConvModulation":
+    """sige_conv_modulation_t of channels-last [B, C, H, W] gamma / beta buffers (read from channel gamma_c0 / beta_c0 on)."""
+    for name, t in (("gamma", gamma), ("beta", beta)):
+        if t.dim() != 4 or not t.is_contiguous(memory_format=torch.channels_last):
+            raise ValueError("conv_modulation: %s must be a channels-last 4-D tensor" % name)
+    m = _cabi.ConvModulation()
+    m.gamma, m.gamma_C, m.gamma_c0 = gamma.data_ptr(), int(gamma.shape[1]), int(gamma_c0)
+    m.beta, m.beta_C, m.beta_c0 = beta.data_ptr(), int(beta.shape[1]), int(beta_c0)
+    m.negative_slope = float(negative_slope)
+    return m
+
+
+def launch_tile_conv_modulated(desc: TileConv, mod: "_cabi.ConvModulation", stream: int) -> None:
+    _cabi.check(_cabi.lib().sige_tile_conv_modulated(byref(desc), byref(mod), stream), "sige_tile_conv_modulated")
     _bump()
 
 

@@ -1,13 +1,16 @@
 """Time the sparse step of GauGAN compressed with GAN Compression (the sub-mobile SPADE generator) on one GPU.
 
-    python tools/bench_gaugan_gc.py [--steps 50] [--warmup 10] [--dtype fp16|bf16] [--size full|mini] [--dump-outputs DIR]
+    python tools/bench_gaugan_gc.py [--steps 50] [--warmup 10] [--dtype fp16|bf16] [--size full|mini] [--headroom 0.5] [--dump-outputs DIR]
 
 Workload: sige_b200/workloads/gaugan_gc.py at full size — 512 x 1024 label map, config 32_32_32_48_32_24_24_32 (the published
 GAN Compression Cityscapes sub-network), 5 sparse blocks, the 2.98 % label edit of the full-size GauGAN workload; fp32 model and
 dense pass, sparse step as a fused fp16 step (`set_fused(True, dtype=torch.float16)`) in one CUDA graph.  As bench.py: warm-up,
 per-step CUDA events around `model(x)`, an L2 flush (256 MiB write) between steps outside the events, GPU name / power limit /
 SM clock read in the same run, the launch mix of the compiled step, and --dump-outputs DIR (the last timed step's output as
-float32 .npy).  Prints one JSON line.
+float32 .npy).  The step is compiled with --headroom (extra tile-list capacity); after the timed steps the next-edit figure is
+the wall time from `set_masks_async` of a second, smaller label edit to the synchronised end of the step that follows it (an
+interactive user's next stroke), taken three times alternating with the first edit; `next_edit_in_place` says whether the
+compiled step took the edit without recompiling.  Prints one JSON line.
 """
 from __future__ import annotations
 
@@ -38,6 +41,47 @@ def gpu_info() -> dict:
     return info
 
 
+def edit_b(size: str):
+    """A second label edit, smaller than the workload's and elsewhere in the image: (edited label map, its mask)."""
+    import torch
+
+    from sige_b200.workloads import gaugan_gc as G
+
+    s0, _, _ = G.gaugan_gc_inputs(size)
+    lab = s0.argmax(1)[0].clone()
+    if size == "full":
+        lab[360:440, 700:800] = 3
+    else:
+        lab[40:48, 16:28] = 3
+    s1 = torch.zeros_like(s0)
+    s1.scatter_(1, lab[None, None], 1.0)
+    return s1, (s1 != s0).any(1)[0]
+
+
+def next_edit(net, x_a, dilate_mask, downsample_mask, size: str, dev):
+    """Wall seconds from set_masks_async of the next edit to the synchronised end of the step after it, three times (edit B, edit A,
+    edit B); and whether every one ran on the step compiled first."""
+    import torch
+
+    from sige_b200.workloads import gaugan_gc as G
+
+    x_b, mask_b = (t.to(dev) for t in edit_b(size))
+    mask_a = G.gaugan_gc_inputs(size)[2].to(dev)
+    pyr = {k: downsample_mask(dilate_mask(m, 1), min_res=(4, 8), dilation=0) for k, m in (("a", mask_a), ("b", mask_b))}
+    first = net.fused_step
+    out, in_place = [], True
+    with torch.no_grad():
+        for k, x in (("b", x_b), ("a", x_a), ("b", x_b)):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            net.set_masks_async(pyr[k])
+            net(x)
+            torch.cuda.synchronize()
+            out.append(time.perf_counter() - t0)
+            in_place = in_place and net.fused_step is first
+    return out, in_place
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--steps", type=int, default=50)
@@ -45,6 +89,7 @@ def main():
     ap.add_argument("--dtype", choices=["fp16", "bf16"], default="fp16")
     ap.add_argument("--size", choices=["full", "mini"], default="full")
     ap.add_argument("--no-flush", action="store_true", help="do not flush L2 between timed steps")
+    ap.add_argument("--headroom", type=float, default=0.5, help="extra tile-list capacity of the compiled step")
     ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
 
@@ -62,7 +107,8 @@ def main():
     torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
     net = G.build_gaugan_gc(args.size).to(dev)
     t0 = time.time()
-    G.run_gaugan_gc(net, downsample_mask, dilate_mask, device=dev, size=args.size, fused=lambda n: n.set_fused(True, dtype=dtype))
+    G.run_gaugan_gc(net, downsample_mask, dilate_mask, device=dev, size=args.size,
+                    fused=lambda n: n.set_fused(True, dtype=dtype, headroom=args.headroom))
     compile_s = time.time() - t0
     step = net.fused_step
     x = G.gaugan_gc_inputs(args.size)[1].to(dev)
@@ -88,6 +134,7 @@ def main():
     if args.dump_outputs:
         os.makedirs(args.dump_outputs, exist_ok=True)
         np.save(os.path.join(args.dump_outputs, "out.npy"), out.float().cpu().numpy())
+    next_edit_s, in_place = next_edit(net, x, dilate_mask, downsample_mask, args.size, dev)
     kinds = Counter(k for k, _ in step.steps) if step is not None else Counter()
     low = step.low if step is not None else None
     line = {
@@ -95,7 +142,10 @@ def main():
         "ms_min": float(np.min(ms)), "ms_max": float(np.max(ms)), "steps": len(ms), "warmup": args.warmup,
         "dtype": args.dtype, "l2": "not flushed" if flush is None else "flushed (256 MiB write) between timed steps",
         "gpu": info, "sm_mhz_before_timing": info_before.get("sm_mhz"), "compile_seconds": compile_s,
+        "next_edit_seconds": next_edit_s, "next_edit_median_seconds": float(np.median(next_edit_s)), "next_edit_in_place": in_place,
+        "headroom": args.headroom,
         "launches": {"tile_conv": len(step.fused) if step else 0, "separable": kinds.get("separable", 0), "spade": kinds.get("spade", 0),
+                     "modulated": sum(1 for f in step.fused if getattr(f.spec, "modulation", None) is not None) if step else 0,
                      "eager_nodes": len(step.eager_nodes) if step else None},
         "eager_node_kinds": dict(Counter(step.eager_nodes).most_common(8)) if step else None,
         "separable_branches": [len(r.branches) for r in getattr(low, "separable", [])] if low is not None else None,
