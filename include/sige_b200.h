@@ -377,7 +377,9 @@ int sige_spade_modulate(const void *x, long long x_pixel_stride, const void *gam
  * dw_weight = scale * w, dw_bias = scale * b + shift.
  * Source: a channel window [src_c0, src_c0 + Cin) of an NHWC buffer [B, H, W, src_C] read through `idx` (zero outside the image;
  * SIGE_TILE_NONE tiles read zeros and write nothing), or of a tile stack [B*N, 6, 6, src_C] (row b*N + i).  Destination: channels
- * [dst_c0, dst_c0 + Cout) of an NHWC buffer [B, dH, dW, dst_C] at (idx + off), or a stack [B*N, 4, 4, dst_C].
+ * [dst_c0, dst_c0 + Cout) of an NHWC buffer [B, dH, dW, dst_C] at (idx + off), or a stack [B*N, 4, 4, dst_C].  With a tile list, a
+ * SIGE_TILE_NONE entry writes nothing to either kind of destination: its stack row keeps its contents (whatever a stack source
+ * holds in that row is read and discarded).  A stack-to-stack launch may pass idx = NULL: every row is then a tile.
  * Cin a multiple of 16 in [16, 256], Cout a multiple of 8 in [8, 1024], f16 / bf16 (sige_separable_conv_supported() tells, k = 3);
  * channel counts and offsets multiples of 8; buffers 16-byte aligned.  flags: SIGE_CONV_PDL. */
 typedef struct {

@@ -16,7 +16,7 @@
 //   pointwise  mma.sync.m16n8k16 + ldmatrix from shared memory, fp32 accumulation; the weight block [64][Cin] is loaded before the
 //              dependency wait (it does not depend on the previous kernel);
 //   epilogue   + bias, rounded, staged in shared memory, written as 16-byte channel vectors into the destination (NHWC buffer
-//              with its own channel count / offset, or a stack).
+//              with its own channel count / offset, or a stack); rows of SIGE_TILE_NONE tiles are skipped for either kind.
 // The depthwise is recomputed per output-channel block: 9 FMAs per element against Cout / 64 * 128 for the GEMM.
 #include <type_traits>
 
@@ -237,13 +237,13 @@ __global__ void __launch_bounds__(NTHREADS) separable_conv_kernel(const Params p
         const int n = n0 + v * 8, gt = t0 + (m >> 4);
         if (n >= p.Cout || gt >= p.total) continue;
         const int oy = (m >> 2) & 3, ox = m & 3;
+        const int b = gt / p.N, ti = gt - b * p.N;
+        const int oh = p.idx ? p.idx[2 * ti] : 0;            // no list: a stack-to-stack launch, every row is a tile
+        if (oh == SIGE_TILE_NONE) continue;                  // padding tiles write nothing, to a stack as to a buffer
         long long off;
         if (p.dst_is_stack[br]) {
             off = (((long long)gt * 4 + oy) * 4 + ox) * dC;
         } else {
-            const int b = gt / p.N, ti = gt - b * p.N;
-            const int oh = p.idx[2 * ti];
-            if (oh == SIGE_TILE_NONE) continue;
             const int h = oh + p.offH + oy, w = p.idx[2 * ti + 1] + p.offW + ox;
             if (h < 0 || h >= p.dH[br] || w < 0 || w >= p.dW[br]) continue;
             off = (((long long)b * p.dH[br] + h) * p.dW[br] + w) * dC;
