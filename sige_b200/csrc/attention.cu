@@ -20,52 +20,6 @@ constexpr int QB = 32;        // queries per CTA
 constexpr int KPC = 64;       // keys (and values) per CTA
 constexpr int NTHREADS = 256;
 
-__device__ __forceinline__ uint32_t s32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void ldsm4(uint32_t addr, uint32_t &r0, uint32_t &r1, uint32_t &r2, uint32_t &r3) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm4t(uint32_t addr, uint32_t &r0, uint32_t &r1, uint32_t &r2, uint32_t &r3) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];\n" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-template <typename T> __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1);
-template <> __device__ __forceinline__ void mma16816<__half>(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-template <> __device__ __forceinline__ void mma16816<__nv_bfloat16>(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-template <typename T> __device__ __forceinline__ uint32_t pack2(float a, float b);
-template <> __device__ __forceinline__ uint32_t pack2<__half>(float a, float b) {
-    __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<uint32_t *>(&h);
-}
-template <> __device__ __forceinline__ uint32_t pack2<__nv_bfloat16>(float a, float b) {
-    __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<uint32_t *>(&h);
-}
-
-// ---- mbarrier / bulk-copy wrappers
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "ATTN_WAIT:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra ATTN_DONE;\n"
-        "bra ATTN_WAIT;\n"
-        "ATTN_DONE:\n"
-        "}\n" ::"r"(bar),
-        "r"(parity)
-        : "memory");
-}
 // one contiguous row, global -> shared, completion counted in bytes on an mbarrier (TMA bulk copy, no tensor map)
 __device__ __forceinline__ void bulk_row(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar)
@@ -110,7 +64,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) attention_kernel(const Params p) 
     constexpr int CQ = CO / 4;            // output channels per warp column
     constexpr int NT2 = CQ / 8;           // n-tiles per warp in P·V
     extern __shared__ __align__(128) unsigned char smem[];
-    const uint32_t sb = s32(smem);
+    const uint32_t sb = smem_u32(smem);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int q0 = blockIdx.x * QB, kr = blockIdx.y, b = blockIdx.z;
     const T *base = reinterpret_cast<const T *>(p.qkv) + (long long)b * N * 3 * C;
@@ -127,8 +81,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) attention_kernel(const Params p) 
     __syncthreads();
     if (KS > 1) cg::this_cluster().barrier_arrive();     // "this CTA is running": matched by barrier_wait() before the first remote store
     if (p.pdl) {
-        asm volatile("griddepcontrol.launch_dependents;\n" ::);
-        asm volatile("griddepcontrol.wait;\n" ::: "memory");     // the qkv convolution has completed
+        pdl_release();
+        pdl_acquire();     // the qkv convolution has completed
     }
     if (tid == 0) {
         mbar_expect_tx(bar_qk, (QB + KPC) * C * 2);
@@ -156,10 +110,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) attention_kernel(const Params p) 
 #pragma unroll 8
         for (int kk = 0; kk < C / 16; ++kk) {
             uint32_t a[4], b0, b1, b2, b3;
-            ldsm4(a_base + kk * 32, a[0], a[1], a[2], a[3]);
-            ldsm4(b_base + kk * 32, b0, b1, b2, b3);
-            mma16816<T>(sacc[0], a, b0, b1);
-            mma16816<T>(sacc[1], a, b2, b3);
+            ldmatrix_x4(a_base + kk * 32, a[0], a[1], a[2], a[3]);
+            ldmatrix_x4(b_base + kk * 32, b0, b1, b2, b3);
+            mma_m16n8k16<T>(sacc[0], a, b0, b1);
+            mma_m16n8k16<T>(sacc[1], a, b2, b3);
         }
     }
     // ---- local softmax numerators: rows g and g+8 of this warp's 16 queries, columns 2t,2t+1 of two key tiles
@@ -252,13 +206,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) attention_kernel(const Params p) 
             for (int k4 = 0; k4 < KPC / 16; ++k4) {
                 const int kk = rk * (KPC / 16) + k4;                  // 16-key step
                 uint32_t a[4];
-                ldsm4(a_base + kk * 32, a[0], a[1], a[2], a[3]);
+                ldmatrix_x4(a_base + kk * 32, a[0], a[1], a[2], a[3]);
 #pragma unroll
                 for (int n2 = 0; n2 < NT2 / 2; ++n2) {
                     uint32_t b0, b1, b2, b3;
-                    ldsm4t(v_base + kk * 16 * L::V_PITCH + n2 * 32, b0, b1, b2, b3);
-                    mma16816<T>(t[2 * n2], a, b0, b1);
-                    mma16816<T>(t[2 * n2 + 1], a, b2, b3);
+                    ldmatrix_x4_trans(v_base + kk * 16 * L::V_PITCH + n2 * 32, b0, b1, b2, b3);
+                    mma_m16n8k16<T>(t[2 * n2], a, b0, b1);
+                    mma_m16n8k16<T>(t[2 * n2 + 1], a, b2, b3);
                 }
             }
 #pragma unroll
@@ -294,28 +248,8 @@ template <typename T, int C, int KS> static int launch(const Params &p, int B, c
         }
         attr_dev = dev;
     }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(L::N / QB, KS, B);
-    cfg.blockDim = dim3(NTHREADS);
-    cfg.dynamicSmemBytes = L::TOTAL;
-    cfg.stream = stream;
-    cudaLaunchAttribute attrs[2];
-    int na = 0;
-    if (KS > 1) {
-        attrs[na].id = cudaLaunchAttributeClusterDimension;
-        attrs[na].val.clusterDim.x = 1;
-        attrs[na].val.clusterDim.y = KS;
-        attrs[na].val.clusterDim.z = 1;
-        ++na;
-    }
-    if (p.pdl) {
-        attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attrs[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
-    cfg.attrs = attrs;
-    cfg.numAttrs = na;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, attention_kernel<T, C, KS>, p);
+    const cudaError_t e = launch_ex(attention_kernel<T, C, KS>, dim3(L::N / QB, KS, B), dim3(NTHREADS), L::TOTAL, stream, p.pdl != 0,
+                                    dim3(1, KS, 1), p);
     if (e != cudaSuccess) {
         set_error("sige_attention_tokens: launch failed: %s", cudaGetErrorString(e));
         (void)cudaGetLastError();

@@ -8,7 +8,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <utility>
+
 #include "../../include/sige_b200.h"
+#include "ptx.cuh"
 
 namespace sige {
 
@@ -46,6 +49,35 @@ int check_launch(const char *what);
             return 1;                    \
         }                                \
     } while (0)
+
+// cudaLaunchKernelEx with a thread-block cluster (attribute added only when `cluster` is not 1x1x1) and programmatic
+// dependent launch (attribute added only when `pdl` is set).  The caller reports a failure in its own words.
+template <typename... KArgs, typename... Args>
+cudaError_t launch_ex(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, bool pdl, dim3 cluster,
+                      Args &&...args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cudaLaunchAttribute attrs[2];
+    int na = 0;
+    if (cluster.x * cluster.y * cluster.z > 1) {
+        attrs[na].id = cudaLaunchAttributeClusterDimension;
+        attrs[na].val.clusterDim.x = cluster.x;
+        attrs[na].val.clusterDim.y = cluster.y;
+        attrs[na].val.clusterDim.z = cluster.z;
+        ++na;
+    }
+    if (pdl) {
+        attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        attrs[na].val.programmaticStreamSerializationAllowed = 1;
+        ++na;
+    }
+    cfg.attrs = attrs;
+    cfg.numAttrs = na;
+    return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+}
 
 // ----------------------------------------------------------------------------
 // dtype traits

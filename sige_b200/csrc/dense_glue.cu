@@ -7,33 +7,15 @@
 // they are pure HBM streams: 16.8 MB written (conv_in) or read (stats, conv_out) at 256x256x128.
 //
 // All three are deterministic (fixed reduction order), stream-ordered and allocation-free.
-#include <type_traits>
-
 #include "common.cuh"
 
 namespace sige {
 
 // Programmatic dependent launch for the glue kernels: each one releases its successor right away
-// (griddepcontrol.launch_dependents: the successor's launch latency and constant staging overlap this kernel) and
-// waits for its predecessor's results just before the first dependent read (griddepcontrol.wait; a no-op when the
-// launch carries no programmatic edge).  Always on: both instructions are harmless in an ordinary stream.
-__device__ __forceinline__ void pdl_release() { asm volatile("griddepcontrol.launch_dependents;\n" ::); }
-__device__ __forceinline__ void pdl_acquire() { asm volatile("griddepcontrol.wait;\n" ::: "memory"); }
-
-template <typename... KArgs, typename... Args>
-static void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = block;
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    at[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    (void)cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);   // errors surface through check_launch()
-}
+// (pdl_release: the successor's launch latency and constant staging overlap this kernel) and waits for its
+// predecessor's results just before the first dependent read (pdl_acquire; a no-op when the launch carries no
+// programmatic edge).  Always on: both instructions are harmless in an ordinary stream, and every glue launch carries
+// the PDL attribute (launch_ex errors surface through check_launch()).
 
 // ------------------------------------------------------------------------------------------
 // conv_in: Cin <= 4, Cout % 8 == 0.  One thread = one pixel x 8 output channels (one 16-byte store);
@@ -443,7 +425,7 @@ __global__ void __launch_bounds__(CO_TH * 32) conv_out_kernel(const T *__restric
     __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;            // warp = output row inside the tile
     float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-    const uint32_t tbase = (uint32_t)__cvta_generic_to_shared(tile), wbase = (uint32_t)__cvta_generic_to_shared(wsm);
+    const uint32_t tbase = smem_u32(tile), wbase = smem_u32(wsm);
     const int a_row = lane & 15, a_khalf = lane >> 4;                      // ldmatrix.x4: 16 pixel rows x {k-lo, k-hi}
     const int b_row = lane & 7, b_khalf = (lane >> 3) & 1;                 // ldmatrix.x2: 8 channel rows x {k-lo, k-hi}
     for (int tap = 0; tap < 9; ++tap) {
@@ -455,19 +437,9 @@ __global__ void __launch_bounds__(CO_TH * 32) conv_out_kernel(const T *__restric
             asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0,%1}, [%2];\n" : "=r"(b0), "=r"(b1) : "r"(brow + kk * 32));
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
-                uint32_t a0, a1, a2, a3;
-                asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n"
-                             : "=r"(a0), "=r"(a1), "=r"(a2), "=r"(a3)
-                             : "r"(arow0 + i * 16 * pitch + kk * 32));
-                if (std::is_same<T, __half>::value) {
-                    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                                 : "+f"(acc[i][0]), "+f"(acc[i][1]), "+f"(acc[i][2]), "+f"(acc[i][3])
-                                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-                } else {
-                    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                                 : "+f"(acc[i][0]), "+f"(acc[i][1]), "+f"(acc[i][2]), "+f"(acc[i][3])
-                                 : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-                }
+                uint32_t a[4];
+                ldmatrix_x4(arow0 + i * 16 * pitch + kk * 32, a[0], a[1], a[2], a[3]);
+                mma_m16n8k16<T>(acc[i], a, b0, b1);
             }
         }
     }
@@ -516,8 +488,8 @@ int sige_conv_in_nhwc(const void *x, const void *w, const void *bias, void *out,
         ia[i] = InAux{aux[i].ptr, aux[i].scale, aux[i].shift, aux[i].act};
     }
     switch (dtype) {
-        case SIGE_F16: launch_pdl(conv_in_kernel<__half>, dim3(grid), dim3(256), smem, st, (const __half *)x, (const __half *)w, (const __half *)bias, (__half *)out, B, H, W, Cin, Cout, n_aux, ia[0], ia[1]); break;
-        case SIGE_BF16: launch_pdl(conv_in_kernel<__nv_bfloat16>, dim3(grid), dim3(256), smem, st, (const __nv_bfloat16 *)x, (const __nv_bfloat16 *)w, (const __nv_bfloat16 *)bias, (__nv_bfloat16 *)out, B, H, W, Cin, Cout, n_aux, ia[0], ia[1]); break;
+        case SIGE_F16: (void)launch_ex(conv_in_kernel<__half>, dim3(grid), dim3(256), smem, st, true, dim3(1, 1, 1), (const __half *)x, (const __half *)w, (const __half *)bias, (__half *)out, B, H, W, Cin, Cout, n_aux, ia[0], ia[1]); break;
+        case SIGE_BF16: (void)launch_ex(conv_in_kernel<__nv_bfloat16>, dim3(grid), dim3(256), smem, st, true, dim3(1, 1, 1), (const __nv_bfloat16 *)x, (const __nv_bfloat16 *)w, (const __nv_bfloat16 *)bias, (__nv_bfloat16 *)out, B, H, W, Cin, Cout, n_aux, ia[0], ia[1]); break;
         default: set_error("sige_conv_in_nhwc: dtype must be f16/bf16"); return 1;
     }
     return check_launch("sige_conv_in_nhwc");
@@ -547,8 +519,8 @@ int sige_conv_in_nhwc_tiles(const void *x, const void *w, const void *bias, void
         ia[i] = InAux{aux[i].ptr, aux[i].scale, aux[i].shift, aux[i].act};
     }
     switch (dtype) {
-        case SIGE_F16: launch_pdl(conv_in_tiles_kernel<__half>, dim3(grid), dim3(256), smem, st, (const __half *)x, (const __half *)w, (const __half *)bias, (__half *)out, H, W, Cin, Cout, idx, n_tiles, NT, R, S, idx_per_image, n_aux, ia[0], ia[1]); break;
-        case SIGE_BF16: launch_pdl(conv_in_tiles_kernel<__nv_bfloat16>, dim3(grid), dim3(256), smem, st, (const __nv_bfloat16 *)x, (const __nv_bfloat16 *)w, (const __nv_bfloat16 *)bias, (__nv_bfloat16 *)out, H, W, Cin, Cout, idx, n_tiles, NT, R, S, idx_per_image, n_aux, ia[0], ia[1]); break;
+        case SIGE_F16: (void)launch_ex(conv_in_tiles_kernel<__half>, dim3(grid), dim3(256), smem, st, true, dim3(1, 1, 1), (const __half *)x, (const __half *)w, (const __half *)bias, (__half *)out, H, W, Cin, Cout, idx, n_tiles, NT, R, S, idx_per_image, n_aux, ia[0], ia[1]); break;
+        case SIGE_BF16: (void)launch_ex(conv_in_tiles_kernel<__nv_bfloat16>, dim3(grid), dim3(256), smem, st, true, dim3(1, 1, 1), (const __nv_bfloat16 *)x, (const __nv_bfloat16 *)w, (const __nv_bfloat16 *)bias, (__nv_bfloat16 *)out, H, W, Cin, Cout, idx, n_tiles, NT, R, S, idx_per_image, n_aux, ia[0], ia[1]); break;
         default: set_error("sige_conv_in_nhwc_tiles: dtype must be f16/bf16"); return 1;
     }
     return check_launch("sige_conv_in_nhwc_tiles");
@@ -580,9 +552,10 @@ int sige_group_norm_fold(const void *x, int dtype, int B, int H, int W, int C, i
 #define SIGE_GN(T)                                                                                                                       \
     do {                                                                                                                                 \
         if (smem1 > 48 * 1024) cudaFuncSetAttribute(gn_partial_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1);        \
-        launch_pdl(gn_partial_kernel<T>, g1, dim3(256), smem1, st, (const T *)x, HW, C, workspace, nblk);                                 \
-        launch_pdl(gn_finalize_kernel<T>, dim3(C / cpb, B), dim3(1024), sizeof(double) * 2 * cpb * (1024 / cpb > 0 ? 1024 / cpb : 1), st,            \
-                   (const float *)workspace, nblk, HW, C, groups, eps, (const T *)gamma, (const T *)beta, scale, shift, cpb);              \
+        (void)launch_ex(gn_partial_kernel<T>, g1, dim3(256), smem1, st, true, dim3(1, 1, 1), (const T *)x, HW, C, workspace, nblk);       \
+        (void)launch_ex(gn_finalize_kernel<T>, dim3(C / cpb, B), dim3(1024), sizeof(double) * 2 * cpb * (1024 / cpb > 0 ? 1024 / cpb : 1), \
+                        st, true, dim3(1, 1, 1), (const float *)workspace, nblk, HW, C, groups, eps, (const T *)gamma, (const T *)beta,    \
+                        scale, shift, cpb);                                                                                                \
     } while (0)
     switch (dtype) {
         case SIGE_F16: SIGE_GN(__half); break;
@@ -607,8 +580,8 @@ int sige_conv_out_nhwc(const void *x, const float *scale, const float *shift, in
 #define SIGE_CO(T)                                                                                                        \
     do {                                                                                                                  \
         cudaFuncSetAttribute(conv_out_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);                  \
-        launch_pdl(conv_out_kernel<T>, grid, dim3(CO_TH * 32), smem, st, (const T *)x, scale, shift, act, (const T *)w, (const T *)bias, (T *)out, B, H, \
-                   W, C, Cout);                                                                                           \
+        (void)launch_ex(conv_out_kernel<T>, grid, dim3(CO_TH * 32), smem, st, true, dim3(1, 1, 1), (const T *)x, scale, shift, act,  \
+                        (const T *)w, (const T *)bias, (T *)out, B, H, W, C, Cout);                                               \
     } while (0)
     switch (dtype) {
         case SIGE_F16: SIGE_CO(__half); break;

@@ -18,8 +18,6 @@
 //   epilogue   + bias, rounded, staged in shared memory, written as 16-byte channel vectors into the destination (NHWC buffer
 //              with its own channel count / offset, or a stack); rows of SIGE_TILE_NONE tiles are skipped for either kind.
 // The depthwise is recomputed per output-channel block: 9 FMAs per element against Cout / 64 * 128 for the GEMM.
-#include <type_traits>
-
 #include "common.cuh"
 
 namespace sige {
@@ -60,24 +58,6 @@ __host__ __device__ constexpr int smem_bytes(int cin) {
     return RING_BYTES + (M + BN) * (cin + 8) * 2 + 10 * cin * 4;
 }
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(valid ? 16 : 0));
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
-__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4]) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
-}
-template <typename T> __device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    if (std::is_same<T, __half>::value)
-        asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-    else
-        asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                     : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
 template <typename T>
 __global__ void __launch_bounds__(NTHREADS) separable_conv_kernel(const Params p) {
     extern __shared__ __align__(128) uint8_t smem[];
@@ -96,7 +76,7 @@ __global__ void __launch_bounds__(NTHREADS) separable_conv_kernel(const Params p
     for (int u = tid; u < BN * cv; u += NTHREADS) {
         const int n = u / cv, v = u - n * cv;
         const bool ok = n0 + n < p.Cout;
-        cp_async16(smem_u32(Ws + n * apitch + v * 8), ok ? pw + (size_t)(n0 + n) * Cin + v * 8 : pw, ok);
+        cp_async16_zfill(smem_u32(Ws + n * apitch + v * 8), ok ? pw + (size_t)(n0 + n) * Cin + v * 8 : pw, ok);
     }
     cp_async_commit();
     const float *dw = p.dw_w[br], *db = p.dw_b[br];
@@ -106,8 +86,8 @@ __global__ void __launch_bounds__(NTHREADS) separable_conv_kernel(const Params p
     }
     for (int c = tid; c < Cin; c += NTHREADS) dwb[c] = db ? db[c] : 0.f;
     if (p.pdl) {
-        asm volatile("griddepcontrol.launch_dependents;\n" ::);
-        asm volatile("griddepcontrol.wait;\n" ::: "memory");
+        pdl_release();
+        pdl_acquire();
     }
 
     // ---- halo addressing: a thread owns the same UPT (tile, pixel, 8-channel half) units in every chunk
@@ -140,7 +120,7 @@ __global__ void __launch_bounds__(NTHREADS) separable_conv_kernel(const Params p
 #pragma unroll
         for (int i = 0; i < UPT; ++i) {
             const int u = tid + i * NTHREADS;
-            if (u < UNITS) cp_async16(smem_u32(hb + u * 8), gok[i] ? src + goff[i] + k * KC : src, gok[i]);
+            if (u < UNITS) cp_async16_zfill(smem_u32(hb + u * 8), gok[i] ? src + goff[i] + k * KC : src, gok[i]);
         }
     };
 
@@ -199,15 +179,16 @@ __global__ void __launch_bounds__(NTHREADS) separable_conv_kernel(const Params p
         for (int kk = 0; kk < Cin; kk += 16) {
             uint32_t a[2][4];
 #pragma unroll
-            for (int i = 0; i < 2; ++i) ldmatrix_x4(smem_u32(As + (wm * 32 + i * 16 + (lane & 15)) * apitch + kk + (lane >> 4) * 8), a[i]);
+            for (int i = 0; i < 2; ++i)
+                ldmatrix_x4(smem_u32(As + (wm * 32 + i * 16 + (lane & 15)) * apitch + kk + (lane >> 4) * 8), a[i][0], a[i][1], a[i][2], a[i][3]);
 #pragma unroll
             for (int jp = 0; jp < 2; ++jp) {
                 uint32_t b[4];
-                ldmatrix_x4(smem_u32(Ws + (wn * 32 + jp * 16 + b_nl) * apitch + kk + b_kh * 8), b);
+                ldmatrix_x4(smem_u32(Ws + (wn * 32 + jp * 16 + b_nl) * apitch + kk + b_kh * 8), b[0], b[1], b[2], b[3]);
 #pragma unroll
                 for (int i = 0; i < 2; ++i) {
-                    mma16816<T>(acc[i][2 * jp], a[i], b[0], b[1]);
-                    mma16816<T>(acc[i][2 * jp + 1], a[i], b[2], b[3]);
+                    mma_m16n8k16<T>(acc[i][2 * jp], a[i], b[0], b[1]);
+                    mma_m16n8k16<T>(acc[i][2 * jp + 1], a[i], b[2], b[3]);
                 }
             }
         }
@@ -266,20 +247,12 @@ template <typename T> static int launch(const Params &p, cudaStream_t st) {
         }
         attr_dev = dev;
     }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(ceil_div(p.total, TILES), ceil_div(p.Cout, BN), p.dst[1] ? 2 : 1);
-    cfg.blockDim = dim3(NTHREADS);
-    cfg.dynamicSmemBytes = smem_bytes(p.Cin);
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = p.pdl ? 1 : 0;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, p);
+    const dim3 grid(ceil_div(p.total, TILES), ceil_div(p.Cout, BN), p.dst[1] ? 2 : 1);
+    const int smem = smem_bytes(p.Cin);
+    const cudaError_t e = launch_ex(kern, grid, dim3(NTHREADS), smem, st, p.pdl != 0, dim3(1, 1, 1), p);
     if (e != cudaSuccess) {
-        set_error("sige_separable_conv: launch failed (grid %d x %d x %d, %d B smem): %s", cfg.gridDim.x, cfg.gridDim.y, cfg.gridDim.z,
-                  (int)cfg.dynamicSmemBytes, cudaGetErrorString(e));
+        set_error("sige_separable_conv: launch failed (grid %d x %d x %d, %d B smem): %s", grid.x, grid.y, grid.z, smem,
+                  cudaGetErrorString(e));
         (void)cudaGetLastError();
         return 2;
     }

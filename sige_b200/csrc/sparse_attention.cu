@@ -21,36 +21,6 @@ constexpr int BM = 64;        // queries per CTA
 constexpr int BNK = 64;       // keys per ring stage
 constexpr int NTHREADS = 128;
 
-__device__ __forceinline__ uint32_t s32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void ldsm4(uint32_t addr, uint32_t &r0, uint32_t &r1, uint32_t &r2, uint32_t &r3) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm4t(uint32_t addr, uint32_t &r0, uint32_t &r1, uint32_t &r2, uint32_t &r3) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];\n" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-template <typename T> __device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1);
-template <> __device__ __forceinline__ void mma16816<__half>(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-template <> __device__ __forceinline__ void mma16816<__nv_bfloat16>(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-template <typename T> __device__ __forceinline__ uint32_t pack2(float a, float b);
-template <> __device__ __forceinline__ uint32_t pack2<__half>(float a, float b) {
-    __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<uint32_t *>(&h);
-}
-template <> __device__ __forceinline__ uint32_t pack2<__nv_bfloat16>(float a, float b) {
-    __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-    return *reinterpret_cast<uint32_t *>(&h);
-}
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, uint32_t src_bytes) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;\n" ::: "memory"); }
-template <int N> __device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N) : "memory"); }
 __device__ __forceinline__ float fast_exp2(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;\n" : "=f"(y) : "f"(x));
@@ -88,7 +58,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) sparse_attention_kernel(const Par
     constexpr int KS = DP / 16;               // k-steps of Q K^T
     constexpr int NT = DP / 8;                // n-tiles of P V (output channels / 8)
     extern __shared__ __align__(128) unsigned char smem[];
-    const uint32_t sb = s32(smem);
+    const uint32_t sb = smem_u32(smem);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int q0 = blockIdx.x * BM;
     const int bh = blockIdx.y, b = bh / p.heads, h = bh - b * p.heads;
@@ -106,7 +76,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) sparse_attention_kernel(const Par
         for (int i = tid; i < BM * CH; i += NTHREADS) {
             const int r = i / CH, c = i - r * CH;
             const bool ok = q0 + r < p.Nq;
-            cp_async16(sb + L::OFF_Q + r * PITCH + c * 16, qp + (ok ? (long long)(q0 + r) * p.q_sn + c * 8 : 0), ok ? 16u : 0u);
+            cp_async16_zfill(sb + L::OFF_Q + r * PITCH + c * 16, qp + (ok ? (long long)(q0 + r) * p.q_sn + c * 8 : 0), ok);
         }
     };
     auto load_kv = [&](int t, int stage) {
@@ -115,14 +85,14 @@ __global__ void __launch_bounds__(NTHREADS, 2) sparse_attention_kernel(const Par
             const int r = i / CH, c = i - r * CH;
             const bool ok = k0 + r < p.Nk;           // rows past the last key: zero fill (their logits are masked, 0 * V must stay finite)
             const long long tok = ok ? (long long)(k0 + r) : 0;
-            cp_async16(sb + L::OFF_K + (stage * BNK + r) * PITCH + c * 16, kp + tok * p.k_sn + c * 8, ok ? 16u : 0u);
-            cp_async16(sb + L::OFF_V + (stage * BNK + r) * PITCH + c * 16, vp + tok * p.v_sn + c * 8, ok ? 16u : 0u);
+            cp_async16_zfill(sb + L::OFF_K + (stage * BNK + r) * PITCH + c * 16, kp + tok * p.k_sn + c * 8, ok);
+            cp_async16_zfill(sb + L::OFF_V + (stage * BNK + r) * PITCH + c * 16, vp + tok * p.v_sn + c * 8, ok);
         }
     };
     const int ntiles = (p.Nk + BNK - 1) / BNK;
     load_q();
     load_kv(0, 0);
-    cp_commit();
+    cp_async_commit();
 
     const int g = lane >> 2, tq = lane & 3;
     uint32_t qf[KS][4];
@@ -136,14 +106,14 @@ __global__ void __launch_bounds__(NTHREADS, 2) sparse_attention_kernel(const Par
     for (int t = 0; t < ntiles; ++t) {
         const int stage = t & 1;
         if (t + 1 < ntiles) load_kv(t + 1, stage ^ 1);
-        cp_commit();
-        cp_wait<1>();                     // tile t (and, for t == 0, the queries) has landed
+        cp_async_commit();
+        cp_async_wait<1>();                     // tile t (and, for t == 0, the queries) has landed
         __syncthreads();
         if (t == 0) {
             const int arow = warp * 16 + (lane & 15), ahalf = lane >> 4;
             const uint32_t a_base = sb + L::OFF_Q + arow * PITCH + ahalf * 16;
 #pragma unroll
-            for (int kk = 0; kk < KS; ++kk) ldsm4(a_base + kk * 32, qf[kk][0], qf[kk][1], qf[kk][2], qf[kk][3]);
+            for (int kk = 0; kk < KS; ++kk) ldmatrix_x4(a_base + kk * 32, qf[kk][0], qf[kk][1], qf[kk][2], qf[kk][3]);
         }
         // ---- S = Q K^T: 16 queries x 64 keys per warp
         float s[BNK / 8][4];
@@ -159,9 +129,9 @@ __global__ void __launch_bounds__(NTHREADS, 2) sparse_attention_kernel(const Par
 #pragma unroll
                 for (int n2 = 0; n2 < BNK / 16; ++n2) {
                     uint32_t b0, b1, b2, b3;
-                    ldsm4(b_base + n2 * 16 * PITCH + kk * 32, b0, b1, b2, b3);
-                    mma16816<T>(s[2 * n2], qf[kk], b0, b1);
-                    mma16816<T>(s[2 * n2 + 1], qf[kk], b2, b3);
+                    ldmatrix_x4(b_base + n2 * 16 * PITCH + kk * 32, b0, b1, b2, b3);
+                    mma_m16n8k16<T>(s[2 * n2], qf[kk], b0, b1);
+                    mma_m16n8k16<T>(s[2 * n2 + 1], qf[kk], b2, b3);
                 }
         }
         // ---- keys past Nk (last tile only): -inf
@@ -207,9 +177,9 @@ __global__ void __launch_bounds__(NTHREADS, 2) sparse_attention_kernel(const Par
 #pragma unroll
                 for (int n2 = 0; n2 < NT / 2; ++n2) {
                     uint32_t b0, b1, b2, b3;
-                    ldsm4t(v_base + kk * 16 * PITCH + n2 * 32, b0, b1, b2, b3);
-                    mma16816<T>(o[2 * n2], pf[kk], b0, b1);
-                    mma16816<T>(o[2 * n2 + 1], pf[kk], b2, b3);
+                    ldmatrix_x4_trans(v_base + kk * 16 * PITCH + n2 * 32, b0, b1, b2, b3);
+                    mma_m16n8k16<T>(o[2 * n2], pf[kk], b0, b1);
+                    mma_m16n8k16<T>(o[2 * n2 + 1], pf[kk], b2, b3);
                 }
         }
         __syncthreads();                  // this stage is rewritten by the prefetch of the next iteration

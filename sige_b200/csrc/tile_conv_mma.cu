@@ -31,7 +31,6 @@
 #include <cooperative_groups.h>
 
 #include <cmath>
-#include <type_traits>
 
 #include "common.cuh"
 
@@ -88,37 +87,6 @@ struct ConvParams {
     int gC, g_c0, bC, b_c0;
     float slope;
 };
-
-__device__ __forceinline__ uint32_t smem_u32(const void *p) {
-    return (uint32_t)__cvta_generic_to_shared(p);
-}
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void *src, bool valid) {
-    const int sz = valid ? 16 : 0;  // src-size 0 -> zero fill
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(dst), "l"(src), "r"(sz));
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-template <int N> __device__ __forceinline__ void cp_async_wait() {
-    asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
-}
-__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t &r0, uint32_t &r1, uint32_t &r2, uint32_t &r3) {
-    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];\n"
-                 : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
-                 : "r"(addr));
-}
-template <typename T>
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    if (std::is_same<T, __half>::value) {
-        asm volatile(
-            "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-    } else {
-        asm volatile(
-            "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-    }
-}
 
 // swizzle key of a halo pixel at in-tile coordinates (y, x): the 8 rows of one ldmatrix 8x8
 // block are 2 image rows x 4 columns of a 4x4 output tile, so (x&3 | (y&1)<<2) is distinct
@@ -269,7 +237,7 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
                 const int n = q >> 3, u = q & 7;
                 const bool ok = (n0 + n) < p.Cout;
                 const T *src = wbase + (long long)(ok ? (n0 + n) : 0) * KC + u * 8;
-                cp_async16(smem_u32(st + n * 128 + ((u ^ (n & 7)) << 4)), src, ok);
+                cp_async16_zfill(smem_u32(st + n * 128 + ((u ^ (n & 7)) << 4)), src, ok);
             }
         }
         cp_async_commit();
@@ -304,8 +272,8 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
 #pragma unroll
     for (int s = 0; s < NSTAGE - 1; ++s) b_issue(j_begin + s);
     if (p.pdl) {
-        asm volatile("griddepcontrol.launch_dependents;\n" ::);   // let the next layer begin ITS weight prefetch
-        asm volatile("griddepcontrol.wait;\n" ::: "memory");       // previous layer's activations are now visible
+        pdl_release();   // let the next layer begin ITS weight prefetch
+        pdl_acquire();   // previous layer's activations are now visible
     }
     halo_issue(c_first);
     halo_store(c_first, halo[0]);
@@ -343,8 +311,8 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
                 ldmatrix_x4(bbase + n * 128 + ((((kk << 1) | b_khalf) ^ (n & 7)) << 4), b0, b1, b2, b3);
 #pragma unroll
                 for (int i = 0; i < WM; ++i) {
-                    mma16816<T>(acc[i][2 * jp], af[i], b0, b1);
-                    mma16816<T>(acc[i][2 * jp + 1], af[i], b2, b3);
+                    mma_m16n8k16<T>(acc[i][2 * jp], af[i], b0, b1);
+                    mma_m16n8k16<T>(acc[i][2 * jp + 1], af[i], b2, b3);
                 }
             }
         }
@@ -481,31 +449,11 @@ static int launch_cfg(ConvParams &p, cudaStream_t st) {
         set_error("sige_tile_conv: ksplit must be 1, 2, 4 or 8 (got %d)", p.ksplit);
         return 1;
     }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(ceil_div(p.NT, p.tpc), ceil_div(p.Cout, Cfg::BN), p.ksplit);
-    cfg.blockDim = dim3(Cfg::NTHREADS);
-    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute attrs[2];
-    int na = 0;
-    if (p.ksplit > 1) {
-        attrs[na].id = cudaLaunchAttributeClusterDimension;
-        attrs[na].val.clusterDim.x = 1;
-        attrs[na].val.clusterDim.y = 1;
-        attrs[na].val.clusterDim.z = p.ksplit;
-        ++na;
-    }
-    if (p.pdl) {
-        attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attrs[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
-    cfg.attrs = attrs;
-    cfg.numAttrs = na;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, p);
+    const dim3 grid(ceil_div(p.NT, p.tpc), ceil_div(p.Cout, Cfg::BN), p.ksplit);
+    const cudaError_t e = launch_ex(kern, grid, dim3(Cfg::NTHREADS), Cfg::SMEM_BYTES, st, p.pdl != 0, dim3(1, 1, p.ksplit), p);
     if (e != cudaSuccess) {
-        set_error("sige_tile_conv: launch failed (grid %d x %d x %d, %d threads, %d B smem): %s", cfg.gridDim.x, cfg.gridDim.y,
-                  cfg.gridDim.z, Cfg::NTHREADS, Cfg::SMEM_BYTES, cudaGetErrorString(e));
+        set_error("sige_tile_conv: launch failed (grid %d x %d x %d, %d threads, %d B smem): %s", grid.x, grid.y, grid.z,
+                  Cfg::NTHREADS, Cfg::SMEM_BYTES, cudaGetErrorString(e));
         (void)cudaGetLastError();
         return 2;
     }

@@ -26,7 +26,6 @@
 #include <cooperative_groups.h>
 #include <cuda.h>
 
-#include <cstdlib>
 #include <type_traits>
 
 #include "common.cuh"
@@ -98,8 +97,7 @@ struct Params {
     int padded;                // SIGE_CONV_PADDED: whole CTAs of SIGE_TILE_NONE padding may follow the real tiles (B == 1)
     int idx_per_image;         // 1: idx / sc_flags hold B*N entries (row b*N + i = tile i of image b), else N shared by all images
     int ksplit;
-    int pdl;
-    int push_async;            // split-K exchange: 1 = st.async + per-owner mbarrier, 0 = plain remote stores + cluster barrier
+    int pdl;                   // launched with programmatic dependent launch: the next layer is released at the epilogue
     int is_bf16;
     long long *trace;          // development aid: per-CTA clock stamps (16 slots), or nullptr
 };
@@ -123,8 +121,8 @@ template <int BN, int TAPS, bool DEEP = false, bool S2 = false, bool DB = false>
     static constexpr int SPC = TAPS / TPS;                     // ring steps per 64-channel chunk
     static constexpr int B_TILE_BYTES = BN * 128;              // one (tap, chunk) weight tile
     static constexpr int B_STAGE_BYTES = TPS * B_TILE_BYTES;
-    // The narrow 3x3 configuration WITHOUT the deep ring is only launched un-split (decide(): every split launch takes the deep
-    // ring), so its split-K exchange slots are never used: their 30 KB hold a third weight stage instead (un-split launches are
+    // The narrow 3x3 configuration WITHOUT the deep ring is only launched un-split (decide() gives the deep ring to exactly the
+    // split launches), so its split-K exchange slots are never used: their 30 KB hold a third weight stage instead (un-split launches are
     // the ones with long K loops per CTA, i.e. weight-ring bound: 72 KB in flight instead of 48).
     static constexpr bool kUnsplit39 = (BN == 64 && TAPS == 9 && !DEEP && !S2);
     static constexpr int NSTB = S2 ? 3 : DEEP ? (DB ? 2 : 5) : ((BN == 128) ? 4 : (TPS == 3 ? 3 : 4));   // weight ring depth (72 / 48 / 120 / 64 / 72 / 32 KB in flight per CTA)
@@ -148,29 +146,8 @@ template <int BN, int TAPS, bool DEEP = false, bool S2 = false, bool DB = false>
 // ------------------------------------------------------------------------------------------
 // PTX wrappers
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t s32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"(bar), "r"(count));
-}
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_LOOP:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra WAIT_DONE;\n"
-        "bra WAIT_LOOP;\n"
-        "WAIT_DONE:\n"
-        "}\n" ::"r"(bar),
-        "r"(parity)
-        : "memory");
 }
 // wait with cluster-scope acquire: the phase is completed by remote st.async complete_tx operations
 __device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
@@ -380,7 +357,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
 
     extern __shared__ unsigned char smem_raw[];
     unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    const uint32_t sbase = s32(smem);
+    const uint32_t sbase = smem_u32(smem);
     const uint32_t bar0 = sbase + C::OFF_BAR;
     // barrier layout (8 bytes each): b_full[NSTB] | b_empty[NSTB] | a_full[2] | a_empty[2] | red_full
     auto B_FULL = [&](int s) { return bar0 + 8 * s; };
@@ -449,11 +426,10 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
     __syncthreads();
     if (p.ksplit > 1) {
         // the receiver's side of the split-K exchange: (ksplit - 1) peers x its share of rows x BN floats will arrive
-        if (tid == 0 && p.push_async) mbar_expect_tx(RED_FULL, (uint32_t)(p.ksplit - 1) * (128 / p.ksplit) * BN * 4);
+        if (tid == 0) mbar_expect_tx(RED_FULL, (uint32_t)(p.ksplit - 1) * (128 / p.ksplit) * BN * 4);
         cg::this_cluster().barrier_arrive();                 // every thread; matched by barrier_wait() before the first remote store
     }
     if (tid == 0) SIGE_TRACE(1);
-    if (p.pdl == 1) asm volatile("griddepcontrol.launch_dependents;\n" ::);   // the next layer may start prefetching ITS weights
 
     auto tl_of = [&](int m) { return S2 ? (m >> 1) & 31 : (TAPS == 9 ? (m >> 2) & 7 : m >> 4); };
     // GEMM row m -> destination pixel index, or -1 (row of a tile that does not exist / outside the image)
@@ -608,7 +584,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
             const uint32_t d_ox0 = sbase + C::OFF_A + (tl * 2) * 128 + ((u ^ ((tl * 2) & 7)) << 4);
             const uint32_t d_ox1 = sbase + C::OFF_A + (tl * 2 + 1) * 128 + ((u ^ ((tl * 2 + 1) & 7)) << 4);
             if (ptid == 0) SIGE_TRACE(2);
-            if (p.pdl) asm volatile("griddepcontrol.wait;\n" ::: "memory");   // activations of the previous layer are complete
+            if (p.pdl) pdl_acquire();   // activations of the previous layer are complete
             int ause = 0;
             for (int c = c_first; c <= c_last; ++c) {
                 mbar_wait(A_EMPTY(0), (ause & 1) ^ 1);                    // the MMAs that read the (single) halo buffer have retired
@@ -792,7 +768,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
             //      destinations; the thread's arrival on A_FULL fires when its copies have landed, so the producer never
             //      waits for data and keeps NAB chunks in flight (register staging kept exactly one in flight)
             auto copy_chunk = [&](int c, unsigned char *abuf, uint32_t full_bar) {
-                const uint32_t abase = s32(abuf);
+                const uint32_t abase = smem_u32(abuf);
                 if (c < NC) {
                     const int cbase = c * KC;
                     const int sg = cbase >= p.C0 ? 1 : 0;
@@ -853,7 +829,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
                 }
                 cp_async_arrive(full_bar);
             };
-            if (p.pdl) asm volatile("griddepcontrol.wait;\n" ::: "memory");   // activations of the previous layer are complete
+            if (p.pdl) pdl_acquire();   // activations of the previous layer are complete
             int ab = 0, ause = 0;
             for (int c = c_first; c <= c_last; ++c) {
                 mbar_wait(A_EMPTY(ab), ((ause / NAB) & 1) ^ 1);           // the MMAs that read this buffer have retired
@@ -864,7 +840,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
                 ab = ause % NAB;
             }
         } else {
-        if (p.pdl) asm volatile("griddepcontrol.wait;\n" ::: "memory");   // activations of the previous layer are complete
+        if (p.pdl) pdl_acquire();   // activations of the previous layer are complete
         issue_any(c_first);
         int ab = 0, ause = 0;
         for (int c = c_first; c <= c_last; ++c) {
@@ -883,7 +859,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
     }
 
     // ---------------- epilogue ----------------
-    if (p.pdl == 2) asm volatile("griddepcontrol.launch_dependents;\n" ::);   // (A/B) release the next layer only now
+    if (p.pdl) pdl_release();             // the next layer's prologue may overlap this epilogue
     float *cst = reinterpret_cast<float *>(smem + C::OFF_A);
     // v[8] (fp32 conv result of 8 consecutive channels starting at n) -> +bias, +residual -> dst and aux destinations
     auto emit = [&](long long pixel, int tl, int n, float (&v)[8]) {
@@ -937,7 +913,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
         }
         __syncthreads();
         if (tid == 0) { SIGE_TRACE(7); SIGE_TRACE(8); SIGE_TRACE(9); }       // (no exchange: staged rows are complete)
-        if (p.pdl) asm volatile("griddepcontrol.wait;\n" ::: "memory");
+        if (p.pdl) pdl_acquire();
         for (int q = tid; q < 128 * (BN / 8); q += NTHREADS) {
             const int m = q / (BN / 8), nv = q - m * (BN / 8);
             const int n = n0 + nv * 8;
@@ -958,7 +934,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
     }
 
     // ---- split-K: every CTA PUSHES the rows of its partial tile straight from registers into the shared memory of the
-    //      rank that owns them (distributed shared memory stores), then each rank sums the ks slots it received (local
+    //      rank that owns them (st.async, counted by the owner's RED_FULL barrier), then each rank sums the ks slots it received (local
     //      reads, fixed order -> deterministic) and stores.  Slot layout at the owner: [source rank][row within the owner's
     //      share][EPI_PITCH]; a rank's own rows go to its halo buffers.  Nobody reads remote memory after the exchange, so
     //      no exit barrier is needed.
@@ -966,13 +942,12 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
     const int per = 128 / p.ksplit;
     cluster.barrier_wait();                // (arrived during setup) every CTA of the cluster is running: remote stores are legal
     if (warp < NCONS_WARPS) {
-        float *rslot = reinterpret_cast<float *>(smem + C::OFF_SLOT);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int m = frag_m + 8 * h;
             const int owner = m / per, lr = m - owner * per;
             const int row_off = ((kr < owner ? kr : kr - 1) * per + lr) * C::EPI_PITCH;      // in the owner's slot region
-            if (p.push_async && owner != kr) {
+            if (owner != kr) {
                 // st.async: the bytes are counted by an mbarrier of the OWNER, which then waits on its own barrier only
                 const uint32_t remote = map_rank(sbase + C::OFF_SLOT + (uint32_t)(row_off + frag_n) * 4, owner);
                 const uint32_t remote_bar = map_rank(RED_FULL, owner);
@@ -980,7 +955,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
                 for (int i = 0; i < BN / 8; ++i)
                     st_async8(remote + 32 * i, __float_as_uint(acc[4 * i + 2 * h]), __float_as_uint(acc[4 * i + 2 * h + 1]), remote_bar);
             } else {
-                float *slot = owner == kr ? cst + lr * C::EPI_PITCH : cluster.map_shared_rank(rslot, owner) + row_off;
+                float *slot = cst + lr * C::EPI_PITCH;
 #pragma unroll
                 for (int i = 0; i < BN / 8; ++i)
                     *reinterpret_cast<float2 *>(slot + 8 * i + frag_n) = make_float2(acc[4 * i + 2 * h], acc[4 * i + 2 * h + 1]);
@@ -988,13 +963,9 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
         }
     }
     if (tid == 0) SIGE_TRACE(7);
-    if (p.pdl) asm volatile("griddepcontrol.wait;\n" ::: "memory");
-    if (p.push_async) {
-        __syncthreads();                   // own rows staged
-        mbar_wait_cluster(RED_FULL, 0);    // the rows the other ranks pushed have landed
-    } else {
-        cluster.sync();                    // all partial rows have landed in their owners' slots
-    }
+    if (p.pdl) pdl_acquire();
+    __syncthreads();                       // own rows staged
+    mbar_wait_cluster(RED_FULL, 0);        // the rows the other ranks pushed have landed
     if (tid == 0) { SIGE_TRACE(8); SIGE_TRACE(9); }
     const float *rslot = reinterpret_cast<const float *>(smem + C::OFF_SLOT);
     for (int q = tid; q < per * (BN / 8); q += NTHREADS) {
@@ -1115,23 +1086,15 @@ static Plan decide(long long NT, int Cin, int Cout, int taps, int Cin2, int kspl
     const long long base = m_blocks * (Cout / pl.bn);
     int ks = ksplit_req;
     if (ks <= 0) {
-        // never spill into a second wave of co-resident CTAs (machine()); splitting pays while every slice keeps >= min_taps taps
+        // never spill into a second wave of co-resident CTAs (machine()); splitting pays while every slice keeps >= kMinTaps taps
+        constexpr int kMinTaps = 3;
         const int *kMaxCtas = mc.max_ctas;
-        static int min_taps = getenv("SIGE_TC5_MIN_TAPS") ? atoi(getenv("SIGE_TC5_MIN_TAPS")) : 3;   // tuning knob (taps per K slice)
         ks = 1;
-        while (split_ok && ks < 8 && base * (ks * 2) <= kMaxCtas[ks * 2] && (J * tps) / (ks * 2) >= min_taps) ks *= 2;
+        while (split_ok && ks < 8 && base * (ks * 2) <= kMaxCtas[ks * 2] && (J * tps) / (ks * 2) >= kMinTaps) ks *= 2;
     }
     if (ks > J || !split_ok) ks = 1;
-    // Two consecutive layers are co-resident under programmatic dependent launch (the successor's prologue overlaps this
-    // layer).  Two layers of 8 clusters of 8 do not fit at once, and a cluster of the successor starts, cold, only when
-    // one of the predecessor exits.  A/B knob: fall back to clusters of 4 there.
-    static int pair_fit = getenv("SIGE_TC5_PAIR_FIT") ? atoi(getenv("SIGE_TC5_PAIR_FIT")) : 0;
-    if (pair_fit && ksplit_req <= 0 && ks == 8 && base > 7) ks = 4;
     pl.ksplit = ks;
-    static int deep_env = getenv("SIGE_TC5_DEEP") ? atoi(getenv("SIGE_TC5_DEEP")) : 1;   // A/B knob
-    // (2 = also for un-split launches: a single halo buffer exposes the gather of every chunk, two weight stages cap the
-    //  weight ring; an A/B knob)
-    pl.deep = (!s2 && pl.bn == 64 && taps == 9 && (ks > 1 || deep_env >= 2)) ? 1 : 0;       // (split launches: always — Cfg::kUnsplit39)
+    pl.deep = (!s2 && pl.bn == 64 && taps == 9 && ks > 1) ? 1 : 0;       // every split narrow 3x3 launch, and only those (Cfg::kUnsplit39)
     return pl;
 }
 
@@ -1178,31 +1141,10 @@ static int launch_v(Params &p, const void *w_packed, const void *w2_packed, cuda
         }
         attr_dev = dev;
     }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(ceil_div(p.NT, C::CT), p.Cout / BN, p.ksplit);
-    cfg.blockDim = dim3(NTHREADS);
-    cfg.dynamicSmemBytes = C::SMEM_BYTES;
-    cfg.stream = st;
-    cudaLaunchAttribute attrs[2];
-    int na = 0;
-    if (p.ksplit > 1) {
-        attrs[na].id = cudaLaunchAttributeClusterDimension;
-        attrs[na].val.clusterDim.x = 1;
-        attrs[na].val.clusterDim.y = 1;
-        attrs[na].val.clusterDim.z = p.ksplit;
-        ++na;
-    }
-    if (p.pdl) {
-        attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attrs[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
-    cfg.attrs = attrs;
-    cfg.numAttrs = na;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, kern, p, wmap, wmap2);
+    const dim3 grid(ceil_div(p.NT, C::CT), p.Cout / BN, p.ksplit);
+    const cudaError_t e = launch_ex(kern, grid, dim3(NTHREADS), C::SMEM_BYTES, st, p.pdl != 0, dim3(1, 1, p.ksplit), p, wmap, wmap2);
     if (e != cudaSuccess) {
-        set_error("sige_tile_conv(wgmma): launch failed (grid %d x %d x %d): %s", cfg.gridDim.x, cfg.gridDim.y, cfg.gridDim.z,
-                  cudaGetErrorString(e));
+        set_error("sige_tile_conv(wgmma): launch failed (grid %d x %d x %d): %s", grid.x, grid.y, grid.z, cudaGetErrorString(e));
         (void)cudaGetLastError();
         return 2;
     }
@@ -1212,9 +1154,8 @@ static int launch_v(Params &p, const void *w_packed, const void *w2_packed, cuda
 // pure-copy gathers (no pre-op in the gather stage) take the cp.async variant
 template <typename T, int BN, int TAPS, bool DEEP = false, bool DB = false>
 static int launch(Params &p, const void *w_packed, const void *w2_packed, cudaStream_t st) {
-    static int async_env = getenv("SIGE_TC5_ASYNC_GATHER") ? atoi(getenv("SIGE_TC5_ASYNC_GATHER")) : 1;      // A/B knob
     const bool pure_copy = p.scale == nullptr && p.shift == nullptr && p.act == SIGE_ACT_IDENTITY;
-    if (pure_copy && async_env) return launch_v<T, BN, TAPS, DEEP, true, false, DB>(p, w_packed, w2_packed, st);
+    if (pure_copy) return launch_v<T, BN, TAPS, DEEP, true, false, DB>(p, w_packed, w2_packed, st);
     return launch_v<T, BN, TAPS, DEEP, false, false, DB>(p, w_packed, w2_packed, st);
 }
 
@@ -1247,8 +1188,7 @@ extern "C" int sige_debug_set_split_halo_buffers(int n) {
 
 // stride-2 geometry: 3x3 stride 2 on 5x5 tiles -> 2x2 outputs, pure-copy gather (no pre-op in the gather stage), no fused shortcut
 static bool tc5_is_s2(const sige_tile_conv_t *a) {
-    static int s2_env = getenv("SIGE_TC5_S2") ? atoi(getenv("SIGE_TC5_S2")) : 1;      // A/B knob (0: these layers stay on the mma.sync kernel)
-    return s2_env && a->kH == 3 && a->kW == 3 && a->stride == 2 && a->R == 5 && a->S == 5 && a->n_src2 == 0 && a->scale == nullptr &&
+    return a->kH == 3 && a->kW == 3 && a->stride == 2 && a->R == 5 && a->S == 5 && a->n_src2 == 0 && a->scale == nullptr &&
            a->shift == nullptr && a->act == SIGE_ACT_IDENTITY;
 }
 
@@ -1299,11 +1239,8 @@ int tc5_launch(const sige_tile_conv_t *a, cudaStream_t st) {
     p.idx_per_image = a->idx_per_image ? 1 : 0;
     p.padded = ((a->flags & SIGE_CONV_PADDED) && a->B == 1 && a->idx && !a->src_is_stack && !a->dst_is_stack) ? 1 : 0;
     p.ksplit = a->ksplit;
-    static int trig_env = getenv("SIGE_TC5_LATE_TRIGGER") ? atoi(getenv("SIGE_TC5_LATE_TRIGGER")) : 1;     // A/B knob
-    p.pdl = (a->flags & SIGE_CONV_PDL) ? (trig_env ? 2 : 1) : 0;
+    p.pdl = (a->flags & SIGE_CONV_PDL) ? 1 : 0;
     p.is_bf16 = a->dtype == SIGE_BF16;
-    static int push_env = getenv("SIGE_TC5_PUSH_ASYNC") ? atoi(getenv("SIGE_TC5_PUSH_ASYNC")) : 1;      // A/B knobs
-    p.push_async = push_env;
     p.trace = g_trace;
     const bool s2 = tc5_is_s2(a);
     const tc5::Plan pl = tc5::decide(p.NT, p.Cin, p.Cout, p.taps, p.Cin2, a->ksplit, s2);

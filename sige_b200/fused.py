@@ -38,8 +38,6 @@ inject a CPU simulator of the launch descriptors to check the lowering without a
 """
 from __future__ import annotations
 
-import os
-
 import math
 from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple
 
@@ -808,10 +806,7 @@ class Lowering:
         self.module_names = module_names or {}
         self.pdl, self.tc5, self.producer_preop, self.fuse_shortcut = pdl, tc5, producer_preop, fuse_shortcut
         self.fused_attention, self.sparse_stem, self.ksplit = fused_attention, sparse_stem, ksplit
-        # SD transformer cores on this repo's kernel (SIGE_SPARSE_ATTENTION=0: the cuDNN flash kernel through torch's SDPA, for A/B)
-        self.sparse_attention = os.environ.get("SIGE_SPARSE_ATTENTION", "1") != "0"
         self.sparse_attention_calls = 0
-        self.spade = os.environ.get("SIGE_SPADE_FUSE", "1") != "0"       # SPADE modulation as one launch (0: recorded torch calls, for A/B)
         self.spade_calls = 0
         self.separable: List[SepLaunch] = []
         self._nhwc_stacks: Dict[int, torch.Tensor] = {}
@@ -1967,20 +1962,19 @@ class Lowering:
         if self._sep_affine(node, False):
             return True
         out = node.outs[0]
-        if self.spade:
-            for t_, c_ in ((a, b), (b, a)):        # 1 + gamma on a value that has no symbolic form (a slice of a tile stack), or on the
-                # re-gathered tiles of a separable launch's destination (the sub-mobile SPADE's gamma)
-                if (isinstance(t_, LazyTensor) and isinstance(c_, (int, float)) and float(c_) == 1.0 and t_.dim() == 4
-                        and (self.sym(t_) is None or self._sep_stack(self.sym(t_)) or self._narrow_dense(self.sym(t_)))
-                        and tuple(t_.shape) == tuple(out.shape) and t_.dtype.is_floating_point):
-                    self.env[id(out)] = Spade(1, t_)
+        for t_, c_ in ((a, b), (b, a)):        # 1 + gamma on a value that has no symbolic form (a slice of a tile stack), or on the
+            # re-gathered tiles of a separable launch's destination (the sub-mobile SPADE's gamma)
+            if (isinstance(t_, LazyTensor) and isinstance(c_, (int, float)) and float(c_) == 1.0 and t_.dim() == 4
+                    and (self.sym(t_) is None or self._sep_stack(self.sym(t_)) or self._narrow_dense(self.sym(t_)))
+                    and tuple(t_.shape) == tuple(out.shape) and t_.dtype.is_floating_point):
+                self.env[id(out)] = Spade(1, t_)
+                return True
+        if isinstance(a, LazyTensor) and isinstance(b, LazyTensor):
+            for m_lt, b_lt in ((a, b), (b, a)):       # x * (1 + gamma) + beta
+                sm = self.sym(m_lt)
+                if isinstance(sm, Spade) and sm.stage == 2 and b_lt.dim() == 4 and tuple(b_lt.shape) == tuple(out.shape) == tuple(m_lt.shape):
+                    self.env[id(out)] = Spade(3, sm.gamma, x=sm.x, beta=b_lt)
                     return True
-            if isinstance(a, LazyTensor) and isinstance(b, LazyTensor):
-                for m_lt, b_lt in ((a, b), (b, a)):       # x * (1 + gamma) + beta
-                    sm = self.sym(m_lt)
-                    if isinstance(sm, Spade) and sm.stage == 2 and b_lt.dim() == 4 and tuple(b_lt.shape) == tuple(out.shape) == tuple(m_lt.shape):
-                        self.env[id(out)] = Spade(3, sm.gamma, x=sm.x, beta=b_lt)
-                        return True
         if isinstance(a, LazyTensor) and isinstance(b, LazyTensor):
             for x, r in ((a, b), (b, a)):
                 co = self.sym(x)
@@ -2245,7 +2239,7 @@ class Lowering:
         o = node.outs[0]
         scale = float(g.scale)
         D = int(o.shape[2])
-        ours = self.sparse_attention and scale > 0 and self.ex.sparse_attention_supported(D)
+        ours = scale > 0 and self.ex.sparse_attention_supported(D)
 
         def operand(t):
             """The [(b h), n, d] operand — or, when it is einops' copy of a "b n (h d)" tensor (reshape -> permute -> reshape,
@@ -2340,7 +2334,7 @@ class Lowering:
         q, k, vv = v.s.q, v.s.k, v.v
         C = q.c1 - q.c0
         B, _, H, W = q.buf.shape
-        if not (self.sparse_attention and k.c1 - k.c0 == C and vv.c1 - vv.c0 == C and k.buf.shape[0] == B and vv.buf.shape[0] == B
+        if not (k.c1 - k.c0 == C and vv.c1 - vv.c0 == C and k.buf.shape[0] == B and vv.buf.shape[0] == B
                 and tuple(k.buf.shape[2:]) == tuple(vv.buf.shape[2:]) and v.s.scale > 0 and self.ex.sparse_attention_supported(C)
                 and all(sl.c0 % 8 == 0 and sl.buf.shape[1] % 8 == 0 for sl in (q, k, vv))):
             return False
