@@ -273,6 +273,14 @@ int sige_tile_conv_modulated_supported(int Cin, int Cout, int k, int stride, int
  * not 16-byte aligned, a non-finite slope.  Everything else is sige_tile_conv's contract; N == 0 is a no-op. */
 int sige_tile_conv_modulated(const sige_tile_conv_t *p, const sige_conv_modulation_t *m, sige_stream_t stream);
 
+/* sige_tile_conv whose single source is a channel window of a wider NHWC buffer: channels [c0, c0 + src[0].C) of a buffer with
+ * `src_pixel_stride` channels per pixel, src[0].ptr pointing at channel c0 of pixel 0 — e.g. one torch.split part of a conv's output
+ * (SPADE's actv_0 / actv_1 / actv_s, reference gaugan/models/spade_generators/sige_fused_spade_generator.py:160-167), read in place.
+ * The launch is the one sige_tile_conv makes for the compacted window (same kernel, plan and result); SIGE_CONV_TC5 is honoured.
+ * Refused before any CUDA call: n_src != 1, a stack source, a fused shortcut, idx_per_image, a stride below src[0].C or not a
+ * multiple of 8, a source pointer that is not 16-byte aligned.  Everything else is sige_tile_conv's contract; N == 0 is a no-op. */
+int sige_tile_conv_strided(const sige_tile_conv_t *p, int src_pixel_stride, sige_stream_t stream);
+
 /* Residual block: conv1 -> conv2 of one block (reference diffusion/models/ddpm_arch/sige_fused_unet.py:100-131: main_gather ->
  * conv1 -> scatter_gather -> conv2 -> scatter[_with_block_residual]) as ONE call.  `conv2` gathers from the buffer `conv1`
  * scatters into (conv1->dst or one of its aux views must be conv2's source); its fused 1x1 shortcut / residual fields carry

@@ -124,6 +124,7 @@ PROTOTYPES = {
     "sige_tile_conv": (_I, [POINTER(TileConv), _P]),
     "sige_tile_conv_modulated_supported": (_I, [_I] * 5),
     "sige_tile_conv_modulated": (_I, [POINTER(TileConv), POINTER(ConvModulation), _P]),
+    "sige_tile_conv_strided": (_I, [POINTER(TileConv), _I, _P]),
     "sige_resblock": (_I, [POINTER(TileConv), POINTER(TileConv), _P]),
     "sige_tile_conv_generic": (_I, [_P, _P, _P, _P] + [_I] * 14 + [_P]),
     "sige_tile_conv_plan": (_I, [_P, _P]),

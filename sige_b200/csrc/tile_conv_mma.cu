@@ -42,8 +42,9 @@ constexpr int KC = 64;        // channels per K chunk (128 bytes of fp16/bf16 pe
 
 struct ConvSeg {
     const void *ptr;
-    int C;    // channels of this segment
-    int up;   // nearest x2 upsample on read
+    int pitch;   // elements from one pixel to the next: the segment's channel count, or more for a channel window of a wider
+                 // NHWC buffer (sige_tile_conv_strided; ptr then points at the window's first channel)
+    int up;      // nearest x2 upsample on read
 };
 
 struct AuxDst {
@@ -173,7 +174,7 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
             if (ld_smem[k] >= 0 && ld_pix[k] >= 0 && cbase + u * 8 < p.Cin) {   // channels >= Cin: zero
                 const int hh = (ld_pix[k] >> 16) >> seg.up, ww = (ld_pix[k] & 0xffff) >> seg.up;
                 const T *src = reinterpret_cast<const T *>(seg.ptr) +
-                               (((long long)ld_img[k] * Hs + hh) * Ws + ww) * seg.C + cl + u * 8;
+                               (((long long)ld_img[k] * Hs + hh) * Ws + ww) * seg.pitch + cl + u * 8;
                 ld_reg[k] = __ldg(reinterpret_cast<const uint4 *>(src));
             }
         }
@@ -482,11 +483,12 @@ template <typename T, bool MOD> static int launch_tile_conv(ConvParams &p, cudaS
     return launch_cfg<T, 2, 2, 1, 4, 72, 8, MOD>(p, st);
 }
 
-bool tc5_supported(const sige_tile_conv_t *a);
-int tc5_launch(const sige_tile_conv_t *a, cudaStream_t st);
+bool tc5_supported(const sige_tile_conv_t *a, int pitch0);
+int tc5_launch(const sige_tile_conv_t *a, int pitch0, cudaStream_t st);
 
-// Argument checks and launch of sige_tile_conv; m != nullptr: sige_tile_conv_modulated (whose own refusals come first).
-static int tile_conv(const sige_tile_conv_t *a, const sige_conv_modulation_t *m, sige_stream_t stream) {
+// Argument checks and launch of sige_tile_conv; m != nullptr: sige_tile_conv_modulated, pitch0 > 0: sige_tile_conv_strided (whose
+// own refusals come first).  pitch0 = elements per pixel of the single source (0: its channel count).
+static int tile_conv(const sige_tile_conv_t *a, const sige_conv_modulation_t *m, int pitch0, sige_stream_t stream) {
     SIGE_REQUIRE(a != nullptr, "sige_tile_conv: null descriptor");
     SIGE_REQUIRE(a->dtype == SIGE_F16 || a->dtype == SIGE_BF16,
                  "sige_tile_conv: tensor-core path needs f16/bf16 (got dtype %d); use sige_tile_conv_generic", a->dtype);
@@ -555,14 +557,14 @@ static int tile_conv(const sige_tile_conv_t *a, const sige_conv_modulation_t *m,
         }
         SIGE_REQUIRE(c2 == a->Cin2 && a->w2_packed && ((uintptr_t)a->w2_packed & 15) == 0, "sige_tile_conv: shortcut channels/weights mismatch");
         SIGE_REQUIRE(!a->src_is_stack && !a->dst_is_stack, "sige_tile_conv: the fused shortcut needs full-tensor source and destination");
-        SIGE_REQUIRE((a->flags & SIGE_CONV_TC5) && tc5_supported(a), "sige_tile_conv: the fused shortcut is implemented by the wgmma kernel only (3x3 stride-1 on 6x6 tiles, SIGE_CONV_TC5)");
+        SIGE_REQUIRE((a->flags & SIGE_CONV_TC5) && tc5_supported(a, 0), "sige_tile_conv: the fused shortcut is implemented by the wgmma kernel only (3x3 stride-1 on 6x6 tiles, SIGE_CONV_TC5)");
         SIGE_REQUIRE(a->sc_flags == nullptr || a->residual != nullptr, "sige_tile_conv: sc_flags given without the cached shortcut (residual)");
     }
     // Hopper-native path (wgmma + TMA, tile_conv_tc5.cu) when requested and the geometry fits
-    if (!m && (a->flags & SIGE_CONV_TC5) && tc5_supported(a)) return tc5_launch(a, (cudaStream_t)stream);
+    if (!m && (a->flags & SIGE_CONV_TC5) && tc5_supported(a, pitch0)) return tc5_launch(a, pitch0, (cudaStream_t)stream);
 
     ConvParams p;
-    p.seg[0] = ConvSeg{a->src[0].ptr, a->src[0].C, a->src[0].up};
+    p.seg[0] = ConvSeg{a->src[0].ptr, pitch0 > 0 ? pitch0 : a->src[0].C, a->src[0].up};
     p.seg[1] = a->n_src == 2 ? ConvSeg{a->src[1].ptr, a->src[1].C, a->src[1].up} : p.seg[0];
     p.C0 = a->src[0].C;
     p.src_is_stack = a->src_is_stack;
@@ -609,7 +611,19 @@ static int tile_conv(const sige_tile_conv_t *a, const sige_conv_modulation_t *m,
 
 using namespace sige;
 
-extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) { return tile_conv(a, nullptr, stream); }
+extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) { return tile_conv(a, nullptr, 0, stream); }
+
+extern "C" int sige_tile_conv_strided(const sige_tile_conv_t *a, int src_pixel_stride, sige_stream_t stream) {
+    SIGE_REQUIRE(a != nullptr, "sige_tile_conv_strided: null descriptor");
+    SIGE_REQUIRE(a->n_src == 1, "sige_tile_conv_strided: one source segment (got n_src %d)", a->n_src);
+    SIGE_REQUIRE(!a->src_is_stack, "sige_tile_conv_strided: the source must be a full tensor read through the tile list, not a stack");
+    SIGE_REQUIRE(a->n_src2 == 0, "sige_tile_conv_strided: no fused shortcut");
+    SIGE_REQUIRE(!a->idx_per_image, "sige_tile_conv_strided: per-image tile lists are not supported");
+    SIGE_REQUIRE(src_pixel_stride >= a->src[0].C && src_pixel_stride % 8 == 0,
+                 "sige_tile_conv_strided: pixel stride %d must be a multiple of 8 and at least the source's %d channels", src_pixel_stride, a->src[0].C);
+    SIGE_REQUIRE(((uintptr_t)a->src[0].ptr & 15) == 0, "sige_tile_conv_strided: source is not 16-byte aligned");
+    return tile_conv(a, nullptr, src_pixel_stride, stream);
+}
 
 extern "C" int sige_tile_conv_modulated_supported(int Cin, int Cout, int k, int stride, int dtype) {
     return (dtype == SIGE_F16 || dtype == SIGE_BF16) && Cin > 0 && Cin % 8 == 0 && Cout > 0 && Cout % 8 == 0 && k >= 1 && stride >= 1 ? 1 : 0;
@@ -623,7 +637,7 @@ extern "C" int sige_tile_conv_modulated(const sige_tile_conv_t *a, const sige_co
     SIGE_REQUIRE(a->n_src2 == 0, "sige_tile_conv_modulated: no fused shortcut");
     SIGE_REQUIRE(!a->idx_per_image, "sige_tile_conv_modulated: per-image tile lists are not supported");
     SIGE_REQUIRE(isfinite(m->negative_slope), "sige_tile_conv_modulated: negative_slope must be finite");
-    return tile_conv(a, m, stream);
+    return tile_conv(a, m, 0, stream);
 }
 
 // conv1 -> conv2 of one residual block as one call (see include/sige_b200.h).

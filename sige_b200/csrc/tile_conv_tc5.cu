@@ -58,7 +58,7 @@ constexpr int S2_BUF_BYTES = 3 * S2_COPY_BYTES;          // 122880 per 64-channe
 
 struct Seg {
     const void *ptr;
-    int C;
+    int pitch;   // elements from one pixel to the next (the segment's channel count, or more for a channel window, see ConvSeg)
     int up;
 };
 
@@ -604,7 +604,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
                     for (int x = 0; x < R; ++x) {
                         const int ww = ww0 + x;
                         const bool ok = row_ok && ww >= 0 && ww < p.W;
-                        const T *src = ok ? sbase_p + (rbase + (ww >> seg.up)) * seg.C : reinterpret_cast<const T *>(seg.ptr);
+                        const T *src = ok ? sbase_p + (rbase + (ww >> seg.up)) * seg.pitch : reinterpret_cast<const T *>(seg.ptr);
                         const uint32_t nb = ok ? 16u : 0u;
 #pragma unroll
                         for (int kx = 0; kx < 3; ++kx) {
@@ -645,7 +645,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
                             img = (p.NT != p.N) ? t / p.N : 0;          // batch > 1 only (SD); DDPM is batch 1
                         }
                         if (hh >= 0 && hh < p.H && ww >= 0 && ww < p.W)
-                            g_off[k] = ((img * Hs + (hh >> seg.up)) * Ws + (ww >> seg.up)) * seg.C + (q & 7) * 8;
+                            g_off[k] = ((img * Hs + (hh >> seg.up)) * Ws + (ww >> seg.up)) * seg.pitch + (q & 7) * 8;
                     }
                 }
             }
@@ -745,7 +745,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
                     if (p.NT != p.N) b = t / p.N;
                     const int hh = y + s_idx[2 * tl], ww = xx + s_idx[2 * tl + 1];
                     if (hh >= 0 && hh < p.H && ww >= 0 && ww < p.W) {
-                        const T *src = reinterpret_cast<const T *>(seg.ptr) + (((long long)b * Hs + (hh >> seg.up)) * Ws + (ww >> seg.up)) * seg.C + cl + u * 8;
+                        const T *src = reinterpret_cast<const T *>(seg.ptr) + (((long long)b * Hs + (hh >> seg.up)) * Ws + (ww >> seg.up)) * seg.pitch + cl + u * 8;
                         regs[k] = __ldg(reinterpret_cast<const uint4 *>(src));
                     }
                 }
@@ -819,7 +819,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
                             if (p.NT != p.N) b = t / p.N;
                             const int hh = y + s_idx[2 * tl], ww = xx + s_idx[2 * tl + 1];
                             if (hh >= 0 && hh < p.H && ww >= 0 && ww < p.W) {
-                                src += (((long long)b * Hs + (hh >> seg.up)) * Ws + (ww >> seg.up)) * seg.C + cl + u * 8;
+                                src += (((long long)b * Hs + (hh >> seg.up)) * Ws + (ww >> seg.up)) * seg.pitch + cl + u * 8;
                                 nb = 16;
                             }
                         }
@@ -1193,14 +1193,18 @@ static bool tc5_is_s2(const sige_tile_conv_t *a) {
 }
 
 // Can the wgmma kernel take this layer?  (3x3 stride 1 on 6x6 tiles, 1x1 on 4x4 tiles, or 3x3 stride 2 on 5x5 tiles; Cout % 64 == 0)
-bool tc5_supported(const sige_tile_conv_t *a) {
+// pitch0: elements per pixel of the first source (0: its channel count).
+bool tc5_supported(const sige_tile_conv_t *a, int pitch0) {
     const bool g3 = (a->kH == 3 && a->kW == 3 && a->stride == 1 && a->R == 6 && a->S == 6) || tc5_is_s2(a);
     const bool g1 = a->kH == 1 && a->kW == 1 && a->stride == 1 && a->R == 4 && a->S == 4;
     if (a->n_src2 > 0 && !g3) return false;
     // the kernel keeps 32-bit element offsets into its sources
     const long long px = a->src_is_stack ? (long long)a->B * a->N * a->R * a->S : (long long)a->B * a->H * a->W;
     long long cmax = 0;
-    for (int i = 0; i < a->n_src; ++i) cmax = a->src[i].C > cmax ? a->src[i].C : cmax;
+    for (int i = 0; i < a->n_src; ++i) {
+        const int pitch = (i == 0 && pitch0 > 0) ? pitch0 : a->src[i].C;
+        cmax = pitch > cmax ? pitch : cmax;
+    }
     if (px * cmax >= (1ll << 31)) return false;
     if ((a->dst_is_stack ? (long long)a->B * a->N * 16 : (long long)a->B * a->dH * a->dW) >= (1ll << 31)) return false;
     if (tc5_is_s2(a) && a->dst_is_stack) return false;          // (stack outputs of this geometry: mma.sync kernel)
@@ -1208,9 +1212,9 @@ bool tc5_supported(const sige_tile_conv_t *a) {
 }
 
 // Arguments were validated by sige_tile_conv (tile_conv_mma.cu) before this is called.
-int tc5_launch(const sige_tile_conv_t *a, cudaStream_t st) {
+int tc5_launch(const sige_tile_conv_t *a, int pitch0, cudaStream_t st) {
     tc5::Params p;
-    p.seg[0] = tc5::Seg{a->src[0].ptr, a->src[0].C, a->src[0].up};
+    p.seg[0] = tc5::Seg{a->src[0].ptr, pitch0 > 0 ? pitch0 : a->src[0].C, a->src[0].up};
     p.seg[1] = a->n_src == 2 ? tc5::Seg{a->src[1].ptr, a->src[1].C, a->src[1].up} : p.seg[0];
     p.C0 = a->src[0].C;
     p.src_is_stack = a->src_is_stack;
@@ -1269,7 +1273,7 @@ extern "C" int sige_tile_conv_plan(const sige_tile_conv_t *a, sige_tile_conv_pla
     using namespace sige;
     SIGE_REQUIRE(a && out, "sige_tile_conv_plan: null pointer");
     out->path = 0; out->bn = 0; out->ksplit = 0; out->deep_ring = 0; out->grid_x = out->grid_y = out->grid_z = 0;
-    if (!((a->flags & SIGE_CONV_TC5) && tc5_supported(a))) return 0;      // mma.sync / CUDA-core paths
+    if (!((a->flags & SIGE_CONV_TC5) && tc5_supported(a, 0))) return 0;      // mma.sync / CUDA-core paths
     const long long NT = (long long)a->B * a->N;
     const bool s2 = tc5_is_s2(a);
     const tc5::Plan pl = tc5::decide(NT, a->Cin, a->Cout, a->kH * a->kW, a->n_src2 > 0 ? a->Cin2 : 0, a->ksplit, s2);

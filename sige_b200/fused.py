@@ -340,6 +340,9 @@ class CudaExecutor:
         d.n_src = len(s.srcs)
         for i, (t, up) in enumerate(s.srcs):
             d.src[i].ptr, d.src[i].C, d.src[i].up = t.data_ptr(), t.shape[1], up
+        pitch = 0                           # a channel window of a wider buffer: the strided launch
+        if not s.src_is_stack and len(s.srcs) == 1 and not s.srcs[0][0].is_contiguous(memory_format=torch.channels_last):
+            pitch = ops.channel_window(s.srcs[0][0])[1]
         d.B, d.H, d.W = s.B, s.H, s.W
         d.src_is_stack = 1 if s.src_is_stack else 0
         idx_t, n_per, sc_flags_t = s.idx, s.N, (None if s.shortcut is None else s.shortcut[3])
@@ -389,6 +392,7 @@ class CudaExecutor:
             d.dst, d.n_aux = None, 1
         d.n_src2 = 0
         if s.modulation is not None:       # the mma.sync kernel with SPADE's modulation in its gather stage
+            assert not pitch, s.name
             gamma, beta, slope = s.modulation
             mod = ops.conv_modulation(gamma, beta, slope)
             fc.desc, fc.keep = d, keep + [idx_t, mod]
@@ -408,6 +412,9 @@ class CudaExecutor:
             keep += [w2, b2]
         keep += [idx_t, sc_flags_t]
         fc.desc, fc.keep = d, keep
+        if pitch:
+            fc.launch_fn = lambda stream, d=d, pitch=pitch: ops.launch_tile_conv_strided(d, pitch, stream)
+            return
         fc.launch_fn = lambda stream, d=d: ops.launch_tile_conv(d, stream)
 
     def prepare_conv_in(self, rec: ConvInRec) -> Callable[[int], None]:
@@ -488,6 +495,10 @@ class CudaExecutor:
         """Can sige_tile_conv_modulated run a conv whose source is SPADE's modulation of `cin` channels?"""
         return self.ops.tile_conv_modulated_supported(cin, cout, k, stride, self.dtype)
 
+    def strided_conv_supported(self, cin: int, cout: int, k: int, stride: int) -> bool:
+        """Can sige_tile_conv_strided run a conv whose source is a `cin`-channel window of a wider buffer?"""
+        return self.ops.tile_conv_strided_supported(cin, cout, k, stride, self.dtype)
+
     def _separable_weights(self, dw: "DWConv", pw_w: torch.Tensor, pw_b: Optional[torch.Tensor]):
         """(depthwise weight, bias with the affine folded in fp32; 1x1 weight in the step's dtype; fp32 1x1 bias), cached by the
         identity (and version) of the parameters and of the tensors the affine was recorded with."""
@@ -542,8 +553,9 @@ class CudaExecutor:
 # symbolic values of the lowering
 # =====================================================================================================================
 class Pre:
-    """Pending per-channel pointwise op act(x*scale+shift); scale/shift are fp32 [C] or [B, C] tensors or None.  `mod` = (gamma Buf,
-    beta Buf, slope): SPADE's modulation leaky((x*scale+shift) * (1 + gamma) + beta) after it (a ModStack's gather stage)."""
+    """Pending per-channel pointwise op act(x*scale+shift); scale/shift are fp32 [C] or [B, C] tensors or None.  `mod` = ((gamma Buf,
+    first channel), (beta Buf, first channel), slope): SPADE's modulation leaky((x*scale+shift) * (1 + gamma) + beta) after it (a
+    ModStack's gather stage)."""
 
     def __init__(self, scale=None, shift=None, act: Optional[str] = None, mod=None):
         self.scale, self.shift, self.act, self.mod = scale, shift, act, mod
@@ -589,12 +601,23 @@ class Stack:
 
 class ModStack(Stack):
     """SPADE's modulation of three lazy Stacks cut with one tile list: the tiles of `src` (with the Gather's scale / shift) times
-    (1 + the same tiles of `gamma`) plus those of `beta`, then leaky_relu(slope).  Only ever the source of a ConvOut: the conv's
-    launch applies it in its gather stage (sige_tile_conv_modulated), so none of the stacks is materialised."""
+    (1 + the same tiles of `gamma`) plus those of `beta`, then leaky_relu(slope).  gamma / beta are channels [c0, c0 + C) of their
+    buffers (C = the source's channels; c0 > 0: a torch.split window).  Only ever the source of a ConvOut: the conv's launch applies
+    it in its gather stage (sige_tile_conv_modulated), so none of the stacks is materialised."""
 
-    def __init__(self, x: Stack, gamma: "Buf", beta: "Buf", slope: float):
+    def __init__(self, x: Stack, gamma: "Buf", beta: "Buf", slope: float, gamma_c0: int = 0, beta_c0: int = 0):
         super().__init__(x.src, x.gather, x.scale, x.shift)
         self.gamma, self.beta, self.slope = gamma, beta, slope
+        self.gamma_c0, self.beta_c0 = gamma_c0, beta_c0
+
+
+class WinStack(Stack):
+    """The tiles of channels [c0, c0 + C) of a plain lazy Stack of one buffer (a torch.split part of it: SPADE's actv_0 / actv_1 /
+    actv_s).  Only ever the source of a ConvOut: the launch reads the window in place (sige_tile_conv_strided)."""
+
+    def __init__(self, st: Stack, c0: int, C: int):
+        super().__init__(st.src, st.gather, st.scale, st.shift)
+        self.c0, self.C = c0, C
 
 
 class RealStack:
@@ -734,6 +757,11 @@ _POINTWISE = {"add", "mul", "sub", "div", "rsub", "neg", "leaky_relu", "relu", "
 _MATERIAL = (Full, Stack, RealStack, ConvOut, RealT)
 _VIEW_OPS = {"reshape", "view", "permute", "transpose", "chunk", "split", "__getitem__", "unsqueeze", "squeeze", "flatten", "unflatten",
              "expand", "narrow", "select", "unbind", "t", "movedim", "swapaxes", "view_as", "reshape_as", "T.__get__", "mT.__get__"}
+
+
+def _channels(t: torch.Tensor, c0: int, C: int) -> torch.Tensor:
+    """Channels [c0, c0 + C) of a (B, C', H, W) buffer: the buffer itself when that is all of it, else the channel-slice view."""
+    return t if (c0 == 0 and int(t.shape[1]) == C) else t[:, c0:c0 + C]
 
 
 def _bits(t: torch.Tensor) -> torch.Tensor:
@@ -936,10 +964,11 @@ class Lowering:
                   weight: torch.Tensor, bias: Optional[torch.Tensor], stride: int, off: int, dst: Optional[Buf], residual: Optional[Buf] = None,
                   shortcut=None, stack_src: Optional[torch.Tensor] = None, dst_stack: Optional[torch.Tensor] = None,
                   weight_fold: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, tile_img: Optional[torch.Tensor] = None,
-                  cin_pad: int = 0, epilogue: Optional[str] = None) -> Optional[FusedConv]:
+                  cin_pad: int = 0, epilogue: Optional[str] = None, window: Optional[Tuple[int, int]] = None) -> Optional[FusedConv]:
         """Each source is (buffer, upsample flag); `pre` spans the concatenated channels.  An affine source is read from the
         pre-transformed view its producer maintains, else the gather stage applies the pre-op.  `cin_pad` zero input channels
-        are appended to the weight; `epilogue` = "relu" writes relu(out) to the destination."""
+        are appended to the weight; `epilogue` = "relu" writes relu(out) to the destination.  `window` = (c0, c1): the launch
+        reads channels [c0, c1) of its single plain source (the spec holds that channel slice of the buffer)."""
         if stack_src is not None:            # rows are b*N + i (reference sige/cuda/gather_kernel.cu:30)
             B = dst.shape[0] if (dst is not None and idx is not None) else 1
             n = int(stack_src.shape[0]) // B
@@ -981,10 +1010,11 @@ class Lowering:
                 s.scale = None if pre.scale is None else pre.scale.contiguous()
                 s.shift = None if pre.shift is None else pre.shift.contiguous()
                 s.per_sample_affine = self._per_sample(pre)
-                gamma, beta, slope = pre.mod
+                (gamma, g0), (beta, b0), slope = pre.mod
                 for b_ in (gamma, beta):
                     b_.readers.append((idx, block, 0, tile_img))
-                s.modulation = (gamma.raw, beta.raw, slope)
+                cin = sum(b_.shape[1] for b_, _ in segs)
+                s.modulation = (_channels(gamma.raw, g0, cin), _channels(beta.raw, b0, cin), slope)
             elif pre is not None and (pre.scale is not None or pre.shift is not None or pre.act):
                 per_sample = (pre.scale is not None and pre.scale.dim() == 2) or (pre.shift is not None and pre.shift.dim() == 2)
                 views, c0 = [], 0
@@ -1006,6 +1036,9 @@ class Lowering:
                     tensors = views
             else:
                 tensors = [b_.raw for (b_, _) in segs]
+                if window is not None:
+                    assert len(segs) == 1, name
+                    tensors = [_channels(tensors[0], window[0], window[1] - window[0])]
             for (b_, up_) in segs:
                 b_.readers.append((idx, block, up_, tile_img))
             s.srcs = [(t, up) for t, (_, up) in zip(tensors, segs)]
@@ -1115,7 +1148,7 @@ class Lowering:
             pre = Pre(self._chan_vec(st.scale, st.src), self._chan_vec(st.shift, st.src), None if g.activation_name == "identity" else g.activation_name)
         if isinstance(st, ModStack):
             pre = pre or Pre()
-            pre.mod = (st.gamma, st.beta, st.slope)
+            pre.mod = ((st.gamma, st.gamma_c0), (st.beta, st.beta_c0), st.slope)
         timg = getattr(g, "tile_images", None)
         if timg is None and int(g.active_indices.shape[0]) > 0 and not exact:
             idx = self.slot(g).buf            # fixed capacity, padded with SIGE_TILE_NONE (see IdxSlot)
@@ -1278,7 +1311,7 @@ class Lowering:
         ro = (block - co.k) // co.stride + 1
         out = torch.empty((B * n, int(co.weight.shape[0]), ro, ro), dtype=self.dtype, device=self.dev, memory_format=torch.channels_last)
         self.emit_conv("n%d.conv_stack" % co.node.index, segs, pre, hw, idx, block, co.weight, co.bias, co.stride, off, None, stack_src=stack_src, dst_stack=out,
-                       cin_pad=co.cin_pad, epilogue=co.act)
+                       cin_pad=co.cin_pad, epilogue=co.act, window=self._window_of(co))
         self.env[id(lt)] = RealStack(out)
         return out
 
@@ -1463,7 +1496,7 @@ class Lowering:
                 return True
             return False
         if isinstance(v, (Stack, RealStack)):
-            src_c = v.src.C if isinstance(v, Stack) else int(v.tensor.shape[1])
+            src_c = v.C if isinstance(v, WinStack) else (v.src.C if isinstance(v, Stack) else int(v.tensor.shape[1]))
             nsegs = len(v.src.segs) if isinstance(v, Stack) else 1
             if p != 0 or cout % 8 != 0 or not (cin % 64 == 0 or self._narrow(cin, src_c, nsegs, cout, k, s)):
                 return False
@@ -1555,6 +1588,8 @@ class Lowering:
         if self._separable_conv(node, m, x):
             return True
         mod = self._modulated(x, m.weight, m.stride)
+        if mod is None:
+            mod = self._windowed(x, m.weight, m.stride)
         if mod is None and not isinstance(self.sym(x), (Stack, RealStack)) and x.dim() == 4:      # SIGEConv2d in sparse mode always sees a tile stack
             t = self.runtime_tensor(x)
             if not t.is_contiguous(memory_format=torch.channels_last):
@@ -1568,27 +1603,74 @@ class Lowering:
         """The source of a conv that reads SPADE's modulation `leaky((x*scale+shift) * (1 + gamma) + beta)` (Spade stage 3) of three lazy
         Stacks of single buffers cut with ONE tile list (reference gaugan/models/sige_normalization.py:84-86: x from the block's
         Gather with the batch norm folded in, gamma / beta re-gathered from the separable launches' buffers), when the executor
-        runs such launches; None otherwise (the modulation is then evaluated on its own)."""
+        runs such launches; None otherwise (the modulation is then evaluated on its own).  When the executor also runs strided
+        launches, gamma and beta may be torch.split windows of one such Stack (the full SPADE's `gamma, beta = torch.split(
+        gamma_beta, norm_nc)`, reference gaugan/models/sige_normalization.py:80)."""
         ok = getattr(self.ex, "modulated_conv_supported", None)
         v = self.sym(x) if isinstance(x, LazyTensor) else None
         if ok is None or not isinstance(v, Spade) or v.stage != 3 or (v.slope is not None and not math.isfinite(v.slope)):
             return None
-        sx, sg, sb = self.sym(v.x), self.sym(v.gamma), self.sym(v.beta)
-        if not all(isinstance(t, Stack) and not isinstance(t, ModStack) for t in (sx, sg, sb)):
+        sx = self.sym(v.x)
+        if not isinstance(sx, Stack) or isinstance(sx, (ModStack, WinStack)):
             return None
         g, f = sx.gather, sx.src
         if (getattr(g, "tile_images", None) is not None or g.activation_name != "identity" or g.block_size[0] != g.block_size[1]
                 or int(g.active_indices.shape[0]) == 0 or not f.plain or len(f.segs) != 1):
             return None
-        shape = (f.B, f.C, *f.HW)
-        for t in (sg, sb):
-            if (t.src.single is None or t.scale is not None or t.shift is not None or t.gather.activation_name != "identity"
-                    or not self._same_gather(t.gather, g) or t.src.single.shape != shape):
+        windows = getattr(self.ex, "strided_conv_supported", None) is not None
+        parts = []
+        for lt in (v.gamma, v.beta):
+            t = self.sym(lt)
+            if isinstance(t, Stack) and not isinstance(t, (ModStack, WinStack)):
+                win = (t, 0, t.src.C)
+            elif t is None and windows and isinstance(lt, LazyTensor):
+                win = self._stack_window(lt)
+            else:
                 return None
+            if win is None:
+                return None
+            t, c0, C = win
+            buf = t.src.single
+            if (buf is None or t.scale is not None or t.shift is not None or t.gather.activation_name != "identity"
+                    or not self._same_gather(t.gather, g) or (buf.shape[0], *buf.shape[2:]) != (f.B, *f.HW) or C != f.C or c0 % 8):
+                return None
+            parts.append((buf, c0))
         k, s = _pair(weight.shape[2:]), _pair(stride)
         if k[0] != k[1] or s[0] != s[1] or not ok(f.C, int(weight.shape[0]), k[0], s[0]):
             return None
-        return ModStack(sx, sg.src.single, sb.src.single, 1.0 if v.slope is None else float(v.slope))
+        (gb, g0), (bb, b0) = parts
+        return ModStack(sx, gb, bb, 1.0 if v.slope is None else float(v.slope), gamma_c0=g0, beta_c0=b0)
+
+    def _stack_window(self, lt: LazyTensor) -> Optional[Tuple[Stack, int, int]]:
+        """(Stack, first channel, channels) of a torch.split part along dim 1 of a lazy Stack that has no other symbolic form (SPADE's
+        actv_0 / actv_1 / actv_s, and gamma / beta of gamma_beta); None otherwise."""
+        if self.sym(lt) is not None or lt.node is None or lt.node.name != "split":
+            return None
+        a = self._bind(lt.node, ("tensor", "split_size_or_sections", "dim"), {"dim": 0})
+        st = self.sym(a["tensor"]) if isinstance(a["tensor"], LazyTensor) else None
+        if not (isinstance(st, Stack) and not isinstance(st, (ModStack, WinStack)) and a["dim"] == 1
+                and isinstance(a["split_size_or_sections"], int)):
+            return None
+        return st, lt.slot * a["split_size_or_sections"], int(lt.shape[1])
+
+    def _windowed(self, x, weight, stride) -> Optional[WinStack]:
+        """The source of a conv on a torch.split window of a lazy Stack of one buffer (no pre-op), read in place by a strided
+        launch when the executor runs such launches; None otherwise (the split is then evaluated on its own)."""
+        ok = getattr(self.ex, "strided_conv_supported", None)
+        if ok is None or not isinstance(x, LazyTensor):
+            return None
+        win = self._stack_window(x)
+        if win is None:
+            return None
+        st, c0, C = win
+        g = st.gather
+        if (st.src.single is None or st.scale is not None or st.shift is not None or g.activation_name != "identity"
+                or g.block_size[0] != g.block_size[1] or getattr(g, "tile_images", None) is not None or c0 % 8 or C % 8):
+            return None
+        k, s = _pair(weight.shape[2:]), _pair(stride)
+        if k[0] != k[1] or s[0] != s[1] or not ok(C, int(weight.shape[0]), k[0], s[0]):
+            return None
+        return WinStack(st, c0, C)
 
     # ---- GAN Compression's separable conv: depthwise 3x3 -> per-channel affine -> 1x1, one launch per SPADE layer
     def _separable_conv(self, node: Node, m, x) -> bool:
@@ -1621,13 +1703,11 @@ class Lowering:
         SIGEConv2d in sparse mode only ever reads tile stacks, so a 6x6 "image" here is one.)"""
         v = self.sym(x)
         c0 = 0
-        if v is None and x.node is not None and x.node.name == "split":
+        win = self._stack_window(x)
+        if win is not None:
             # torch.split of the lazy re-gather of a buffer a fused launch wrote (actvs after a fused mlp_shared): the window is
             # read in place through the tile list
-            a = self._bind(x.node, ("tensor", "split_size_or_sections", "dim"), {"dim": 0})
-            st = self.sym(a["tensor"]) if isinstance(a["tensor"], LazyTensor) else None
-            if isinstance(st, Stack) and a["dim"] == 1 and isinstance(a["split_size_or_sections"], int):
-                v, c0 = st, x.slot * a["split_size_or_sections"]
+            v, c0 = win[0], win[1]
         if v is None and x.node is not None:
             self.runtime_tensor(x)               # a stack from a call the lowering does not know (the eager scatter_gather)
             v = self.sym(x)
@@ -1737,7 +1817,11 @@ class Lowering:
         if stack_src is not None and gather is not None:      # a materialised stack scattered through `gather`'s tile set
             idx, off = gather.active_indices.to(self.dev), int(gather.offset[0])
         self.emit_conv(name or ("n%d" % node.index), segs, pre, hw, idx, block, co.weight, co.bias, co.stride, off, dst, residual=residual,
-                       shortcut=shortcut, stack_src=stack_src, tile_img=timg, cin_pad=co.cin_pad, epilogue=co.act)
+                       shortcut=shortcut, stack_src=stack_src, tile_img=timg, cin_pad=co.cin_pad, epilogue=co.act, window=self._window_of(co))
+
+    @staticmethod
+    def _window_of(co: ConvOut) -> Optional[Tuple[int, int]]:
+        return (co.src.c0, co.src.c0 + co.src.C) if isinstance(co.src, WinStack) else None
 
     def _module_name(self, node: Node) -> str:
         return self.module_names.get(id(node.module), "n%d" % node.index)
@@ -1828,7 +1912,8 @@ class Lowering:
         # reference gaugan/models/spade_generators/sige_fused_spade_generator.py:160-198 — such a launch scatters through the
         # module's own tile sets and always takes the un-fused form below)
         main_real, sc_real = isinstance(co.src, RealStack), isinstance(sc.src, RealStack)
-        modulated = isinstance(co.src, ModStack) or isinstance(sc.src, ModStack)     # (the fused shortcut reads its source raw)
+        # (the fused shortcut reads its source raw and whole)
+        modulated = isinstance(co.src, (ModStack, WinStack)) or isinstance(sc.src, (ModStack, WinStack))
         if not ((isinstance(co.src, Stack) or main_real) and (isinstance(sc.src, Stack) or sc_real)):
             return False
         mg, sg = m.main_gather.module, m.shortcut_gather.module

@@ -350,6 +350,12 @@ def tile_conv_modulated_supported(cin: int, cout: int, k: int, stride: int, dtyp
     return code is not None and bool(_cabi.lib().sige_tile_conv_modulated_supported(int(cin), int(cout), int(k), int(stride), code))
 
 
+def tile_conv_strided_supported(cin: int, cout: int, k: int, stride: int, dtype: torch.dtype) -> bool:
+    """Does ``sige_tile_conv_strided`` take a conv whose single source is a `cin`-channel window of a wider buffer?  (The window is
+    a multiple of 8 channels, like its offset and the buffer's width; one of 64 is the plain tensor-core launch, else the narrow one.)"""
+    return dtype in (torch.float16, torch.bfloat16) and cin > 0 and cin % 8 == 0 and cout > 0 and cout % 8 == 0 and k >= 1 and stride >= 1
+
+
 def tile_conv_descriptor() -> TileConv:
     return TileConv()
 
@@ -359,20 +365,39 @@ def launch_tile_conv(desc: TileConv, stream: int) -> None:
     _bump()
 
 
+def channel_window(t: torch.Tensor) -> Tuple[int, int, int]:
+    """(address of channel 0 of pixel 0, channels per pixel, first channel) of a [B, C, H, W] tensor that is a whole channels-last
+    buffer or a channel slice of one (``buf[:, c0:c1]``, a torch.split part)."""
+    if t.dim() != 4 or t.stride(1) != 1:
+        raise ValueError("channel_window: not a channel window of a channels-last 4-D tensor")
+    B, C, H, W = (int(d) for d in t.shape)
+    pitch = int(t.stride(3)) if W > 1 else (int(t.stride(2)) if H > 1 else C)
+    if pitch < C or (H > 1 and t.stride(2) != W * pitch) or (B > 1 and t.stride(0) != H * W * pitch):
+        raise ValueError("channel_window: pixels are not evenly spaced")
+    c0 = int(t.storage_offset()) % pitch
+    return t.data_ptr() - c0 * t.element_size(), pitch, c0
+
+
 def conv_modulation(gamma: torch.Tensor, beta: torch.Tensor, negative_slope: float, gamma_c0: int = 0, beta_c0: int = 0) -> "_cabi.ConvModulation":
-    """sige_conv_modulation_t of channels-last [B, C, H, W] gamma / beta buffers (read from channel gamma_c0 / beta_c0 on)."""
-    for name, t in (("gamma", gamma), ("beta", beta)):
-        if t.dim() != 4 or not t.is_contiguous(memory_format=torch.channels_last):
-            raise ValueError("conv_modulation: %s must be a channels-last 4-D tensor" % name)
+    """sige_conv_modulation_t of [B, C, H, W] gamma / beta read from channel gamma_c0 / beta_c0 on: channels-last buffers or channel
+    windows of such buffers (the two torch.split halves of SPADE's gamma_beta, one buffer)."""
     m = _cabi.ConvModulation()
-    m.gamma, m.gamma_C, m.gamma_c0 = gamma.data_ptr(), int(gamma.shape[1]), int(gamma_c0)
-    m.beta, m.beta_C, m.beta_c0 = beta.data_ptr(), int(beta.shape[1]), int(beta_c0)
+    g, gC, gc0 = channel_window(gamma)
+    b, bC, bc0 = channel_window(beta)
+    m.gamma, m.gamma_C, m.gamma_c0 = g, gC, gc0 + int(gamma_c0)
+    m.beta, m.beta_C, m.beta_c0 = b, bC, bc0 + int(beta_c0)
     m.negative_slope = float(negative_slope)
     return m
 
 
 def launch_tile_conv_modulated(desc: TileConv, mod: "_cabi.ConvModulation", stream: int) -> None:
     _cabi.check(_cabi.lib().sige_tile_conv_modulated(byref(desc), byref(mod), stream), "sige_tile_conv_modulated")
+    _bump()
+
+
+def launch_tile_conv_strided(desc: TileConv, src_pixel_stride: int, stream: int) -> None:
+    """sige_tile_conv_strided: the single source is a channel window of a buffer with `src_pixel_stride` channels per pixel."""
+    _cabi.check(_cabi.lib().sige_tile_conv_strided(byref(desc), int(src_pixel_stride), stream), "sige_tile_conv_strided")
     _bump()
 
 

@@ -1,16 +1,21 @@
-"""Time the sparse step of GauGAN compressed with GAN Compression (the sub-mobile SPADE generator) on one GPU.
+"""Time the sparse step of a GauGAN generator on one GPU: GauGAN compressed with GAN Compression (the sub-mobile SPADE generator,
+the default) or the full SPADE generator.
 
-    python tools/bench_gaugan_gc.py [--steps 50] [--warmup 10] [--dtype fp16|bf16] [--size full|mini] [--headroom 0.5] [--dump-outputs DIR]
+    python tools/bench_gaugan_gc.py [--generator gc|spade] [--steps 50] [--warmup 10] [--dtype fp16|bf16] [--size full|mini]
+                                    [--headroom 0.5] [--dump-outputs DIR] [--per-launch]
 
-Workload: sige_b200/workloads/gaugan_gc.py at full size — 512 x 1024 label map, config 32_32_32_48_32_24_24_32 (the published
-GAN Compression Cityscapes sub-network), 5 sparse blocks, the 2.98 % label edit of the full-size GauGAN workload; fp32 model and
-dense pass, sparse step as a fused fp16 step (`set_fused(True, dtype=torch.float16)`) in one CUDA graph.  As bench.py: warm-up,
+Workload (--generator gc): sige_b200/workloads/gaugan_gc.py at full size — 512 x 1024 label map, config 32_32_32_48_32_24_24_32 (the
+published GAN Compression Cityscapes sub-network), 5 sparse blocks, the 2.98 % label edit of the full-size GauGAN workload.
+--generator spade: sige_b200/workloads/gaugan_spade.py (ngf 64, `more` up-sampling layers, 5 sparse blocks) on the same label maps
+and edit.  Either way: fp32 model and dense pass, sparse step as a fused fp16 step (`set_fused(True, dtype=torch.float16)`) in one
+CUDA graph.  As bench.py: warm-up,
 per-step CUDA events around `model(x)`, an L2 flush (256 MiB write) between steps outside the events, GPU name / power limit /
 SM clock read in the same run, the launch mix of the compiled step, and --dump-outputs DIR (the last timed step's output as
 float32 .npy).  The step is compiled with --headroom (extra tile-list capacity); after the timed steps the next-edit figure is
 the wall time from `set_masks_async` of a second, smaller label edit to the synchronised end of the step that follows it (an
 interactive user's next stroke), taken three times alternating with the first edit; `next_edit_in_place` says whether the
-compiled step took the edit without recompiling.  Prints one JSON line.
+compiled step took the edit without recompiling.  --per-launch adds the CUDA-event time of every tile-conv launch of the compiled
+step, each after an L2 flush (launch latency included).  Prints one JSON line.
 """
 from __future__ import annotations
 
@@ -84,6 +89,7 @@ def next_edit(net, x_a, dilate_mask, downsample_mask, size: str, dev):
 
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
+    ap.add_argument("--generator", choices=["gc", "spade"], default="gc", help="sub-mobile (GAN Compression) or full SPADE generator")
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=10)
     ap.add_argument("--dtype", choices=["fp16", "bf16"], default="fp16")
@@ -91,6 +97,7 @@ def main():
     ap.add_argument("--no-flush", action="store_true", help="do not flush L2 between timed steps")
     ap.add_argument("--headroom", type=float, default=0.5, help="extra tile-list capacity of the compiled step")
     ap.add_argument("--dump-outputs", metavar="DIR", default=None)
+    ap.add_argument("--per-launch", action="store_true", help="time every tile-conv launch of the compiled step on its own")
     args = ap.parse_args()
 
     import numpy as np
@@ -105,7 +112,12 @@ def main():
     torch.cuda.set_device(0)
     dtype = torch.float16 if args.dtype == "fp16" else torch.bfloat16
     torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
-    net = G.build_gaugan_gc(args.size).to(dev)
+    if args.generator == "spade":
+        from sige_b200.workloads.gaugan_spade import build_gaugan_spade
+
+        net = build_gaugan_spade(args.size).to(dev)
+    else:
+        net = G.build_gaugan_gc(args.size).to(dev)
     t0 = time.time()
     G.run_gaugan_gc(net, downsample_mask, dilate_mask, device=dev, size=args.size,
                     fused=lambda n: n.set_fused(True, dtype=dtype, headroom=args.headroom))
@@ -134,11 +146,29 @@ def main():
     if args.dump_outputs:
         os.makedirs(args.dump_outputs, exist_ok=True)
         np.save(os.path.join(args.dump_outputs, "out.npy"), out.float().cpu().numpy())
+    per_launch = None
+    if args.per_launch:
+        stream = torch.cuda.current_stream(dev)
+        per_launch = []
+        with torch.no_grad():
+            for f in step.fused:
+                evs = []
+                for i in range(10):
+                    if flush is not None:
+                        flush.fill_(i)
+                    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    a.record(stream)
+                    f.launch(stream.cuda_stream)
+                    b.record(stream)
+                    evs.append((a, b))
+                torch.cuda.synchronize()
+                per_launch.append({"launch": f.name, "us": 1e3 * float(np.median([a.elapsed_time(b) for a, b in evs])),
+                                   "modulated": f.spec.modulation is not None, "Cin": f.spec.Cin, "Cout": f.spec.Cout, "k": f.spec.k})
     next_edit_s, in_place = next_edit(net, x, dilate_mask, downsample_mask, args.size, dev)
     kinds = Counter(k for k, _ in step.steps) if step is not None else Counter()
     low = step.low if step is not None else None
     line = {
-        "metric": "gaugan-gc %s sparse step" % args.size, "ms_per_step": float(np.median(ms)), "ms_mean": float(np.mean(ms)),
+        "metric": "gaugan-%s %s sparse step" % (args.generator, args.size), "generator": args.generator, "ms_per_step": float(np.median(ms)), "ms_mean": float(np.mean(ms)),
         "ms_min": float(np.min(ms)), "ms_max": float(np.max(ms)), "steps": len(ms), "warmup": args.warmup,
         "dtype": args.dtype, "l2": "not flushed" if flush is None else "flushed (256 MiB write) between timed steps",
         "gpu": info, "sm_mhz_before_timing": info_before.get("sm_mhz"), "compile_seconds": compile_s,
@@ -150,6 +180,8 @@ def main():
         "eager_node_kinds": dict(Counter(step.eager_nodes).most_common(8)) if step else None,
         "separable_branches": [len(r.branches) for r in getattr(low, "separable", [])] if low is not None else None,
     }
+    if per_launch is not None:
+        line["per_launch"] = per_launch
     print(json.dumps(line), flush=True)
 
 
