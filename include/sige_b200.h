@@ -267,7 +267,9 @@ typedef struct {
 } sige_conv_modulation_t;
 /* Host-only: does sige_tile_conv_modulated take a conv of Cin -> Cout, k x k, this stride, in `dtype`? */
 int sige_tile_conv_modulated_supported(int Cin, int Cout, int k, int stride, int dtype);
-/* sige_tile_conv whose pre-op is followed by the modulation above; always the mma.sync kernel (SIGE_CONV_TC5 is ignored).
+/* sige_tile_conv whose pre-op is followed by the modulation above.  With SIGE_CONV_TC5, the stride-1 wgmma geometries (3x3 on 6x6
+ * tiles, 1x1 on 4x4 tiles, Cin and Cout multiples of 64) run on the wgmma kernel with the same plan as sige_tile_conv; everything
+ * else (narrow Cin, other Cout, stride 2, no flag) runs on the mma.sync kernel.  Both stage the same operand.
  * Refused before any CUDA call: n_src != 1, a stack source, act != SIGE_ACT_IDENTITY (negative_slope is the activation), a fused
  * shortcut, idx_per_image, gamma / beta windows that overrun their buffer or are not multiples of 8 elements, pointers that are
  * not 16-byte aligned, a non-finite slope.  Everything else is sige_tile_conv's contract; N == 0 is a no-op. */
@@ -312,6 +314,8 @@ typedef struct {
     int grid_x, grid_y, grid_z;
 } sige_tile_conv_plan_t;
 int sige_tile_conv_plan(const sige_tile_conv_t *desc, sige_tile_conv_plan_t *plan);
+/* The same for sige_tile_conv_modulated (the kernel and grid it would use for this descriptor), host-only. */
+int sige_tile_conv_modulated_plan(const sige_tile_conv_t *desc, sige_tile_conv_plan_t *plan);
 
 /* 3x3 / stride 1 / pad 1 convolution with Cin <= 4 (the RGB stem): x NHWC (B,H,W,Cin), w OIHW, out NHWC;
  * up to two extra outputs aux[i] = act(out*scale+shift) (NHWC, Cout channels). */

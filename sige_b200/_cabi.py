@@ -128,6 +128,7 @@ PROTOTYPES = {
     "sige_resblock": (_I, [POINTER(TileConv), POINTER(TileConv), _P]),
     "sige_tile_conv_generic": (_I, [_P, _P, _P, _P] + [_I] * 14 + [_P]),
     "sige_tile_conv_plan": (_I, [_P, _P]),
+    "sige_tile_conv_modulated_plan": (_I, [_P, _P]),
     "sige_conv_in_nhwc": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
     "sige_conv_in_nhwc_tiles": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _I, _I, _I, _I, _I, _P, _P]),
     "sige_group_norm_fold_workspace": (_I, [_I, _I]),

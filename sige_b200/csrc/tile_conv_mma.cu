@@ -25,6 +25,9 @@
 // halo path: leaky((x*scale + shift) * (1 + gamma) + beta) with gamma / beta read at the halo pixel, so
 // the modulated tile stack the reference gathers and modulates with pointwise torch calls never exists.
 //
+// With SIGE_CONV_TC5, modulated launches of the wgmma geometries run the wgmma kernel's MOD instantiations (tile_conv_tc5.cu), which
+// stage the same operand.
+//
 // Tensor-core instruction: mma.sync.m16n8k16 (HMMA on sm_90a).  The wgmma/TMA variant
 // for large edit ratios lives in tile_conv_tc5.cu (when built); this kernel is the latency-
 // oriented path used when the GEMM M dimension is a few hundred rows.
@@ -484,7 +487,8 @@ template <typename T, bool MOD> static int launch_tile_conv(ConvParams &p, cudaS
 }
 
 bool tc5_supported(const sige_tile_conv_t *a, int pitch0);
-int tc5_launch(const sige_tile_conv_t *a, int pitch0, cudaStream_t st);
+bool tc5_supported_modulated(const sige_tile_conv_t *a);
+int tc5_launch(const sige_tile_conv_t *a, int pitch0, const sige_conv_modulation_t *m, cudaStream_t st);
 
 // Argument checks and launch of sige_tile_conv; m != nullptr: sige_tile_conv_modulated, pitch0 > 0: sige_tile_conv_strided (whose
 // own refusals come first).  pitch0 = elements per pixel of the single source (0: its channel count).
@@ -560,8 +564,9 @@ static int tile_conv(const sige_tile_conv_t *a, const sige_conv_modulation_t *m,
         SIGE_REQUIRE((a->flags & SIGE_CONV_TC5) && tc5_supported(a, 0), "sige_tile_conv: the fused shortcut is implemented by the wgmma kernel only (3x3 stride-1 on 6x6 tiles, SIGE_CONV_TC5)");
         SIGE_REQUIRE(a->sc_flags == nullptr || a->residual != nullptr, "sige_tile_conv: sc_flags given without the cached shortcut (residual)");
     }
-    // Hopper-native path (wgmma + TMA, tile_conv_tc5.cu) when requested and the geometry fits
-    if (!m && (a->flags & SIGE_CONV_TC5) && tc5_supported(a, pitch0)) return tc5_launch(a, pitch0, (cudaStream_t)stream);
+    // Hopper-native path (wgmma + TMA, tile_conv_tc5.cu) when requested and the geometry fits; a modulated launch takes its MOD
+    // instantiations on the stride-1 geometries
+    if ((a->flags & SIGE_CONV_TC5) && (m ? tc5_supported_modulated(a) : tc5_supported(a, pitch0))) return tc5_launch(a, pitch0, m, (cudaStream_t)stream);
 
     ConvParams p;
     p.seg[0] = ConvSeg{a->src[0].ptr, pitch0 > 0 ? pitch0 : a->src[0].C, a->src[0].up};

@@ -99,7 +99,14 @@ struct Params {
     int ksplit;
     int pdl;                   // launched with programmatic dependent launch: the next layer is released at the epilogue
     int is_bf16;
+    // SPADE modulation in the gather stage (MOD instantiations only, sige_tile_conv_modulated): gamma / beta are NHWC at the logical
+    // source extent with gC / bC elements per pixel, each pointing at the first channel of its window (sige_conv_modulation_t's c0);
+    // slope is the leaky-ReLU slope.  The fields take the padding before `trace` and the tail up to the tensor maps' 64-byte-aligned
+    // parameter offset, so every other field and both tensor maps keep their offsets.
+    float slope;
     long long *trace;          // development aid: per-CTA clock stamps (16 slots), or nullptr
+    const void *gamma, *beta;
+    int gC, bC;
 };
 
 template <int BN, int TAPS, bool DEEP = false, bool S2 = false, bool DB = false> struct Cfg {
@@ -341,12 +348,14 @@ __host__ __device__ __forceinline__ int k_slice(int J, int kr, int ks) { return 
 
 // ASYNC: the gather is a pure copy (no pre-op: the producer of the source already applied it) and is done with cp.async.
 // DB: the double-buffered split-K layout (Cfg).
-template <typename T, int BN, int TAPS, bool DEEP, bool ASYNC, bool S2 = false, bool DB = false>
+// MOD: the register-staged gather applies SPADE's modulation after the pre-op (see Params::gamma); the source is a full tensor.
+template <typename T, int BN, int TAPS, bool DEEP, bool ASYNC, bool S2 = false, bool DB = false, bool MOD = false>
 __global__ void __launch_bounds__(NTHREADS, 1)
 tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ CUtensorMap wmap,
                      const __grid_constant__ CUtensorMap wmap2) {
     using C = Cfg<BN, TAPS, DEEP, S2, DB>;
     static_assert(!S2 || ASYNC, "stride-2 geometry: pure-copy (cp.async) gather only");
+    static_assert(!MOD || !ASYNC, "modulated gather: register-staged only");
     constexpr int NSTB = C::NSTB, TPS = C::TPS, SPC = C::SPC, NAB = C::NAB;
     constexpr int TILES = C::CT;                      // (shadows the namespace constant: 32 for the stride-2 geometry)
     constexpr int A_COPY_BYTES = C::A_COPY, A_BUF_BYTES = C::A_BUF;
@@ -676,7 +685,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
                 }
             }
         };
-        const bool pre = (p.scale != nullptr) || (p.shift != nullptr) || (p.act != SIGE_ACT_IDENTITY);
+        const bool pre = MOD || (p.scale != nullptr) || (p.shift != nullptr) || (p.act != SIGE_ACT_IDENTITY);
         auto store = [&](int c, unsigned char *abuf) {
 #pragma unroll
             for (int k = 0; k < LOADS; ++k) {
@@ -700,11 +709,27 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
                         const float4 a = __ldg(s4), b = __ldg(s4 + 1);
                         sh[0] = a.x; sh[1] = a.y; sh[2] = a.z; sh[3] = a.w; sh[4] = b.x; sh[5] = b.y; sh[6] = b.z; sh[7] = b.w;
                     }
+                    if constexpr (MOD) {
+                        // leaky((x*scale + shift) * (1 + gamma) + beta) at the halo pixel's LOGICAL coordinates (the source may be read
+                        // up-sampled), rounded once: the expression and order of the mma.sync MOD path, so the staged operand is the same
+                        const int tl = g_xyt[k] >> 8;
+                        const long long px = ((long long)ab_k * p.H + (((g_xyt[k] >> 4) & 15) + s_idx[2 * tl])) * p.W + ((g_xyt[k] & 15) + s_idx[2 * tl + 1]);
+                        const uint4 gr = __ldg(reinterpret_cast<const uint4 *>(reinterpret_cast<const T *>(p.gamma) + px * p.gC + ch));
+                        const uint4 br = __ldg(reinterpret_cast<const uint4 *>(reinterpret_cast<const T *>(p.beta) + px * p.bC + ch));
+                        const T *ge = reinterpret_cast<const T *>(&gr), *be = reinterpret_cast<const T *>(&br);
 #pragma unroll
-                    for (int z = 0; z < 8; ++z) {
-                        float f = fmaf(DT<T>::to_f(e[z]), sc[z], sh[z]);
-                        f = activate<true>(p.act, f);
-                        e[z] = DT<T>::from_f(f);
+                        for (int z = 0; z < 8; ++z) {
+                            float f = fmaf(DT<T>::to_f(e[z]), sc[z], sh[z]);
+                            f = fmaf(f, 1.f + DT<T>::to_f(ge[z]), DT<T>::to_f(be[z]));
+                            e[z] = DT<T>::from_f(f < 0.f ? f * p.slope : f);
+                        }
+                    } else {
+#pragma unroll
+                        for (int z = 0; z < 8; ++z) {
+                            float f = fmaf(DT<T>::to_f(e[z]), sc[z], sh[z]);
+                            f = activate<true>(p.act, f);
+                            e[z] = DT<T>::from_f(f);
+                        }
                     }
                 }
                 const int x = g_xyt[k] & 15, y = (g_xyt[k] >> 4) & 15, tl = g_xyt[k] >> 8;
@@ -1098,7 +1123,7 @@ static Plan decide(long long NT, int Cin, int Cout, int taps, int Cin2, int kspl
     return pl;
 }
 
-template <typename T, int BN, int TAPS, bool DEEP, bool ASYNC, bool S2 = false, bool DB = false>
+template <typename T, int BN, int TAPS, bool DEEP, bool ASYNC, bool S2 = false, bool DB = false, bool MOD = false>
 static int launch_v(Params &p, const void *w_packed, const void *w2_packed, cudaStream_t st) {
     using C = Cfg<BN, TAPS, DEEP, S2, DB>;
     EncodeTiledFn enc = encode_fn();
@@ -1129,7 +1154,7 @@ static int launch_v(Params &p, const void *w_packed, const void *w2_packed, cuda
             return 2;
         }
     }
-    auto kern = tile_conv_tc5_kernel<T, BN, TAPS, DEEP, ASYNC, S2, DB>;
+    auto kern = tile_conv_tc5_kernel<T, BN, TAPS, DEEP, ASYNC, S2, DB, MOD>;
     static int attr_dev = -1;
     int dev = 0;
     cudaGetDevice(&dev);
@@ -1151,9 +1176,10 @@ static int launch_v(Params &p, const void *w_packed, const void *w2_packed, cuda
     return 0;
 }
 
-// pure-copy gathers (no pre-op in the gather stage) take the cp.async variant
+// pure-copy gathers (no pre-op in the gather stage) take the cp.async variant; modulated ones the register-staged MOD variant
 template <typename T, int BN, int TAPS, bool DEEP = false, bool DB = false>
 static int launch(Params &p, const void *w_packed, const void *w2_packed, cudaStream_t st) {
+    if (p.gamma) return launch_v<T, BN, TAPS, DEEP, false, false, DB, true>(p, w_packed, w2_packed, st);
     const bool pure_copy = p.scale == nullptr && p.shift == nullptr && p.act == SIGE_ACT_IDENTITY;
     if (pure_copy) return launch_v<T, BN, TAPS, DEEP, true, false, DB>(p, w_packed, w2_packed, st);
     return launch_v<T, BN, TAPS, DEEP, false, false, DB>(p, w_packed, w2_packed, st);
@@ -1211,8 +1237,12 @@ bool tc5_supported(const sige_tile_conv_t *a, int pitch0) {
     return (g3 || g1) && a->Cout % 64 == 0 && a->Cin % 64 == 0 && (a->ksplit == 0 || a->ksplit == 1 || a->ksplit == 2 || a->ksplit == 4 || a->ksplit == 8);
 }
 
-// Arguments were validated by sige_tile_conv (tile_conv_mma.cu) before this is called.
-int tc5_launch(const sige_tile_conv_t *a, int pitch0, cudaStream_t st) {
+// ... and a modulated one (sige_tile_conv_modulated)?  The stride-1 geometries only: the stride-2 one has no register-staged gather.
+bool tc5_supported_modulated(const sige_tile_conv_t *a) { return a->stride == 1 && tc5_supported(a, 0); }
+
+// Arguments were validated by sige_tile_conv (tile_conv_mma.cu) before this is called; m != nullptr: a modulated launch
+// (tc5_supported_modulated).
+int tc5_launch(const sige_tile_conv_t *a, int pitch0, const sige_conv_modulation_t *m, cudaStream_t st) {
     tc5::Params p;
     p.seg[0] = tc5::Seg{a->src[0].ptr, pitch0 > 0 ? pitch0 : a->src[0].C, a->src[0].up};
     p.seg[1] = a->n_src == 2 ? tc5::Seg{a->src[1].ptr, a->src[1].C, a->src[1].up} : p.seg[0];
@@ -1246,7 +1276,13 @@ int tc5_launch(const sige_tile_conv_t *a, int pitch0, cudaStream_t st) {
     p.pdl = (a->flags & SIGE_CONV_PDL) ? 1 : 0;
     p.is_bf16 = a->dtype == SIGE_BF16;
     p.trace = g_trace;
-    const bool s2 = tc5_is_s2(a);
+    const size_t esz = 2;                                                  // f16 / bf16
+    p.gamma = m ? static_cast<const char *>(m->gamma) + (size_t)m->gamma_c0 * esz : nullptr;
+    p.beta = m ? static_cast<const char *>(m->beta) + (size_t)m->beta_c0 * esz : nullptr;
+    p.gC = m ? m->gamma_C : 0;
+    p.bC = m ? m->beta_C : 0;
+    p.slope = m ? m->negative_slope : 1.f;
+    const bool s2 = !m && tc5_is_s2(a);
     const tc5::Plan pl = tc5::decide(p.NT, p.Cin, p.Cout, p.taps, p.Cin2, a->ksplit, s2);
     p.ksplit = pl.ksplit;
     if (s2) {
@@ -1268,12 +1304,9 @@ int tc5_launch(const sige_tile_conv_t *a, int pitch0, cudaStream_t st) {
 
 }  // namespace sige
 
-// Which kernel and grid sige_tile_conv would use for this descriptor (no pointer is dereferenced, nothing is launched).
-extern "C" int sige_tile_conv_plan(const sige_tile_conv_t *a, sige_tile_conv_plan_t *out) {
+// The wgmma plan of a descriptor whose launch takes the wgmma kernel.
+static void tc5_plan(const sige_tile_conv_t *a, sige_tile_conv_plan_t *out) {
     using namespace sige;
-    SIGE_REQUIRE(a && out, "sige_tile_conv_plan: null pointer");
-    out->path = 0; out->bn = 0; out->ksplit = 0; out->deep_ring = 0; out->grid_x = out->grid_y = out->grid_z = 0;
-    if (!((a->flags & SIGE_CONV_TC5) && tc5_supported(a, 0))) return 0;      // mma.sync / CUDA-core paths
     const long long NT = (long long)a->B * a->N;
     const bool s2 = tc5_is_s2(a);
     const tc5::Plan pl = tc5::decide(NT, a->Cin, a->Cout, a->kH * a->kW, a->n_src2 > 0 ? a->Cin2 : 0, a->ksplit, s2);
@@ -1284,5 +1317,23 @@ extern "C" int sige_tile_conv_plan(const sige_tile_conv_t *a, sige_tile_conv_pla
     out->grid_x = ceil_div(NT, s2 ? tc5::S2_TILES : tc5::TILES);
     out->grid_y = a->Cout / pl.bn;
     out->grid_z = pl.ksplit;
+}
+
+// Which kernel and grid sige_tile_conv would use for this descriptor (no pointer is dereferenced, nothing is launched).
+extern "C" int sige_tile_conv_plan(const sige_tile_conv_t *a, sige_tile_conv_plan_t *out) {
+    using namespace sige;
+    SIGE_REQUIRE(a && out, "sige_tile_conv_plan: null pointer");
+    out->path = 0; out->bn = 0; out->ksplit = 0; out->deep_ring = 0; out->grid_x = out->grid_y = out->grid_z = 0;
+    if ((a->flags & SIGE_CONV_TC5) && tc5_supported(a, 0)) tc5_plan(a, out);      // else the mma.sync / CUDA-core paths
+    return 0;
+}
+
+// The same for sige_tile_conv_modulated: the wgmma kernel's MOD instantiations take the stride-1 wgmma geometries, everything else
+// runs on mma.sync.
+extern "C" int sige_tile_conv_modulated_plan(const sige_tile_conv_t *a, sige_tile_conv_plan_t *out) {
+    using namespace sige;
+    SIGE_REQUIRE(a && out, "sige_tile_conv_modulated_plan: null pointer");
+    out->path = 0; out->bn = 0; out->ksplit = 0; out->deep_ring = 0; out->grid_x = out->grid_y = out->grid_z = 0;
+    if ((a->flags & SIGE_CONV_TC5) && tc5_supported_modulated(a)) tc5_plan(a, out);
     return 0;
 }

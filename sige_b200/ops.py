@@ -345,7 +345,8 @@ def tile_conv_narrow_supported(cin: int, cout: int, k: int, stride: int, dtype: 
 
 
 def tile_conv_modulated_supported(cin: int, cout: int, k: int, stride: int, dtype: torch.dtype) -> bool:
-    """Does ``sige_tile_conv_modulated`` (SPADE's modulation in the gather stage, mma.sync kernel) take this conv?"""
+    """Does ``sige_tile_conv_modulated`` (SPADE's modulation in the gather stage) take this conv?  With the wgmma flag, the wgmma
+    kernel runs the stride-1 geometries whose Cin and Cout are multiples of 64; the mma.sync kernel runs the rest."""
     code = {torch.float16: _cabi.F16, torch.bfloat16: _cabi.BF16}.get(dtype)
     return code is not None and bool(_cabi.lib().sige_tile_conv_modulated_supported(int(cin), int(cout), int(k), int(stride), code))
 

@@ -144,22 +144,33 @@ def measure_engine(engine, flush, reps: int = 5):
     }
 
 
+def plan_of(fc):
+    """The launch plan (sige_tile_conv_plan_t) of a FusedConv: the kernel and grid its launch uses.  Modulated launches are planned by
+    sige_tile_conv_modulated_plan, which knows which of them run on the wgmma kernel."""
+    import ctypes
+
+    from . import _cabi
+
+    pl = _cabi.TileConvPlan()
+    query = _cabi.lib().sige_tile_conv_modulated_plan if fc.spec.modulation is not None else _cabi.lib().sige_tile_conv_plan
+    _cabi.check(query(ctypes.byref(fc.desc), ctypes.byref(pl)), "tile-conv plan")
+    return pl
+
+
+def kernel_name(pl) -> str:
+    """'wgmma bn=<BN> ksplit=<K>' or 'mma.sync' for a plan_of() result."""
+    return "wgmma bn=%d ksplit=%d" % (pl.bn, pl.ksplit) if pl.path == 1 else "mma.sync"
+
+
 def _traced_step(model, args, options):
     """A fused, graph-captured step whose wgmma launches stamp %globaltimer per CTA (16 slots each) into a device buffer:
     (step, plans, ctas, offs, buf) with offs[i] the first slot of launch i (ctas[i] == 0: not a wgmma launch)."""
-    import ctypes
-
     from . import _cabi
     from .fused import FusedConv, FusedStep
 
     lib = _cabi.lib()
     dev = args[0].device
     order = {}
-
-    def plan_of(fc):
-        pl = _cabi.TileConvPlan()
-        lib.sige_tile_conv_plan(ctypes.byref(fc.desc), ctypes.byref(pl))
-        return pl
 
     # pass 1 (no trace): learn the grids, size the trace buffer
     opts = dict(options)

@@ -15,7 +15,8 @@ float32 .npy).  The step is compiled with --headroom (extra tile-list capacity);
 the wall time from `set_masks_async` of a second, smaller label edit to the synchronised end of the step that follows it (an
 interactive user's next stroke), taken three times alternating with the first edit; `next_edit_in_place` says whether the
 compiled step took the edit without recompiling.  --per-launch adds the CUDA-event time of every tile-conv launch of the compiled
-step, each after an L2 flush (launch latency included).  Prints one JSON line.
+step, each after an L2 flush (launch latency included), and the kernel it runs (from its launch plan: `wgmma bn=.. ksplit=..` or
+`mma.sync`).  Prints one JSON line.
 """
 from __future__ import annotations
 
@@ -148,6 +149,8 @@ def main():
         np.save(os.path.join(args.dump_outputs, "out.npy"), out.float().cpu().numpy())
     per_launch = None
     if args.per_launch:
+        from sige_b200.roofline import kernel_name, plan_of
+
         stream = torch.cuda.current_stream(dev)
         per_launch = []
         with torch.no_grad():
@@ -163,7 +166,8 @@ def main():
                     evs.append((a, b))
                 torch.cuda.synchronize()
                 per_launch.append({"launch": f.name, "us": 1e3 * float(np.median([a.elapsed_time(b) for a, b in evs])),
-                                   "modulated": f.spec.modulation is not None, "Cin": f.spec.Cin, "Cout": f.spec.Cout, "k": f.spec.k})
+                                   "modulated": f.spec.modulation is not None, "Cin": f.spec.Cin, "Cout": f.spec.Cout, "k": f.spec.k,
+                                   "kernel": kernel_name(plan_of(f))})
     next_edit_s, in_place = next_edit(net, x, dilate_mask, downsample_mask, args.size, dev)
     kinds = Counter(k for k, _ in step.steps) if step is not None else Counter()
     low = step.low if step is not None else None
