@@ -304,14 +304,18 @@ int sige_tile_conv_generic(const void *x, const void *w, const void *bias, void 
 /*   :431-433 (norm_out -> swish -> conv_out), models/common.py:37-57 (fold)   */
 /* ------------------------------------------------------------------------- */
 /* Launch plan sige_tile_conv would use for a descriptor: pure host logic (no pointer is dereferenced, nothing is
- * launched) — exported so that the tile-width / split-K / ring heuristics can be tested without a GPU. */
+ * launched) — exported so that the tile-width / split-K / ring heuristics can be tested without a GPU (which then plan
+ * for 132 SMs).  path 0 with every other field 0: the mma.sync kernel would not take the descriptor either (fp32, a tile
+ * that fits no CTA configuration, a ksplit that is not a cluster size, ...). */
 typedef struct {
-    int path;      /* 1 = wgmma kernel, 0 = mma.sync kernel (the fields below are then 0) */
-    int bn;        /* output channels per CTA (64 or 128) */
+    int path;      /* 1 = wgmma kernel, 0 = mma.sync kernel */
+    int bn;        /* output channels per CTA (64 or 128); mma.sync: 128 = the L configuration (128 GEMM rows), 64 = M (64
+                      rows) or S (32 rows), each packing min(rows / (Ro*So), halo pixels / (R*S)) tiles per CTA, halo 288 /
+                      144 / 72 pixels: grid_x = ceil(B*N / tiles per CTA) tells M from S */
     int ksplit;    /* K slices = thread-block cluster size (1, 2, 4, 8) */
     int deep_ring; /* 1 = the split-K layout of the narrow 3x3 configuration: one halo buffer + five weight stages when every
                       K slice needs one halo fill, else two halo buffers + two weight stages fed from L2 */
-    int grid_x, grid_y, grid_z;
+    int grid_x, grid_y, grid_z;   /* mma.sync: ceil(B*N / tiles per CTA), ceil(Cout / bn), ksplit; deep_ring 0 */
 } sige_tile_conv_plan_t;
 int sige_tile_conv_plan(const sige_tile_conv_t *desc, sige_tile_conv_plan_t *plan);
 /* The same for sige_tile_conv_modulated (the kernel and grid it would use for this descriptor), host-only. */

@@ -419,9 +419,75 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
     if (p.ksplit > 1) cg::this_cluster().sync();   // nobody leaves while a peer still reads its partial tile
 }
 
-template <typename T, int WM, int WN, int WARPS_M, int WARPS_N, int HALO_PIX, int NSTAGE, bool MOD>
-static int launch_cfg(ConvParams &p, cudaStream_t st) {
+// The three CTA configurations: GEMM rows and output channels per CTA, halo pixels one buffer holds.
+//   L: 128x128 CTA tile, 8 warps, 5-stage weight ring; M: 64x64, 4 warps, 8 stages; S: 32x64, 4 warps, 8 stages.
+struct MmaCfg {
+    int bm, bn, halo_pix;
+};
+constexpr MmaCfg kMmaCfgs[3] = {{128, 128, 288}, {64, 64, 144}, {32, 64, 72}};
+enum { MMA_L = 0, MMA_M = 1, MMA_S = 2 };
+
+// Launch plan of the mma.sync kernel: configuration, tiles per CTA, K split and grid.  Host logic only; the launch and the plan
+// queries (sige_tile_conv_plan, sige_tile_conv_modulated_plan) both take it from mma_plan().
+struct MmaPlan {
+    int cfg;      // MMA_L / MMA_M / MMA_S
+    int tpc;      // tiles per CTA
+    int ksplit;   // effective split-K factor == cluster size along z
+    int grid_x, grid_y;
+};
+
+static inline int tiles_per_cta(const MmaCfg &c, int P, int RS) { return min(c.bm / P, c.halo_pix / RS); }
+
+// CTA-count estimate used to pick a configuration: small grids want small CTA tiles.  -1: the tile does not fit.
+static inline long long ctas_for(int NT, int P, int RS, int Cout, const MmaCfg &c) {
+    const int tpc = tiles_per_cta(c, P, RS);
+    if (tpc < 1) return -1;
+    return (long long)ceil_div(NT, tpc) * ceil_div(Cout, c.bn);
+}
+
+// 0, or 1 with the error set: the tile fits no configuration (L holds whatever M or S hold), or ksplit is not a cluster size.
+// Both refusals come before the device is asked for its SM count.
+static int mma_plan(int NT, int R, int S, int P, int Cin, int taps, int Cout, int ksplit_req, MmaPlan *pl) {
+    const int RS = R * S;
+    if (tiles_per_cta(kMmaCfgs[MMA_L], P, RS) < 1) {
+        set_error("sige_tile_conv: tile %dx%d (%d output pixels) does not fit the CTA tile (BM=%d, halo %d px)", R, S, P,
+                  kMmaCfgs[MMA_L].bm, kMmaCfgs[MMA_L].halo_pix);
+        return 1;
+    }
+    const int J = ceil_div(Cin, KC) * taps;
+    if (ksplit_req > J) ksplit_req = 1;
+    if (ksplit_req > 0 && ksplit_req != 1 && ksplit_req != 2 && ksplit_req != 4 && ksplit_req != 8) {
+        set_error("sige_tile_conv: ksplit must be 1, 2, 4 or 8 (got %d)", ksplit_req);
+        return 1;
+    }
+    // Prefer the largest tile that still fills the machine; below that, the smallest tile plus split-K.
+    const long long cL = ctas_for(NT, P, RS, Cout, kMmaCfgs[MMA_L]);
+    const long long cM = ctas_for(NT, P, RS, Cout, kMmaCfgs[MMA_M]);
+    const long long cS = ctas_for(NT, P, RS, Cout, kMmaCfgs[MMA_S]);
+    const int sms = sm_count();
+    if (cL >= 2 * sms) pl->cfg = MMA_L;
+    else if (cM >= sms || cS < 0) pl->cfg = cM > 0 ? MMA_M : MMA_L;
+    else pl->cfg = MMA_S;
+    const MmaCfg &c = kMmaCfgs[pl->cfg];
+    pl->tpc = tiles_per_cta(c, P, RS);
+    pl->grid_x = ceil_div(NT, pl->tpc);
+    pl->grid_y = ceil_div(Cout, c.bn);
+    int ks = ksplit_req;
+    if (ks <= 0) {
+        // auto split-K: aim for ~2 CTAs per SM, keep >= 4 K steps per slice, cluster size <= 8 (portable limit)
+        const long long base = (long long)pl->grid_x * pl->grid_y;
+        ks = 1;
+        while (ks < 8 && base * (ks * 2) <= 2 * sms && J / (ks * 2) >= 4) ks *= 2;
+    }
+    pl->ksplit = ks;
+    return 0;
+}
+
+template <typename T, int CFG, int WM, int WN, int WARPS_M, int WARPS_N, int HALO_PIX, int NSTAGE, bool MOD>
+static int launch_cfg(ConvParams &p, const MmaPlan &pl, cudaStream_t st) {
     using Cfg = ConvCfg<T, WM, WN, WARPS_M, WARPS_N, HALO_PIX, NSTAGE>;
+    static_assert(Cfg::BM == kMmaCfgs[CFG].bm && Cfg::BN == kMmaCfgs[CFG].bn && HALO_PIX == kMmaCfgs[CFG].halo_pix,
+                  "the plan's table does not describe this instantiation");
     auto kern = tile_conv_mma_kernel<T, WM, WN, WARPS_M, WARPS_N, HALO_PIX, NSTAGE, MOD>;
     static int attr_dev = -1;   // per instantiation; one process drives one GPU, but stay correct if not
     int dev = 0;
@@ -434,26 +500,9 @@ static int launch_cfg(ConvParams &p, cudaStream_t st) {
         }
         attr_dev = dev;
     }
-    p.tpc = min(Cfg::BM / p.P, HALO_PIX / p.RS);
-    if (p.tpc < 1) {
-        set_error("sige_tile_conv: tile %dx%d (%d output pixels) does not fit the CTA tile (BM=%d, halo %d px)", p.R, p.S,
-                  p.P, Cfg::BM, HALO_PIX);
-        return 1;
-    }
-    const int J = ceil_div(p.Cin, KC) * p.taps;
-    const long long base = (long long)ceil_div(p.NT, p.tpc) * ceil_div(p.Cout, Cfg::BN);
-    if (p.ksplit <= 0) {
-        // auto split-K: aim for ~2 CTAs per SM, keep >= 4 K steps per slice, cluster size <= 8 (portable limit)
-        int ks = 1;
-        while (ks < 8 && base * (ks * 2) <= 2 * sm_count() && J / (ks * 2) >= 4) ks *= 2;
-        p.ksplit = ks;
-    }
-    if (p.ksplit > J) p.ksplit = 1;
-    if (p.ksplit != 1 && p.ksplit != 2 && p.ksplit != 4 && p.ksplit != 8) {
-        set_error("sige_tile_conv: ksplit must be 1, 2, 4 or 8 (got %d)", p.ksplit);
-        return 1;
-    }
-    const dim3 grid(ceil_div(p.NT, p.tpc), ceil_div(p.Cout, Cfg::BN), p.ksplit);
+    p.tpc = pl.tpc;
+    p.ksplit = pl.ksplit;
+    const dim3 grid(pl.grid_x, pl.grid_y, pl.ksplit);
     const cudaError_t e = launch_ex(kern, grid, dim3(Cfg::NTHREADS), Cfg::SMEM_BYTES, st, p.pdl != 0, dim3(1, 1, p.ksplit), p);
     if (e != cudaSuccess) {
         set_error("sige_tile_conv: launch failed (grid %d x %d x %d, %d threads, %d B smem): %s", grid.x, grid.y, grid.z,
@@ -464,26 +513,30 @@ static int launch_cfg(ConvParams &p, cudaStream_t st) {
     return 0;
 }
 
-// CTA-count estimate used to pick a configuration: small grids want small CTA tiles.
-static inline long long ctas_for(int NT, int P, int RS, int Cout, int BM, int BN, int halo_pix) {
-    int tpc = min(BM / P, halo_pix / RS);
-    if (tpc < 1) return -1;
-    return (long long)ceil_div(NT, tpc) * ceil_div(Cout, BN);
+template <typename T, bool MOD> static int launch_tile_conv(ConvParams &p, cudaStream_t st) {
+    MmaPlan pl;
+    if (mma_plan(p.NT, p.R, p.S, p.P, p.Cin, p.taps, p.Cout, p.ksplit, &pl) != 0) return 1;
+    if (pl.cfg == MMA_L) return launch_cfg<T, MMA_L, 2, 8, 4, 2, 288, 5, MOD>(p, pl, st);
+    if (pl.cfg == MMA_M) return launch_cfg<T, MMA_M, 2, 4, 2, 2, 144, 8, MOD>(p, pl, st);
+    return launch_cfg<T, MMA_S, 2, 2, 1, 4, 72, 8, MOD>(p, pl, st);
 }
 
-template <typename T, bool MOD> static int launch_tile_conv(ConvParams &p, cudaStream_t st) {
-    // L: 128x128 CTA tile, 8 warps, 5-stage weight ring; M: 64x64, 4 warps, 8 stages; S: 32x64, 4 warps, 8 stages.
-    // Prefer the largest tile that still fills the machine; below that, the smallest tile plus split-K.
-    const long long cL = ctas_for(p.NT, p.P, p.RS, p.Cout, 128, 128, 288);
-    const long long cM = ctas_for(p.NT, p.P, p.RS, p.Cout, 64, 64, 144);
-    const long long cS = ctas_for(p.NT, p.P, p.RS, p.Cout, 32, 64, 72);
-    const int sms = sm_count();
-    if (cL >= 2 * sms) return launch_cfg<T, 2, 8, 4, 2, 288, 5, MOD>(p, st);
-    if (cM >= sms || cS < 0) {
-        if (cM > 0) return launch_cfg<T, 2, 4, 2, 2, 144, 8, MOD>(p, st);
-        return launch_cfg<T, 2, 8, 4, 2, 288, 5, MOD>(p, st);
-    }
-    return launch_cfg<T, 2, 2, 1, 4, 72, 8, MOD>(p, st);
+// The mma.sync plan of a descriptor for sige_tile_conv_plan / sige_tile_conv_modulated_plan: fills bn, ksplit and the grid when the
+// mma.sync kernel would take the launch (f16 / bf16, a geometry and a ksplit it accepts, no fused shortcut); otherwise leaves
+// `out` as it is.  No pointer of the descriptor is looked at.
+void mma_plan_of(const sige_tile_conv_t *a, sige_tile_conv_plan_t *out) {
+    if (a->dtype != SIGE_F16 && a->dtype != SIGE_BF16) return;
+    if (a->B <= 0 || a->N <= 0 || a->R <= 0 || a->S <= 0 || a->kH <= 0 || a->kW <= 0 || a->stride <= 0) return;
+    if (a->R < a->kH || a->S < a->kW || a->Cin <= 0 || a->Cin % 8 != 0 || a->Cout <= 0 || a->Cout % 8 != 0) return;
+    if (a->ksplit < 0 || a->ksplit > 8 || a->n_src2 != 0) return;
+    const int Ro = (a->R - a->kH) / a->stride + 1, So = (a->S - a->kW) / a->stride + 1;
+    MmaPlan pl;
+    if (mma_plan(a->B * a->N, a->R, a->S, Ro * So, a->Cin, a->kH * a->kW, a->Cout, a->ksplit, &pl) != 0) return;
+    out->bn = kMmaCfgs[pl.cfg].bn;
+    out->ksplit = pl.ksplit;
+    out->grid_x = pl.grid_x;
+    out->grid_y = pl.grid_y;
+    out->grid_z = pl.ksplit;
 }
 
 bool tc5_supported(const sige_tile_conv_t *a, int pitch0);

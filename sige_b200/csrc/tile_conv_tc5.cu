@@ -1302,6 +1302,8 @@ int tc5_launch(const sige_tile_conv_t *a, int pitch0, const sige_conv_modulation
 #undef SIGE_TC5
 }
 
+void mma_plan_of(const sige_tile_conv_t *a, sige_tile_conv_plan_t *out);   // tile_conv_mma.cu
+
 }  // namespace sige
 
 // The wgmma plan of a descriptor whose launch takes the wgmma kernel.
@@ -1324,7 +1326,8 @@ extern "C" int sige_tile_conv_plan(const sige_tile_conv_t *a, sige_tile_conv_pla
     using namespace sige;
     SIGE_REQUIRE(a && out, "sige_tile_conv_plan: null pointer");
     out->path = 0; out->bn = 0; out->ksplit = 0; out->deep_ring = 0; out->grid_x = out->grid_y = out->grid_z = 0;
-    if ((a->flags & SIGE_CONV_TC5) && tc5_supported(a, 0)) tc5_plan(a, out);      // else the mma.sync / CUDA-core paths
+    if ((a->flags & SIGE_CONV_TC5) && tc5_supported(a, 0)) tc5_plan(a, out);
+    else mma_plan_of(a, out);
     return 0;
 }
 
@@ -1335,5 +1338,6 @@ extern "C" int sige_tile_conv_modulated_plan(const sige_tile_conv_t *a, sige_til
     SIGE_REQUIRE(a && out, "sige_tile_conv_modulated_plan: null pointer");
     out->path = 0; out->bn = 0; out->ksplit = 0; out->deep_ring = 0; out->grid_x = out->grid_y = out->grid_z = 0;
     if ((a->flags & SIGE_CONV_TC5) && tc5_supported_modulated(a)) tc5_plan(a, out);
+    else mma_plan_of(a, out);
     return 0;
 }

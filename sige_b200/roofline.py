@@ -158,8 +158,10 @@ def plan_of(fc):
 
 
 def kernel_name(pl) -> str:
-    """'wgmma bn=<BN> ksplit=<K>' or 'mma.sync' for a plan_of() result."""
-    return "wgmma bn=%d ksplit=%d" % (pl.bn, pl.ksplit) if pl.path == 1 else "mma.sync"
+    """'wgmma bn=<BN> ksplit=<K>' or 'mma.sync bn=<BN> ksplit=<K> grid=<X>x<Y>' for a plan_of() result."""
+    if pl.path == 1:
+        return "wgmma bn=%d ksplit=%d" % (pl.bn, pl.ksplit)
+    return "mma.sync bn=%d ksplit=%d grid=%dx%d" % (pl.bn, pl.ksplit, pl.grid_x, pl.grid_y)
 
 
 def _traced_step(model, args, options):

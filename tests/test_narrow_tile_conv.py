@@ -22,6 +22,7 @@ from conftest import REPO
 sys.path.insert(0, os.path.join(REPO, "tests"))
 sys.path.insert(0, os.path.join(REPO, "baseline"))
 
+import mma_tile_conv_contract as MC  # noqa: E402
 import tile_conv_contract as TC  # noqa: E402
 
 ACT_RELU = 2
@@ -83,7 +84,9 @@ def test_narrow_launches_plan_on_the_mma_sync_kernel(cabi_lib):
             continue
         for k, stride in ((3, 1), (1, 1), (3, 2)):
             p = TC.plan_of(_host_desc(srcs=((cin, 0),), cout=64, k=k, stride=stride))
-            assert p.path == 0, (cin, k, stride)
+            R = 6 if (k == 3 and stride == 1) else (4 if k == 1 else 5)
+            want = MC.plan(16, R, R, k, k, stride, cin, 64, 0)       # 16 tiles: the S configuration, K split while a slice keeps 4 steps
+            assert p.path == 0 and MC.plan_tuple(p) == MC.expected_plan_tuple(want) and want.config == "S", (cin, k, stride)
 
 
 # ---------------------------------------------------------------------------------------------------------------- lowering (CPU)

@@ -20,6 +20,7 @@ from conftest import REPO
 
 sys.path.insert(0, os.path.join(REPO, "tests"))
 
+import mma_tile_conv_contract as MC  # noqa: E402
 import tile_conv_contract as TC  # noqa: E402
 import test_modulated_tile_conv as TM  # noqa: E402
 from test_modulated_tile_conv import Mod  # noqa: E402
@@ -133,9 +134,10 @@ def test_modulated_case_table_sizes_do_not_depend_on_the_h100_variant():
                 assert m_blocks * spec.Cout // 64 <= 100, spec.name
 
 
-def test_launches_that_stay_on_mma_sync(cabi_lib):
-    """No flag, a narrow Cin, a Cout that is not a multiple of 64, stride 2: sige_tile_conv_modulated_plan says mma.sync (path 0) and
-    nothing else; the wgmma geometries with the flag plan wgmma exactly as sige_tile_conv_plan does."""
+def test_launches_that_stay_on_mma_sync_report_its_plan(cabi_lib):
+    """No flag, a narrow Cin, a Cout that is not a multiple of 64, stride 2: sige_tile_conv_modulated_plan says mma.sync (path 0) with
+    that kernel's configuration and grid (restated in tests/mma_tile_conv_contract.py); the wgmma geometries with the flag plan wgmma
+    exactly as sige_tile_conv_plan does."""
     def plans(spec, flags):
         d = TC.descriptor(TC.make_case(spec, torch.float16, "cpu"), 0, flags)
         return modulated_plan(d), TC.plan_of(d)
@@ -149,7 +151,8 @@ def test_launches_that_stay_on_mma_sync(cabi_lib):
                         (dataclasses.replace(base, Cout=96), TC.TC5),
                         (dataclasses.replace(base, k=1, srcs=((40, 0),)), TC.TC5)):
         mod, _ = plans(spec, flags)
-        assert (mod.path, mod.bn, mod.ksplit, mod.deep_ring, mod.grid_x) == (0, 0, 0, 0, 0), (spec.srcs, spec.Cout, flags)
+        want = MC.plan(spec.B * spec.N, spec.R, spec.R, spec.k, spec.k, spec.stride, spec.Cin, spec.Cout, 0)
+        assert MC.plan_tuple(mod) == MC.expected_plan_tuple(want) and mod.path == 0 and mod.bn == 64, (spec.srcs, spec.Cout, flags)
     # stride 2 without a pre-op is a wgmma geometry for sige_tile_conv (pure-copy gather), not for the modulated launch
     s2 = TC.Spec("s2", B=1, H=34, W=30, stride=2, srcs=((64, 0),), Cout=128, counts=(40,), seed=812)
     mod, plain = plans(s2, TC.TC5)
