@@ -425,6 +425,28 @@ int sige_separable_conv_supported(int Cin, int Cout, int k, int dtype);
 int sige_separable_conv(const sige_separable_conv_t *p, sige_stream_t stream);
 
 /* ------------------------------------------------------------------------- */
+/* a8: sparse_update write-back (reference sige/nn/scatter.py:59-60,114-129,  */
+/*     sige/nn/scatter_gather.py:65-77)                                        */
+/* ------------------------------------------------------------------------- */
+/* Copies the output tiles of many NHWC buffers into their caches, one launch.  Entry e: tile i of image b (b < B) writes rows
+ * [(idx_h + offH) / strideH, + Ro) and columns [(idx_w + offW) / strideW, + So) — sige_scatter's paste rule, C division —
+ * clipped to the image, every channel, from `src` (NHWC [B, H, W, C], f16 / bf16) into `dst` (the same logical [B, C, H, W] in
+ * dst_layout; dst_dtype SIGE_F32 or src_dtype, so every conversion is exact).  SIGE_TILE_NONE entries write nothing, so a
+ * fixed-capacity list may be passed whole.  An entry with N == 0 is skipped and its pointers are not looked at.  C a multiple
+ * of 8, Ro and So in [1, 8], buffers 16-byte aligned.  At most SIGE_WRITEBACK_MAX_ENTRIES entries per call (the table travels
+ * in the launch's parameters); every entry is validated before any device call. */
+#define SIGE_WRITEBACK_MAX_ENTRIES 64
+typedef struct {
+    const void *src;
+    void *dst;
+    const int32_t *idx;     /* [N,2] tile origins */
+    int N, B, C, H, W;
+    int src_dtype, dst_dtype, dst_layout;
+    int offH, offW, strideH, strideW, Ro, So;
+} sige_writeback_entry_t;
+int sige_tile_writeback(const sige_writeback_entry_t *entries, int n_entries, sige_stream_t stream);
+
+/* ------------------------------------------------------------------------- */
 /* diagnostics                                                                */
 /* ------------------------------------------------------------------------- */
 /* In-kernel timeline: while `buf` (device int64, 16 slots per CTA of the NEXT sige_tile_conv launch that takes the wgmma

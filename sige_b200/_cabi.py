@@ -74,6 +74,15 @@ class SeparableConv(Structure):
                 ("offH", c_int), ("offW", c_int), ("nbranch", c_int), ("branch", SeparableBranch * 2), ("flags", c_int)]
 
 
+class WritebackEntry(Structure):
+    _fields_ = [("src", c_void_p), ("dst", c_void_p), ("idx", c_void_p), ("N", c_int), ("B", c_int), ("C", c_int), ("H", c_int), ("W", c_int),
+                ("src_dtype", c_int), ("dst_dtype", c_int), ("dst_layout", c_int), ("offH", c_int), ("offW", c_int),
+                ("strideH", c_int), ("strideW", c_int), ("Ro", c_int), ("So", c_int)]
+
+
+WRITEBACK_MAX_ENTRIES = 64
+
+
 class TileConv(Structure):
     _fields_ = [
         ("dtype", c_int),
@@ -141,6 +150,7 @@ PROTOTYPES = {
     "sige_spade_modulate": (_I, [_P, c_int64, _P, c_int64, _P, c_int64, _P, c_int64, c_int64, _I, ctypes.c_float, _I, _P]),
     "sige_separable_conv_supported": (_I, [_I, _I, _I, _I]),
     "sige_separable_conv": (_I, [POINTER(SeparableConv), _P]),
+    "sige_tile_writeback": (_I, [POINTER(WritebackEntry), _I, _P]),
     "sige_debug_set_trace": (_I, [_P]),
     "sige_debug_set_split_halo_buffers": (_I, [_I]),
 }

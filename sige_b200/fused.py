@@ -38,6 +38,7 @@ inject a CPU simulator of the launch descriptors to check the lowering without a
 """
 from __future__ import annotations
 
+import copy
 import math
 from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple
 
@@ -486,6 +487,14 @@ class CudaExecutor:
     def separable_supported(self, cin: int, cout: int) -> bool:
         return self.ops.separable_conv_supported(cin, cout, self.dtype)
 
+    def writeback_supported(self) -> bool:
+        """Can the step copy its output tiles into the module caches (sige_tile_writeback: sparse_update on the fused path)?"""
+        return True
+
+    def prepare_writeback(self, entries) -> Callable[[int], None]:
+        """One `sige_tile_writeback` over (src buffer, module cache, tile list, off, stride, output tile) entries."""
+        return self.ops.tile_writeback_launcher(entries)
+
     def narrow_conv_supported(self, cin: int, cout: int, k: int, stride: int) -> bool:
         """Can sige_tile_conv run a conv whose single source has `cin` channels, a multiple of 8 but not of 64 (the mma.sync
         kernel with a partial last K chunk)?"""
@@ -846,6 +855,13 @@ class Lowering:
         self.slots: Dict[int, IdxSlot] = {}
         self.flag_recipes: List = []       # (flags buffer, main slot, off, shortcut slot, soff) of fused shortcuts
         self.cached_bufs: List[Buf] = []
+        # sparse_update: (cached Buf, IdxSlot or None, off, stride, output tile) of every launch that writes a cached buffer, and
+        # (name, shortcut source Bufs, weight, bias, skip Buf, IdxSlot, off, conv2's launch) of every shortcut fused into conv2
+        self.cache_writers: List[Tuple[Buf, Optional[IdxSlot], int, int, int]] = []
+        self.shortcut_relaunches: List = []
+        self.epilogue: List[Tuple[str, Callable[[int], None]]] = []
+        self.epilogue_fused: List[FusedConv] = []
+        self.sparse_update_reason: Optional[str] = "not lowered yet"
         self.view_nodes = 0              # view ops resolved at build time (no run-time work)
         self._all_idx: Dict = {}
         self._vecs: Dict = {}
@@ -1058,6 +1074,9 @@ class Lowering:
             return None
         if dst is not None:
             dst.producers.append(fc)
+            if dst.cached_init is not None:
+                self.cache_writers.append((dst, s.slot if tile_img is None else None, off, stride, (block - s.k) // stride + 1))
+        fc.pos = len(self.steps)
         self.fused.append(fc)
         self.steps.append(("conv", fc.launch))
         return fc
@@ -1796,6 +1815,8 @@ class Lowering:
                 self.steps[rec.slot] = ("separable", ex.prepare_separable(rec))
 
             self._pending_prepare.append(prep)
+        slot = next((sl for sl in self.slots.values() if sl.buf is idx), None)
+        self.cache_writers.append((dst, slot, int(g.offset[0]), 1, 4))
         _ = dst.raw               # written in place every step: the buffer must exist (initialised from the module's cache)
 
     # ---- operator modules
@@ -1959,7 +1980,12 @@ class Lowering:
                 self.flag_recipes.append((fbuf, ms, off, ss, soff))
                 flags = fbuf
             shortcut = ([b for b, _ in sc_full.segs], sc.weight, sc.bias, flags)
+            n_fused = len(self.fused)
             self._tile_emit(node, co, dst, residual=skip, shortcut=shortcut, name=name)
+            if len(self.fused) > n_fused and mg.tile_images is None:
+                # the shortcut's output exists only inside conv2's launch: sparse_update relaunches it into `skip` (the un-fused form)
+                self.shortcut_relaunches.append((name + ".shortcut", shortcut[0], sc.weight, sc.bias, skip, ss, soff, self.fused[-1]))
+                self.cache_writers.append((skip, ss, soff, 1, 4))
         else:
             if not subset:
                 return False
@@ -2459,6 +2485,93 @@ class Lowering:
             self.ex.prepare_conv(fc)
         for prep in self._pending_prepare:
             prep()
+        self._build_sparse_update()
+
+    # ------------------------------------------------------------------ sparse_update epilogue
+    def _sparse_update_refusal(self) -> Optional[str]:
+        """Why this step cannot write its results back into the module caches (None: it can)."""
+        ok = getattr(self.ex, "writeback_supported", None)
+        if ok is None or not ok():
+            return "the executor has no tile write-back"
+        if any(b.shape[0] != b.cached_init.shape[0] for b in self.cached_bufs) or any(f.spec.tile_img is not None for f in self.fused):
+            return "a batch of edits (a cache holds one image)"
+        eager = [n for n in self.eager_nodes if n.startswith("sige.scatter")]
+        if eager:
+            return "eager operator-module scatters in the step (%s)" % ", ".join(eager)
+        for (buf, slot, _off, _st, _ro) in self.cache_writers:
+            if slot is None:
+                return "a cached %s buffer is written through a tile list without a fixed-capacity buffer" % (buf.shape,)
+        for buf in self.cached_bufs:
+            c = buf.cached_init
+            if c.dtype not in (torch.float32, self.dtype):
+                return "a %s cache cannot take %s tiles exactly" % (c.dtype, self.dtype)
+            if c.dim() != 4 or tuple(c.shape) != buf.shape or c.shape[1] % 8 or not (c.is_contiguous() or c.is_contiguous(memory_format=torch.channels_last)):
+                return "a cache of shape %s is not a dense [B, C, H, W] tensor with C a multiple of 8" % (tuple(c.shape),)
+        return None
+
+    def _relaunch(self, spec: ConvSpec, name: str) -> FusedConv:
+        spec.name, spec.pdl = name, False          # (the epilogue's first launch follows another graph)
+        fc = FusedConv(spec)
+        self.ex.prepare_conv(fc)
+        self.epilogue_fused.append(fc)
+        self.epilogue.append(("conv", fc.launch))
+        return fc
+
+    def _build_sparse_update(self) -> None:
+        """The program `FusedStep.sparse_update()` runs after the main program: (1) every shortcut fused into a conv2 launch as its own
+        1x1 tile conv into `skip` (its tiles of the reference's `original_residuals`), (2) every launch whose cached destination
+        only exists as producer-written views again, writing the raw values, (3) one `sige_tile_writeback` of the output tiles of
+        every cached buffer into its module cache.  The main program is not touched: its launches were prepared before this runs."""
+        self.sparse_update_reason = self._sparse_update_refusal()
+        if self.sparse_update_reason is not None:
+            return
+        plan: List[Tuple[ConvSpec, str, int]] = []
+        for (name, sc_bufs, w, b, skip, slot, soff, conv2) in self.shortcut_relaunches:
+            s = ConvSpec()
+            s.srcs = [(sb.raw, 0) for sb in sc_bufs]
+            s.B, s.H, s.W = skip.shape[0], sc_bufs[0].shape[2], sc_bufs[0].shape[3]
+            s.idx, s.N, s.slot, s.block, s.k, s.stride, s.off = slot.buf, slot.cap, slot, 4, 1, 1, soff
+            s.weight, s.bias, s.weight_key = w.detach().float(), None if b is None else b.detach().float(), (w, "w")
+            s.tc5, s.ksplit, s.dst = self.tc5, self.ksplit, skip
+            plan.append((s, name, conv2.pos))
+        raw_less = {id(b) for b in self.cached_bufs if not b.has_raw}
+        for fc in self.fused:
+            if fc.spec.dst is not None and id(fc.spec.dst) in raw_less:
+                s = copy.copy(fc.spec)
+                s.aux = []                # the launch wrote only transformed views of its destination: write the raw values
+                plan.append((s, fc.name + ".raw", fc.pos))
+        # the relaunched launches read their sources after the whole main program: nothing may rewrite them after the launch
+        # they repeat, nor in the epilogue
+        writes: List[Tuple[int, int]] = []       # (storage, position)
+        for fc in self.fused:
+            s = fc.spec
+            outs = [v for (v, _, _, _) in s.aux] + ([s.dst_stack] if s.dst_stack is not None else []) + ([s.dst.raw] if s.dst is not None and s.dst.has_raw else [])
+            writes += [(t.untyped_storage().data_ptr(), fc.pos) for t in outs]
+        for rec in self.separable:
+            writes += [(br[3].raw.untyped_storage().data_ptr(), rec.slot) for br in rec.branches]
+        writes += [(s.dst.raw.untyped_storage().data_ptr(), len(self.steps)) for (s, _, _) in plan]
+
+        def sources(s: ConvSpec) -> List[torch.Tensor]:
+            out = [t for t, _ in s.srcs] + ([s.residual] if s.residual is not None else [])
+            if s.shortcut is not None:
+                out += list(s.shortcut[0])
+            if s.modulation is not None:
+                out += [s.modulation[0], s.modulation[1]]
+            return out
+
+        for (s, name, pos) in plan:
+            for t in sources(s):
+                key = t.untyped_storage().data_ptr()
+                if any(k == key and p > pos for (k, p) in writes):
+                    self.sparse_update_reason = "%s: a source is rewritten after the launch the epilogue repeats" % name
+                    return
+        for (s, name, _pos) in plan:
+            self._relaunch(s, name)
+        entries = []
+        for (buf, slot, off, stride, ro) in self.cache_writers:
+            entries.append((buf.raw, buf.cached_init, slot.buf, off, stride, ro))
+        if entries:
+            self.epilogue.append(("writeback", self.ex.prepare_writeback(entries)))
 
 
 # =====================================================================================================================
@@ -2517,17 +2630,41 @@ class FusedStep:
         self.outputs = self.low.outputs
         self.output = self.outputs if isinstance(self.outputs, torch.Tensor) else None
         self.eager_nodes = self.low.eager_nodes
+        # sparse_update (the reference's apply step): whether this step can write its results back into the module caches
+        self.sparse_update_reason: Optional[str] = self.low.sparse_update_reason
+        self.sparse_update_supported = self.sparse_update_reason is None
         self.graph = None
+        self.epilogue_graph = None
         self.launches_per_step = 0
         self._finalize(use_graph)
 
     # ------------------------------------------------------------------ execution
     def run_eager(self):
+        self._run(self.steps)
+        return self.outputs
+
+    def _run(self, steps) -> None:
         stream = torch.cuda.current_stream(self.dev).cuda_stream if self.dev.type == "cuda" else 0
         with torch.no_grad():
-            for _kind, fn in self.steps:
+            for _kind, fn in steps:
                 fn(stream)
-        return self.outputs
+
+    def sparse_update(self) -> None:
+        """After a call: write its results into the module caches, as the reference's modules do with ``sparse_update=True``
+        (sige/nn/scatter.py:59-60,114-129, scatter_gather.py:65-77) — only the output tiles of the current tile lists.  Runs the
+        epilogue program the lowering built (`Lowering._build_sparse_update`); the first call runs it eagerly and captures it in
+        a second CUDA graph, later calls replay that graph.  The main program and its graph are not involved."""
+        if not self.sparse_update_supported:
+            raise RuntimeError("this fused step cannot write back into the module caches: %s" % self.sparse_update_reason)
+        if self.epilogue_graph is not None:
+            self.epilogue_graph.replay()
+            return
+        self._run(self.low.epilogue)
+        if self.graph is not None:
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._run(self.low.epilogue)
+            self.epilogue_graph = g
 
     def _finalize(self, use_graph: bool) -> None:
         if self.dev.type != "cuda":

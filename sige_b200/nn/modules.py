@@ -267,8 +267,6 @@ class Scatter(SIGEModule):
             g = self.gather.module
             cached = self.original_outputs[self.cache_id]
             if lazy.is_lazy(x, residual):
-                if self.sparse_update:
-                    raise lazy.TraceUnsupported("sparse_update=True runs through the eager operator modules")
                 shape = tuple(cached.shape) if g.num_edits is None else (g.num_edits, *cached.shape[1:])
                 return lazy.record_module_call("sige.scatter", self, (x, residual), shape, x if lazy.is_lazy(x) else residual)
             g._no_batched_edits()
@@ -317,8 +315,6 @@ class ScatterWithBlockResidual(SIGEModule):
             mg, sg = self.main_gather.module, self.shortcut_gather.module
             y0, y1 = self.original_outputs[self.cache_id], self.original_residuals[self.cache_id]
             if lazy.is_lazy(x, residual):
-                if self.sparse_update:
-                    raise lazy.TraceUnsupported("sparse_update=True runs through the eager operator modules")
                 shape = tuple(y0.shape) if mg.num_edits is None else (mg.num_edits, *y0.shape[1:])
                 return lazy.record_module_call("sige.scatter_block_residual", self, (x, residual), shape, x if lazy.is_lazy(x) else residual)
             mg._no_batched_edits()
@@ -368,8 +364,6 @@ class ScatterGather(SIGEModule):
         if self.mode == "sparse":
             cached = self.original_outputs[self.cache_id]
             if lazy.is_lazy(x, scale, shift):
-                if self.sparse_update:
-                    raise lazy.TraceUnsupported("sparse_update=True runs through the eager operator modules")
                 n = g.active_indices.size(0)
                 rows = n if g.tile_images is not None else cached.size(0) * n
                 return lazy.record_module_call("sige.scatter_gather", self, (x, scale, shift), (rows, x.shape[1], *g.block_size), x)

@@ -229,7 +229,7 @@ class SIGEModel(nn.Module):
 
     def _fused_lookup(self, args, kwargs=None):
         d = self.__dict__
-        if not d.get("_fused_enabled", False) or d.get("mode") != "sparse" or d.get("_sige_sparse_update", False) or torch.is_grad_enabled():
+        if not d.get("_fused_enabled", False) or d.get("mode") != "sparse" or torch.is_grad_enabled():
             return None
         x = args[0] if args else None
         compute = d.get("_fused_options", {}).get("dtype")
@@ -263,7 +263,12 @@ class SIGEModel(nn.Module):
                 del steps[k]           # older masks / older caches: their buffers are garbage now
             from ..fused import FusedStep
 
+            update = d.get("_sige_sparse_update", False)
             try:
+                # built with sparse_update off: an eager operator-module node of the step must never write a cache from inside the
+                # captured graph (the write-back is the step's own epilogue, `FusedStep.sparse_update`)
+                if update:
+                    self.set_sparse_update(False)
                 steps[key] = FusedStep(self, *args, call_kwargs=kwargs, **d.get("_fused_options", {}))
             except Exception as e:  # noqa: BLE001
                 # TraceUnsupported = the forward needs tensor VALUES at trace time; anything else = a pattern the lowering
@@ -275,15 +280,34 @@ class SIGEModel(nn.Module):
 
                 warnings.warn("sige: this forward does not run as a fused step (%s: %s); using the eager operator modules" % (type(e).__name__, e))
                 steps[key] = None
+            finally:
+                if update:
+                    self.set_sparse_update(True)
         return steps[key]
+
+    def _drop_stale_steps(self, keep=None) -> None:
+        """A write-back changed the caches of the current cache id without a new cache generation: every other compiled step of that
+        id holds buffers cloned from the old contents."""
+        steps = self.__dict__.get("_fused_steps", {})
+        cid = self.__dict__.get("_sige_cache_id", 0)
+        for k in [k for k, st in steps.items() if k[2] == cid and st is not None and st is not keep]:
+            del steps[k]
 
     def __call__(self, *args, **kwargs):
         step = self._fused_lookup(args, kwargs)
+        update = self.__dict__.get("_sige_sparse_update", False)
+        if step is not None and update and not step.sparse_update_supported:
+            step = None                       # this step cannot write back: the operator modules apply the edit
         if step is None:
             self._sync_async_masks()
+            if update and self.__dict__.get("mode") == "sparse":
+                self._drop_stale_steps()
             return super().__call__(*args, **kwargs)
         self.__dict__["fused_step"] = step
         out = step(*args, **kwargs)
+        if update:
+            step.sparse_update()
+            self._drop_stale_steps(keep=step)
         like = args[0].dtype      # results are fresh tensors in the caller's dtype (the static buffers are reused by the next call)
 
         def fresh(o):

@@ -752,3 +752,59 @@ def separable_conv(x: torch.Tensor, branches, idx: Optional[torch.Tensor] = None
     with torch.cuda.device(x.device):
         _cabi.check(_cabi.lib().sige_separable_conv(byref(d), _stream(x)), "sige_separable_conv")
     _bump()
+
+
+# --------------------------------------------------------------------------------------
+# a8: sparse_update write-back       (reference sige/nn/scatter.py:59-60,114-129, scatter_gather.py:65-77)
+# --------------------------------------------------------------------------------------
+def tile_writeback_launcher(entries):
+    """Prepare `sige_tile_writeback` over ``entries`` and return ``run(stream)``, which enqueues it (one launch per
+    SIGE_WRITEBACK_MAX_ENTRIES entries).  Entry = (src, dst, idx, off, stride, tile): ``src`` a channels-last f16 / bf16 buffer
+    [B, C, H, W]; ``dst`` its cache, the same shape, NCHW- or NHWC-dense, f32 or src's dtype; ``idx`` int32 [N, 2] tile origins
+    (SIGE_TILE_NONE entries write nothing); ``off`` / ``stride`` / ``tile`` = (h, w) pairs or ints: tile i writes rows
+    [(idx_h + off_h) / stride_h, + tile_h) and the matching columns, clipped to the image.  The tensors are not copied: the
+    launch reads them (and the tile lists) as they are when it runs."""
+    from ._cabi import WRITEBACK_MAX_ENTRIES, WritebackEntry
+
+    def pair(v):
+        return (int(v[0]), int(v[1])) if isinstance(v, (tuple, list)) else (int(v), int(v))
+
+    rows, keep, dev = [], [], None
+    for k, (src, dst, idx, off, stride, tile) in enumerate(entries):
+        _require_cuda(src, dst, idx)
+        idx = _idx(idx)
+        if src.dim() != 4 or tuple(dst.shape) != tuple(src.shape) or not src.is_contiguous(memory_format=torch.channels_last):
+            raise ValueError("tile_writeback: entry %d: src must be a channels-last [B, C, H, W] buffer and dst the same shape" % k)
+        lo = layout_of(dst)
+        if lo < 0:
+            raise ValueError("tile_writeback: entry %d: dst must be NCHW- or NHWC-dense" % k)
+        if idx.dim() != 2 or idx.shape[1] != 2:
+            raise ValueError("tile_writeback: entry %d: idx must be int32 [N, 2]" % k)
+        dev = dev or src.device
+        e = WritebackEntry()
+        e.src, e.dst, e.idx = src.data_ptr(), dst.data_ptr(), idx.data_ptr()
+        e.N, e.B, e.C, e.H, e.W = int(idx.shape[0]), int(src.shape[0]), int(src.shape[1]), int(src.shape[2]), int(src.shape[3])
+        e.src_dtype, e.dst_dtype, e.dst_layout = _dt(src), _dt(dst), lo
+        (e.offH, e.offW), (e.strideH, e.strideW), (e.Ro, e.So) = pair(off), pair(stride), pair(tile)
+        rows.append(e)
+        keep.append((src, dst, idx))
+    tables = []
+    for s in range(0, len(rows), WRITEBACK_MAX_ENTRIES):
+        part = rows[s:s + WRITEBACK_MAX_ENTRIES]
+        tables.append(((WritebackEntry * len(part))(*part), len(part)))
+
+    def run(stream: int) -> None:
+        _ = keep
+        for table, n in tables:
+            with torch.cuda.device(dev):
+                _cabi.check(_cabi.lib().sige_tile_writeback(table, n, stream), "sige_tile_writeback")
+            _bump()
+
+    return run
+
+
+def tile_writeback(entries) -> None:
+    """`tile_writeback_launcher(entries)` enqueued once on the current stream."""
+    entries = list(entries)
+    if entries:
+        tile_writeback_launcher(entries)(_stream(entries[0][0]))
