@@ -249,6 +249,8 @@ extern "C" int sige_sparse_attention(const sige_sparse_attention_t *a, sige_stre
                  a->Nq, a->Nk);
     SIGE_REQUIRE(sige_sparse_attention_supported(a->D, a->dtype), "sige_sparse_attention: unsupported head dim %d (32, 40, 64, 80, 128, 160) / dtype %d (f16, bf16)",
                  a->D, a->dtype);
+    // scale = 0 makes the last-block mask -inf * 0 = NaN; scale < 0 takes the running maximum at the wrong end
+    SIGE_REQUIRE(a->scale > 0.f && isfinite(a->scale), "sige_sparse_attention: scale = %g must be positive and finite", (double)a->scale);
     if (a->B == 0 || a->Nq == 0) return 0;          // no active tile: nothing to do
     SIGE_REQUIRE(a->q && a->k && a->v && a->out, "sige_sparse_attention: null buffer");
     const long long strides[12] = {a->q_stride[0], a->q_stride[1], a->q_stride[2], a->k_stride[0], a->k_stride[1], a->k_stride[2],

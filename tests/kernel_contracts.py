@@ -102,6 +102,12 @@ class Expect:
             return "(b, c, h, w) = (%d, %d, %d, %d)" % tuple(c)
         if self.g.layout == "bnc":
             return "(b, token, c) = (%d, %d, %d)" % tuple(c)
+        if self.g.layout == "bhnd":
+            return "(b, head, token, d) = (%d, %d, %d, %d)" % tuple(c)
+        if self.g.layout == "bnhd":
+            return "(b, token, head, d) = (%d, %d, %d, %d)" % tuple(c)
+        if self.g.layout == "pc":
+            return "(pixel, c) = (%d, %d)" % tuple(c)
         return "(b, c) = (%d, %d)" % tuple(c)
 
 
@@ -137,7 +143,8 @@ def check(label: str, expects: List[Expect], got: Dict[str, torch.Tensor], init:
         if not bool(w.any()):
             continue
         err = (g.double()[w] - e.want[w]).abs()
-        ratio = torch.nan_to_num(err / e.bound[w], nan=float("inf"))
+        # a bound of 0 demands the exact value (0 / 0 passes); a NaN error fails
+        ratio = torch.nan_to_num(torch.where(err == 0, torch.zeros_like(err), err / e.bound[w]), nan=float("inf"))
         r = float(ratio.max())
         if r > 1.0:
             k = int(ratio.argmax())
@@ -158,6 +165,45 @@ def snapshot(bufs: Dict[str, Guarded]) -> Dict[str, torch.Tensor]:
 def restore(bufs: Dict[str, Guarded], init: Dict[str, torch.Tensor]) -> None:
     for k, g in bufs.items():
         g.flat.copy_(init[k])
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# launching a case on the device (the GPU test files)
+# ----------------------------------------------------------------------------------------------------------------------
+def _launch(case, init, call):
+    """Restore every written buffer, run `call` (a C-ABI call returning a status), wait, and return the flat buffers."""
+    from sige_b200 import _cabi
+
+    restore(case.buffers(), init)
+    rc = call()
+    torch.cuda.synchronize()
+    assert rc == 0, _cabi.last_error()
+    return {k: g.flat.clone() for k, g in case.buffers().items()}
+
+
+def _same(a, b):
+    return all(torch.equal(bits(a[k]), bits(b[k])) for k in a)
+
+
+def _report(kernel, label, r):
+    print("[kernel contract] %-10s %-52s worst |err| / bound %.3f, beyond rounding %.3f" % (kernel, label, r[0], r[1]))
+
+
+def _run_and_check(kernel, label, case, expects, call, flag_variants=(0,)):
+    """Launch once per flags value and once more with the first: each within the contract, all bitwise equal."""
+    init = snapshot(case.buffers())
+    inputs0 = {k: t.clone() for k, t in case.inputs().items()}
+    first = None
+    for flags in flag_variants:
+        lab = label + (" pdl" if flags & PDL else "")
+        got = _launch(case, init, lambda: call(flags))
+        _report(kernel, lab, check(lab, expects, got, init, case.inputs(), inputs0))
+        if first is None:
+            first = got
+        else:
+            assert _same(got, first), "%s: programmatic dependent launch changed the result" % lab
+    assert _same(_launch(case, init, lambda: call(flag_variants[0])), first), "%s: a second launch differs" % label
+    return first
 
 
 # ----------------------------------------------------------------------------------------------------------------------

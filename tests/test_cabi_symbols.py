@@ -78,7 +78,8 @@ def test_attention_shape_predicate_is_pure_host_logic(cabi_lib):
 
 def test_sparse_attention_predicate_and_argument_checks_need_no_device(cabi_lib):
     """sige_sparse_attention_supported() is host logic; the entry point validates its descriptor before touching the device
-    (null descriptor, unsupported head dim, misaligned strides) and treats Nq == 0 as a no-op."""
+    (null descriptor, unsupported head dim, a scale that is not positive and finite, misaligned strides) and treats Nq == 0
+    as a no-op."""
     from sige_b200 import _cabi
 
     h = _cabi.lib()
@@ -94,6 +95,18 @@ def test_sparse_attention_predicate_and_argument_checks_need_no_device(cabi_lib)
     a.D, a.Nq = 40, 16
     assert h.sige_sparse_attention(ctypes.byref(a), None) != 0 and b"null buffer" in h.sige_last_error()
     assert h.sige_sparse_attention(None, None) != 0
+    # scale = 0 would turn the masked keys of a partial last block into -inf * 0 = NaN, scale < 0 would take the running
+    # maximum at the wrong end: refused, as are NaN and infinities, with or without queries (the pointers here are not device
+    # memory, so a launch would fault)
+    P = 0x10000
+    a.q = a.k = a.v = a.out = P
+    for nq in (0, 16):
+        for bad in (0.0, -0.0, -0.158, float("nan"), float("inf"), float("-inf")):
+            a.Nq, a.scale = nq, bad
+            assert h.sige_sparse_attention(ctypes.byref(a), None) != 0, (nq, bad)
+            assert b"scale" in h.sige_last_error() and b"positive and finite" in h.sige_last_error()
+    a.Nq, a.scale = 0, 1e-30                                              # tiny but positive: accepted (a no-op here)
+    assert h.sige_sparse_attention(ctypes.byref(a), None) == 0
 
 
 def _conv_desc(n_tiles, cin, cout, k, *, stride=1, cin2=0, ksplit=0, res=64):

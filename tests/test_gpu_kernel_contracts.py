@@ -12,6 +12,7 @@ import pytest
 import torch
 
 import kernel_contracts as kc
+from kernel_contracts import _launch, _run_and_check
 from tile_conv_contract import DTYPE_NAME
 
 pytestmark = pytest.mark.gpu
@@ -23,42 +24,6 @@ def _lib():
     from sige_b200 import _cabi
 
     return _cabi.lib()
-
-
-def _launch(case, init, call):
-    """Restore every written buffer, run `call` (a C-ABI call returning a status), wait, and return the flat buffers."""
-    from sige_b200 import _cabi
-
-    kc.restore(case.buffers(), init)
-    rc = call()
-    torch.cuda.synchronize()
-    assert rc == 0, _cabi.last_error()
-    return {k: g.flat.clone() for k, g in case.buffers().items()}
-
-
-def _same(a, b):
-    return all(torch.equal(kc.bits(a[k]), kc.bits(b[k])) for k in a)
-
-
-def _report(kernel, label, r):
-    print("[kernel contract] %-10s %-52s worst |err| / bound %.3f, beyond rounding %.3f" % (kernel, label, r[0], r[1]))
-
-
-def _run_and_check(kernel, label, case, expects, call, flag_variants=(0,)):
-    """Launch once per flags value and once more with the first: each within the contract, all bitwise equal."""
-    init = kc.snapshot(case.buffers())
-    inputs0 = {k: t.clone() for k, t in case.inputs().items()}
-    first = None
-    for flags in flag_variants:
-        lab = label + (" pdl" if flags & kc.PDL else "")
-        got = _launch(case, init, lambda: call(flags))
-        _report(kernel, lab, kc.check(lab, expects, got, init, case.inputs(), inputs0))
-        if first is None:
-            first = got
-        else:
-            assert _same(got, first), "%s: programmatic dependent launch changed the result" % lab
-    assert _same(_launch(case, init, lambda: call(flag_variants[0])), first), "%s: a second launch differs" % label
-    return first
 
 
 # ---------------------------------------------------------------------------------------------------------------- separable
