@@ -206,6 +206,23 @@ def _run_and_check(kernel, label, case, expects, call, flag_variants=(0,)):
     return first
 
 
+def graph_equals_stream(case, call):
+    """`call` (a C-ABI call returning a status) captured in a CUDA graph and replayed leaves bitwise what a stream launch does."""
+    init = snapshot(case.buffers())
+    want = _launch(case, init, call)
+    g = torch.cuda.CUDAGraph()
+    restore(case.buffers(), init)
+    torch.cuda.synchronize()
+    with torch.cuda.graph(g):
+        rc = call()
+    assert rc == 0
+    restore(case.buffers(), init)
+    g.replay()
+    torch.cuda.synchronize()
+    got = {k: gb.flat.clone() for k, gb in case.buffers().items()}
+    assert _same(got, want), "a graph replay differs from the stream launch"
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # sige_separable_conv
 # ----------------------------------------------------------------------------------------------------------------------

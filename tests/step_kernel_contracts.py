@@ -1,4 +1,4 @@
-"""The C-ABI contracts of the sparse-query attention, SPADE modulation and the 16-bit tile ops, restated in float64.
+"""The C-ABI contracts of the sparse-query attention, SPADE modulation and the tile ops, restated in float64.
 
 These are the kernels a compiled step launches besides the tile convs and the dense glue: sige_sparse_attention (the SD step's
 attention, and attention cores outside the cluster kernel's range), sige_spade_modulate (the GauGAN steps' SPADE layers that
@@ -17,8 +17,9 @@ Bounds (u = unit roundoff of the launch dtype, U32 = 2^-24):
                     once: (u + 2 U32) |want| + HALF_SUBNORMAL (an f16 result below the normal range rounds to a
                     fixed step).  With g = b = 0 and slope 1 the output is x, bitwise (bound 0).
   tile ops          identity moves: 0 (every path is bitwise exact).  Affine / swish: the fp32 chain's error (U32 per
-                    multiply and add, SWISH_LIP through swish, and the fast swish's own error swish_rel: __expf and __fdividef,
-                    common.cuh swish<true>), plus one rounding u |want| + HALF_SUBNORMAL.  Residual add: U32 + u.
+                    multiply and add, SWISH_LIP through swish, and swish's own error: for 16-bit storage the fast swish's
+                    swish_rel (__expf and __fdividef, common.cuh swish<true>), for f32 the accurate one's SWISH_ACCURATE_REL
+                    (expf and an IEEE division, swish<false>)), plus one rounding u |want| + HALF_SUBNORMAL.  Residual add: U32 + u.
                     scatter_with_block_residual: scatter's rounding restated literally (fp32 add, then the launch dtype),
                     then calibrate's out + (x1 - y1) bounded like a residual add.
 """
@@ -458,7 +459,7 @@ def spade_reference(case: SpadeCase) -> List[Expect]:
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-# sige_gather / sige_scatter / sige_scatter_gather / sige_scatter_with_block_residual in f16 / bf16
+# sige_gather / sige_scatter / sige_scatter_gather / sige_scatter_with_block_residual in f32, f16 and bf16
 # ----------------------------------------------------------------------------------------------------------------------
 ACT_IDENTITY, ACT_SWISH = 0, 1
 TILE_OPS = ("gather", "scatter", "scatter_gather", "swbr")
@@ -472,6 +473,17 @@ def swish_rel(z):
     return (16 + 2 * z.abs()) * U32
 
 
+# expf's maximum error, in ulps of its result, over its whole range (CUDA C++ Programming Guide, "Mathematical Functions":
+# single-precision functions without -use_fast_math)
+EXPF_ULPS = 2
+# The accurate swish z / (1 + expf(-z)) of f32 storage, relative to z sigmoid(z): t = expf(-z) is within EXPF_ULPS ulps of e^-z,
+# a relative error of at most EXPF_ULPS * 2^-23 = 2 EXPF_ULPS U32 (an fp32 ulp is at most 2^-23 of the value); 1 + t rounds once
+# (U32) and moves by less than t's relative error, since t / (1 + t) < 1; the IEEE division rounds once more (U32).  First order
+# 2 EXPF_ULPS + 2 = 6 U32; one U32 more covers the products of these terms.  Much tighter than swish_rel, so f32 switched to the
+# fast intrinsics would not pass unnoticed.
+SWISH_ACCURATE_REL = (2 * EXPF_ULPS + 3) * U32
+
+
 @dataclass(frozen=True)
 class TileSpec:
     """One tile-op launch on a [B, C, H, W] tensor (NCHW or NHWC) and its tile stacks.
@@ -482,7 +494,7 @@ class TileSpec:
     whose pixels come from the stack of 4x4 conv outputs (via the map of get_scatter_map) or the cached tensor.  swbr: scatter
     with the cached shortcut output as residual, then 4x4 calibration tiles at raw origins.
     scale / shift / residual: a broadcast shape (BCAST_SHAPES) or None; aff_dt: "f32" or "x" (the launch dtype).
-    misalign: the destination 2 bytes off 16-byte alignment (on NHWC: the scalar path)."""
+    misalign: the destination one element (4 bytes for f32, 2 for 16 bits) off 16-byte alignment (on NHWC: the scalar path)."""
     name: str
     op: str
     layout: str
@@ -631,7 +643,7 @@ def make_tile(spec: TileSpec, dtype: torch.dtype, device, oracle_safe: bool = Fa
         out_shape = (B * len(o), C, 6, 6)
     else:
         raise ValueError(spec.op)
-    lead = 66 if spec.misalign else 64
+    lead = 64 + (_esize(dtype) if spec.misalign else 0)
     out = guarded(_phys(out_shape, spec.layout), dtype, device, gen, spec.layout, lead_bytes=lead)
     return TileCase(spec, dtype, t, idx, bc, out)
 
@@ -698,8 +710,9 @@ def _bc(case: TileCase, name: str) -> Optional[torch.Tensor]:
     return None if t is None else t.double()
 
 
-def affine_act_bound(z: torch.Tensor, scale, shift, act: int, act_first: bool):
-    """The float64 value of the kernels' affine_act (common.cuh) and a bound on the fp32 evaluation's error."""
+def affine_act_bound(z: torch.Tensor, scale, shift, act: int, act_first: bool, dtype):
+    """The float64 value of the kernels' affine_act (common.cuh) and a bound on the fp32 evaluation's error.  The kernels
+    evaluate swish accurately for f32 storage and with the fast intrinsics for 16-bit storage (tile_ops.cu kFast)."""
     err = torch.zeros_like(z)
 
     def affine(z, err):
@@ -715,7 +728,8 @@ def affine_act_bound(z: torch.Tensor, scale, shift, act: int, act_first: bool):
         z, err = affine(z, err)
     if act == ACT_SWISH:
         y = z * torch.sigmoid(z)
-        err = SWISH_LIP * err + swish_rel(z) * y.abs()
+        rel = SWISH_ACCURATE_REL if dtype == torch.float32 else swish_rel(z)
+        err = SWISH_LIP * err + rel * y.abs()
         z = y
     if act_first:
         z, err = affine(z, err)
@@ -776,7 +790,7 @@ def tile_reference(case: TileCase) -> List[Expect]:
             t = t.expand(B, C, H, W)
             return t[bi[:, None, None], :, hc[:, :, None], wc[:, None, :]].permute(0, 3, 1, 2)
 
-        val, err = affine_act_bound(z, at("scale"), at("shift"), s.act, s.act_first)
+        val, err = affine_act_bound(z, at("scale"), at("shift"), s.act, s.act_first, case.dtype)
         ins = inside[:, None].expand_as(val)
         val, err = torch.where(ins, val, torch.zeros((), dtype=val.dtype, device=dev)), torch.where(ins, err, torch.zeros((), dtype=val.dtype, device=dev))
         finish(val, err, exact=~ins)                                                   # zeros outside the image: exact
@@ -863,6 +877,9 @@ def _tile_cases():
     cases += [
         T("g_nhwc_vec_scale_only", "gather", "nhwc", C=16, scale=(0, 1, 0, 0), seed=40),
         T("g_nhwc_vec_shift_only_swish_first", "gather", "nhwc", C=16, shift=(1, 1, 0, 0), act=ACT_SWISH, act_first=True, seed=41),
+        # C not a multiple of 4: the scalar NHWC path in every dtype, f32 included, with aligned pointers
+        T("g_nhwc_scalar_c6_affine_swish", "gather", "nhwc", C=6, scale=(1, 1, 0, 0), shift=(0, 1, 1, 1), act=ACT_SWISH, seed=42),
+        T("g_nhwc_scalar_c10_up_identity", "gather", "nhwc", C=10, H=20, W=18, up=1, seed=43),
         # scatter: copy and in-place forms, every path, stride 2 with origins -1 and -2, residual in every broadcast shape
         T("s_nchw_copy", "scatter", "nchw", seed=50),
         T("s_nhwc_vec_copy", "scatter", "nhwc", C=32, seed=51),
@@ -875,6 +892,8 @@ def _tile_cases():
         T("s_nchw_stride2", "scatter", "nchw", stride=2, seed=58),
         T("s_nhwc_vec_stride2_inplace", "scatter", "nhwc", C=16, stride=2, inplace=True, seed=59),
         T("s_nhwc_scalar_c12_stride2_residual", "scatter", "nhwc", C=12, stride=2, residual=(0, 1, 0, 0), seed=60),
+        T("s_nhwc_scalar_c6_copy", "scatter", "nhwc", C=6, seed=61),
+        T("s_nhwc_scalar_c10_inplace_residual", "scatter", "nhwc", C=10, inplace=True, residual=(1, 1, 0, 0), seed=62),
     ]
     for i, shp in enumerate(BCAST_SHAPES):
         lay, C, mis = paths[i % 4]
@@ -890,12 +909,15 @@ def _tile_cases():
         T("sg_nchw_affine_x_swish_first", "scatter_gather", "nchw", scale=(0, 1, 1, 1), shift=(1, 1, 1, 1), aff_dt="x", act=ACT_SWISH,
           act_first=True, seed=85),
         T("sg_nhwc_scalar_c12_swish", "scatter_gather", "nhwc", C=12, act=ACT_SWISH, shift=(0, 0, 1, 1), seed=86),
+        T("sg_nhwc_scalar_c10_affine_swish_first", "scatter_gather", "nhwc", C=10, scale=(0, 1, 0, 0), shift=(1, 1, 0, 0), act=ACT_SWISH,
+          act_first=True, seed=87),
         # scatter_with_block_residual
         T("swbr_nchw", "swbr", "nchw", seed=90),
         T("swbr_nhwc_vec", "swbr", "nhwc", C=32, seed=91),
         T("swbr_nhwc_scalar_c12", "swbr", "nhwc", C=12, seed=92),
         T("swbr_nhwc_scalar_misaligned", "swbr", "nhwc", C=16, misalign=True, seed=93),
         T("swbr_nhwc_vec_stride2", "swbr", "nhwc", C=16, stride=2, seed=94),
+        T("swbr_nhwc_scalar_c6", "swbr", "nhwc", C=6, seed=95),
     ]
     return cases
 

@@ -1,4 +1,4 @@
-"""The sparse-query attention, SPADE modulation and the 16-bit tile ops against the float64 restatements of their C-ABI contracts
+"""The sparse-query attention, SPADE modulation and the tile ops against the float64 restatements of their C-ABI contracts
 (tests/step_kernel_contracts.py).
 
 Every launch must be within the per-element bound on every element it writes, leave every other element of every buffer (guard
@@ -20,6 +20,7 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 NAME = {torch.float32: "f32", torch.float16: "f16", torch.bfloat16: "bf16"}
 DT16 = pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16], ids=["f16", "bf16"])
+DTYPES = pytest.mark.parametrize("dtype", [torch.float32, torch.float16, torch.bfloat16], ids=["f32", "f16", "bf16"])
 
 
 def _lib():
@@ -84,13 +85,14 @@ def _device_map(case: sk.TileCase) -> torch.Tensor:
     return m
 
 
-@DT16
+@DTYPES
 @pytest.mark.parametrize("spec", sk.TILE_CASES, ids=lambda s: s.name)
 def test_tile_op_matches_the_float64_contract(spec, dtype):
     case = sk.make_tile(spec, dtype, DEV)
     path = sk.tile_path(spec, dtype)
     ptrs = [case.out.view.data_ptr()] + [case.t[k].data_ptr() for k in ("x", "y") if k in case.t]
-    assert (path == "vec") == (spec.layout == "nhwc" and spec.C % 8 == 0 and all(p % 16 == 0 for p in ptrs)), spec.name
+    vec = 16 // case.out.flat.element_size()
+    assert (path == "vec") == (spec.layout == "nhwc" and spec.C % vec == 0 and all(p % 16 == 0 for p in ptrs)), spec.name
     if spec.op == "scatter_gather":
         m = _device_map(case)
         assert torch.equal(m, case.idx["map"]), "%s: get_scatter_map differs from its restatement" % spec.name
@@ -101,11 +103,11 @@ def test_tile_op_matches_the_float64_contract(spec, dtype):
     _run_and_check("tile_ops", "%s %s (%s)" % (spec.name, NAME[dtype], path), case, expects, lambda flags: sk.tile_call(case, lib, keep))
 
 
-@DT16
+@DTYPES
 @pytest.mark.parametrize("spec", [s for s in sk.TILE_CASES if sk.tile_path(s, torch.float16) == "vec"], ids=lambda s: s.name)
 def test_tile_op_scalar_path_matches_the_vector_path(spec, dtype):
-    """The same inputs through the 16-byte-vector NHWC kernel and, with the destination 2 bytes off alignment, the scalar one:
-    bitwise the same written elements."""
+    """The same inputs through the 16-byte-vector NHWC kernel and, with the destination one element off alignment, the scalar
+    one: bitwise the same written elements."""
     lib = _lib()
     res = []
     for mis in (False, True):
@@ -119,29 +121,14 @@ def test_tile_op_scalar_path_matches_the_vector_path(spec, dtype):
 
 
 # ---------------------------------------------------------------------------------------------------------------- CUDA graphs
-def _graph_equals_stream(case, call):
-    init = kc.snapshot(case.buffers())
-    want = _launch(case, init, call)
-    g = torch.cuda.CUDAGraph()
-    kc.restore(case.buffers(), init)
-    torch.cuda.synchronize()
-    with torch.cuda.graph(g):
-        rc = call()
-    assert rc == 0
-    kc.restore(case.buffers(), init)
-    g.replay()
-    torch.cuda.synchronize()
-    got = {k: gb.flat.clone() for k, gb in case.buffers().items()}
-    assert kc._same(got, want), "a graph replay differs from the stream launch"
-
-
 def test_graph_replay_matches_the_stream_launch():
     lib = _lib()
     spec = next(s for s in sk.SATTN_CASES if s.name == "d40_q65_k130_random_bnhd")
     case = sk.make_sattn(spec, torch.float16, DEV)
     d = sk.sattn_descriptor(case)
-    _graph_equals_stream(case, lambda: sk.sattn_call(case, lib, d))
+    kc.graph_equals_stream(case, lambda: sk.sattn_call(case, lib, d))
     spec = next(s for s in sk.TILE_CASES if s.name.startswith("g_nhwc_1111_afff32"))
-    case = sk.make_tile(spec, torch.bfloat16, DEV)
-    keep = []
-    _graph_equals_stream(case, lambda: sk.tile_call(case, lib, keep))
+    for dt in (torch.bfloat16, torch.float32):
+        case = sk.make_tile(spec, dt, DEV)
+        keep = []
+        kc.graph_equals_stream(case, lambda: sk.tile_call(case, lib, keep))

@@ -257,10 +257,11 @@ def test_tile_op_case_table_covers_every_path():
     cases = sk.TILE_CASES
     for op in sk.TILE_OPS:
         mine = [s for s in cases if s.op == op]
-        for dt in sk.F16_BF16:
-            assert {sk.tile_path(s, dt) for s in mine} == {"nchw", "vec", "scalar"}, op
+        for dt in (torch.float32,) + sk.F16_BF16:
+            vec = 16 // sk._esize(dt)
+            assert {sk.tile_path(s, dt) for s in mine} == {"nchw", "vec", "scalar"}, (op, dt)
             scal = [s for s in mine if sk.tile_path(s, dt) == "scalar"]
-            assert any(s.C % 8 for s in scal) and any(s.misalign and s.C % 8 == 0 for s in scal), op
+            assert any(s.C % vec for s in scal) and any(s.misalign and s.C % vec == 0 for s in scal), (op, dt)
     g = [s for s in cases if s.op == "gather"]
     assert any(s.up for s in g) and {sk.tile_path(s, torch.float16) for s in g if s.up} == {"nchw", "vec", "scalar"}
     for name in ("scale", "shift"):
@@ -273,6 +274,30 @@ def test_tile_op_case_table_covers_every_path():
     assert any(s.inplace for s in sc) and any(not s.inplace for s in sc)
     assert {sk.tile_path(s, torch.float16) for s in sc if s.inplace} == {"nchw", "vec", "scalar"}
     assert any(s.stride == 2 for s in sc) and any(s.op == "scatter_gather" and s.act for s in cases)
+
+
+def test_tile_op_misalignment_is_one_element_in_every_dtype():
+    """A misaligned destination sits one whole element (4 bytes for f32, 2 for 16 bits) off 16-byte alignment, so f32 takes
+    the scalar NHWC path too; the inputs stay aligned and hold the same values."""
+    spec = next(s for s in sk.TILE_CASES if s.name == "s_nhwc_scalar_misaligned_copy")
+    for dt in (torch.float32,) + sk.F16_BF16:
+        case = sk.make_tile(spec, dt, "cpu")
+        es = sk._esize(dt)
+        assert case.out.view.data_ptr() % 16 == es and sk.tile_path(spec, dt) == "scalar", dt
+        assert all(t.data_ptr() % 16 == 0 for t in case.t.values())
+
+
+def test_f32_swish_bound_is_the_accurate_one():
+    """The f32 tile ops evaluate swish as z / (1 + expf(-z)) with an IEEE division: a float32 evaluation of that formula is
+    within SWISH_ACCURATE_REL of z sigmoid(z), which is tighter than the fast intrinsics' swish_rel everywhere."""
+    z = torch.linspace(-30, 30, 200001, dtype=torch.float32)
+    y32 = z / (1 + torch.exp(-z))
+    y = z.double() * torch.sigmoid(z.double())
+    assert bool(((y32.double() - y).abs() <= sk.SWISH_ACCURATE_REL * y.abs() + sk.HALF_SUBNORMAL[torch.float32]).all())
+    assert bool((sk.swish_rel(z.double()) > 2 * sk.SWISH_ACCURATE_REL).all())
+    _, err32 = sk.affine_act_bound(z.double(), None, None, sk.ACT_SWISH, False, torch.float32)
+    _, err16 = sk.affine_act_bound(z.double(), None, None, sk.ACT_SWISH, False, torch.float16)
+    assert torch.equal(err32, sk.SWISH_ACCURATE_REL * y.abs()) and bool((err16 > err32)[y != 0].all())
 
 
 def test_tile_op_geometries_reach_the_edges():
