@@ -31,6 +31,10 @@ class SimExecutor:
     # ------------------------------------------------------------------ fused tile conv
     def prepare_conv(self, fc) -> None:
         s = fc.spec
+        # as in the product executor, whether the launch writes its destination's raw tensor is decided when it is prepared: a
+        # destination with producer-written views and no raw tensor yet keeps receiving only the views, even when the
+        # sparse_update epilogue gives the buffer a raw tensor later; one with neither gets a raw tensor
+        write_raw = s.dst is not None and (s.dst.has_raw or not s.aux)
 
         def run(_stream):
             self.launches += 1
@@ -117,7 +121,7 @@ class SimExecutor:
                         v = out[m, :, r, c].clone()
                         if res is not None and not fresh[m]:
                             v = v + res[bi, :, hh, ww]
-                        if dst.has_raw:
+                        if write_raw:
                             dst.raw[bi, :, hh, ww] = v
                         for (view, sc, sh, act) in s.aux:
                             z = v
@@ -187,8 +191,9 @@ class SimExecutor:
     def prepare_spade(self, x, gamma, beta, slope, out):
         def run(_stream):
             self.launches += 1
-            z = x.float() * (1 + gamma.float()) + beta.float()
-            out.copy_(torch.where(z > 0, z, z * slope))
+            # as the kernel: 1 + gamma in fp32, then one fused multiply-add (a single rounding, here of the float64 value)
+            z = x.double() * (1 + gamma.float()).double() + beta.double()
+            out.copy_(torch.where(z > 0, z, z * float(torch.tensor(slope, dtype=torch.float32))))
 
         return run
 
