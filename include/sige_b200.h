@@ -32,7 +32,7 @@
 extern "C" {
 #endif
 
-#define SIGE_B200_ABI_VERSION 2
+#define SIGE_B200_ABI_VERSION 3
 
 typedef enum { SIGE_F32 = 0, SIGE_F16 = 1, SIGE_BF16 = 2 } sige_dtype_t;
 typedef enum { SIGE_NCHW = 0, SIGE_NHWC = 1 } sige_layout_t;
@@ -179,6 +179,22 @@ typedef struct {
                            the launch writes relu(conv + bias [+ residual])) */
 } sige_conv_aux_t;
 
+/* SPADE's modulation applied in the gather stage of a tile conv (sige_tile_conv_t.modulation): for channel c < Cin of an in-image
+ * halo pixel the conv reads
+ *   a = leaky((x*scale[c] + shift[c]) * (1 + gamma[c]) + beta[c], negative_slope)      (fp32, rounded once to the dtype)
+ * — reference gaugan/models/sige_normalization.py:84-86 plus the block's F.leaky_relu(., 0.2) on the three stacks its Gather /
+ * ScatterGather modules cut, without materialising them.  gamma and beta are NHWC [B, H, W, C] at the source's LOGICAL extent
+ * (B, H, W of the descriptor; the source itself may be read through x2 up-sampling), each read from channels
+ * [c0, c0 + Cin) of its C.  Pixels outside the image and SIGE_TILE_NONE tiles read zero; on a narrow source gamma and beta are
+ * never read at or past Cin. */
+typedef struct {
+    const void *gamma;
+    int gamma_C, gamma_c0;
+    const void *beta;
+    int beta_C, beta_c0;
+    float negative_slope;   /* 1 = no activation (the shortcut SPADE) */
+} sige_conv_modulation_t;
+
 typedef struct {
     int dtype; /* SIGE_F16 / SIGE_BF16 (tensor cores) */
     /* ---- source: where halo tiles are gathered from ----
@@ -232,6 +248,22 @@ typedef struct {
      * than N are padded with SIGE_TILE_NONE origins (such a tile reads zeros and writes nothing).  Weights are read once for
      * the whole batch.  Full-tensor source and destination only (no stacks). */
     int idx_per_image;
+    /* ---- single source read as a channel window of a wider NHWC buffer ----
+     * 0: src[0] has src[0].C channels per pixel.  Otherwise src[0] is channels [c0, c0 + src[0].C) of a buffer with
+     * src_pixel_stride channels per pixel, src[0].ptr pointing at channel c0 of pixel 0 — e.g. one torch.split part of a conv's
+     * output (SPADE's actv_0 / actv_1 / actv_s, reference gaugan/models/spade_generators/sige_fused_spade_generator.py:160-167),
+     * read in place.  The launch is the one of the compacted window (same kernel, plan and result); SIGE_CONV_TC5 is honoured.
+     * Needs n_src == 1, a full-tensor source, no fused shortcut, idx_per_image == 0, a stride that is a multiple of 8 and at
+     * least src[0].C, a 16-byte aligned source, and no modulation. */
+    int src_pixel_stride;
+    /* ---- SPADE's modulation in the gather stage (sige_conv_modulation_t above), or NULL ----
+     * The pre-op is followed by the modulation.  With SIGE_CONV_TC5, the stride-1 wgmma geometries (3x3 on 6x6 tiles, 1x1 on 4x4
+     * tiles, Cin and Cout multiples of 64) run on the wgmma kernel with the plan of the unmodulated launch; everything else (narrow
+     * Cin, other Cout, stride 2, no flag) runs on the mma.sync kernel.  Both stage the same operand.  Needs n_src == 1, a
+     * full-tensor source, act == SIGE_ACT_IDENTITY (negative_slope is the activation), no fused shortcut, idx_per_image == 0, a
+     * finite slope, non-null 16-byte aligned gamma / beta whose windows are multiples of 8 elements within their buffers, and
+     * src_pixel_stride == 0. */
+    const sige_conv_modulation_t *modulation;
 } sige_tile_conv_t;
 
 /* Launch with programmatic dependent launch: the kernel prefetches its weights while the previous kernel
@@ -247,41 +279,10 @@ typedef struct {
 /* Origin of a padding entry of a per-image tile list (both coordinates). */
 #define SIGE_TILE_NONE (-30000)
 
-/* Fused gather -> (affine+SiLU) -> conv (+bias) -> (+residual) -> scatter, one launch. */
+/* Fused gather -> (affine+SiLU) [-> SPADE modulation] -> conv (+bias) -> (+residual) -> scatter, one launch.  Every refusal
+ * comes before any CUDA call: a null descriptor and one with both src_pixel_stride and modulation set first, then a window or a
+ * modulation that lacks what its field needs, then whatever fails the checks every launch makes.  N == 0 is a no-op. */
 int sige_tile_conv(const sige_tile_conv_t *p, sige_stream_t stream);
-
-/* SPADE's modulation applied in the gather stage of a tile conv (sige_tile_conv_modulated): for channel c < Cin of an in-image
- * halo pixel the conv reads
- *   a = leaky((x*scale[c] + shift[c]) * (1 + gamma[c]) + beta[c], negative_slope)      (fp32, rounded once to the dtype)
- * — reference gaugan/models/sige_normalization.py:84-86 plus the block's F.leaky_relu(., 0.2) on the three stacks its Gather /
- * ScatterGather modules cut, without materialising them.  gamma and beta are NHWC [B, H, W, C] at the source's LOGICAL extent
- * (B, H, W of the descriptor; the source itself may be read through x2 up-sampling), each read from channels
- * [c0, c0 + Cin) of its C.  Pixels outside the image and SIGE_TILE_NONE tiles read zero; on a narrow source gamma and beta are
- * never read at or past Cin. */
-typedef struct {
-    const void *gamma;
-    int gamma_C, gamma_c0;
-    const void *beta;
-    int beta_C, beta_c0;
-    float negative_slope;   /* 1 = no activation (the shortcut SPADE) */
-} sige_conv_modulation_t;
-/* Host-only: does sige_tile_conv_modulated take a conv of Cin -> Cout, k x k, this stride, in `dtype`? */
-int sige_tile_conv_modulated_supported(int Cin, int Cout, int k, int stride, int dtype);
-/* sige_tile_conv whose pre-op is followed by the modulation above.  With SIGE_CONV_TC5, the stride-1 wgmma geometries (3x3 on 6x6
- * tiles, 1x1 on 4x4 tiles, Cin and Cout multiples of 64) run on the wgmma kernel with the same plan as sige_tile_conv; everything
- * else (narrow Cin, other Cout, stride 2, no flag) runs on the mma.sync kernel.  Both stage the same operand.
- * Refused before any CUDA call: n_src != 1, a stack source, act != SIGE_ACT_IDENTITY (negative_slope is the activation), a fused
- * shortcut, idx_per_image, gamma / beta windows that overrun their buffer or are not multiples of 8 elements, pointers that are
- * not 16-byte aligned, a non-finite slope.  Everything else is sige_tile_conv's contract; N == 0 is a no-op. */
-int sige_tile_conv_modulated(const sige_tile_conv_t *p, const sige_conv_modulation_t *m, sige_stream_t stream);
-
-/* sige_tile_conv whose single source is a channel window of a wider NHWC buffer: channels [c0, c0 + src[0].C) of a buffer with
- * `src_pixel_stride` channels per pixel, src[0].ptr pointing at channel c0 of pixel 0 — e.g. one torch.split part of a conv's output
- * (SPADE's actv_0 / actv_1 / actv_s, reference gaugan/models/spade_generators/sige_fused_spade_generator.py:160-167), read in place.
- * The launch is the one sige_tile_conv makes for the compacted window (same kernel, plan and result); SIGE_CONV_TC5 is honoured.
- * Refused before any CUDA call: n_src != 1, a stack source, a fused shortcut, idx_per_image, a stride below src[0].C or not a
- * multiple of 8, a source pointer that is not 16-byte aligned.  Everything else is sige_tile_conv's contract; N == 0 is a no-op. */
-int sige_tile_conv_strided(const sige_tile_conv_t *p, int src_pixel_stride, sige_stream_t stream);
 
 /* Residual block: conv1 -> conv2 of one block (reference diffusion/models/ddpm_arch/sige_fused_unet.py:100-131: main_gather ->
  * conv1 -> scatter_gather -> conv2 -> scatter[_with_block_residual]) as ONE call.  `conv2` gathers from the buffer `conv1`
@@ -305,8 +306,9 @@ int sige_tile_conv_generic(const void *x, const void *w, const void *bias, void 
 /* ------------------------------------------------------------------------- */
 /* Launch plan sige_tile_conv would use for a descriptor: pure host logic (no pointer is dereferenced, nothing is
  * launched) — exported so that the tile-width / split-K / ring heuristics can be tested without a GPU (which then plan
- * for 132 SMs).  path 0 with every other field 0: the mma.sync kernel would not take the descriptor either (fp32, a tile
- * that fits no CTA configuration, a ksplit that is not a cluster size, ...). */
+ * for 132 SMs).  A window is planned with its pixel stride and a modulated descriptor (modulation only tested against NULL) with
+ * the kernels that take modulated launches, so the plan is the launch's.  path 0 with every other field 0: the mma.sync kernel
+ * would not take the descriptor either (fp32, a tile that fits no CTA configuration, a ksplit that is not a cluster size, ...). */
 typedef struct {
     int path;      /* 1 = wgmma kernel, 0 = mma.sync kernel */
     int bn;        /* output channels per CTA (64 or 128); mma.sync: 128 = the L configuration (128 GEMM rows), 64 = M (64
@@ -318,8 +320,6 @@ typedef struct {
     int grid_x, grid_y, grid_z;   /* mma.sync: ceil(B*N / tiles per CTA), ceil(Cout / bn), ksplit; deep_ring 0 */
 } sige_tile_conv_plan_t;
 int sige_tile_conv_plan(const sige_tile_conv_t *desc, sige_tile_conv_plan_t *plan);
-/* The same for sige_tile_conv_modulated (the kernel and grid it would use for this descriptor), host-only. */
-int sige_tile_conv_modulated_plan(const sige_tile_conv_t *desc, sige_tile_conv_plan_t *plan);
 
 /* 3x3 / stride 1 / pad 1 convolution with Cin <= 4 (the RGB stem): x NHWC (B,H,W,Cin), w OIHW, out NHWC;
  * up to two extra outputs aux[i] = act(out*scale+shift) (NHWC, Cout channels). */

@@ -108,6 +108,8 @@ class TileConv(Structure):
         ("n_aux", c_int), ("aux", ConvAux * 2),
         ("n_src2", c_int), ("src2", ConvSrc * 2), ("Cin2", c_int), ("w2_packed", c_void_p), ("bias2", c_void_p), ("sc_flags", c_void_p),
         ("idx_per_image", c_int),
+        ("src_pixel_stride", c_int),
+        ("modulation", POINTER(ConvModulation)),
     ]
 
 
@@ -131,13 +133,9 @@ PROTOTYPES = {
     "sige_scatter_gather": (_I, [_P, _P] + [_I] * 10 + [_P, _I, _P, _BP, _BP, _I, _I, _P, _P]),
     "sige_pack_conv_weight": (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _P]),
     "sige_tile_conv": (_I, [POINTER(TileConv), _P]),
-    "sige_tile_conv_modulated_supported": (_I, [_I] * 5),
-    "sige_tile_conv_modulated": (_I, [POINTER(TileConv), POINTER(ConvModulation), _P]),
-    "sige_tile_conv_strided": (_I, [POINTER(TileConv), _I, _P]),
     "sige_resblock": (_I, [POINTER(TileConv), POINTER(TileConv), _P]),
     "sige_tile_conv_generic": (_I, [_P, _P, _P, _P] + [_I] * 14 + [_P]),
     "sige_tile_conv_plan": (_I, [_P, _P]),
-    "sige_tile_conv_modulated_plan": (_I, [_P, _P]),
     "sige_conv_in_nhwc": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P]),
     "sige_conv_in_nhwc_tiles": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _I, _I, _I, _I, _I, _P, _P]),
     "sige_group_norm_fold_workspace": (_I, [_I, _I]),
@@ -171,7 +169,7 @@ def lib() -> ctypes.CDLL:
             fn = getattr(handle, name)  # AttributeError if the symbol is missing: loud by design
             fn.restype = res
             fn.argtypes = args
-        if handle.sige_abi_version() != 2:
+        if handle.sige_abi_version() != 3:
             raise SigeLibraryMissing("sige_b200: ABI version mismatch, rebuild the library")
         _lib = handle
     return _lib

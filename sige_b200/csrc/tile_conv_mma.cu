@@ -21,7 +21,7 @@
 // hold real channels are issued — the skipped ones would add exact zeros.  The epilogue stages the
 // fp32 accumulators in shared memory and writes 16-byte channel vectors straight into the
 // destination tensor (coalesced 128-byte lines per pixel), adding bias and the residual.
-// The MOD instantiations (sige_tile_conv_modulated) apply SPADE's modulation in the same register-staged
+// The MOD instantiations (sige_tile_conv_t.modulation) apply SPADE's modulation in the same register-staged
 // halo path: leaky((x*scale + shift) * (1 + gamma) + beta) with gamma / beta read at the halo pixel, so
 // the modulated tile stack the reference gathers and modulates with pointwise torch calls never exists.
 //
@@ -46,7 +46,7 @@ constexpr int KC = 64;        // channels per K chunk (128 bytes of fp16/bf16 pe
 struct ConvSeg {
     const void *ptr;
     int pitch;   // elements from one pixel to the next: the segment's channel count, or more for a channel window of a wider
-                 // NHWC buffer (sige_tile_conv_strided; ptr then points at the window's first channel)
+                 // NHWC buffer (sige_tile_conv_t.src_pixel_stride; ptr then points at the window's first channel)
     int up;      // nearest x2 upsample on read
 };
 
@@ -428,7 +428,7 @@ constexpr MmaCfg kMmaCfgs[3] = {{128, 128, 288}, {64, 64, 144}, {32, 64, 72}};
 enum { MMA_L = 0, MMA_M = 1, MMA_S = 2 };
 
 // Launch plan of the mma.sync kernel: configuration, tiles per CTA, K split and grid.  Host logic only; the launch and the plan
-// queries (sige_tile_conv_plan, sige_tile_conv_modulated_plan) both take it from mma_plan().
+// query (sige_tile_conv_plan) both take it from mma_plan().
 struct MmaPlan {
     int cfg;      // MMA_L / MMA_M / MMA_S
     int tpc;      // tiles per CTA
@@ -521,7 +521,7 @@ template <typename T, bool MOD> static int launch_tile_conv(ConvParams &p, cudaS
     return launch_cfg<T, MMA_S, 2, 2, 1, 4, 72, 8, MOD>(p, pl, st);
 }
 
-// The mma.sync plan of a descriptor for sige_tile_conv_plan / sige_tile_conv_modulated_plan: fills bn, ksplit and the grid when the
+// The mma.sync plan of a descriptor for sige_tile_conv_plan: fills bn, ksplit and the grid when the
 // mma.sync kernel would take the launch (f16 / bf16, a geometry and a ksplit it accepts, no fused shortcut); otherwise leaves
 // `out` as it is.  No pointer of the descriptor is looked at.
 void mma_plan_of(const sige_tile_conv_t *a, sige_tile_conv_plan_t *out) {
@@ -539,14 +539,35 @@ void mma_plan_of(const sige_tile_conv_t *a, sige_tile_conv_plan_t *out) {
     out->grid_z = pl.ksplit;
 }
 
-bool tc5_supported(const sige_tile_conv_t *a, int pitch0);
-bool tc5_supported_modulated(const sige_tile_conv_t *a);
-int tc5_launch(const sige_tile_conv_t *a, int pitch0, const sige_conv_modulation_t *m, cudaStream_t st);
+bool tc5_supported(const sige_tile_conv_t *a);
+int tc5_launch(const sige_tile_conv_t *a, cudaStream_t st);
 
-// Argument checks and launch of sige_tile_conv; m != nullptr: sige_tile_conv_modulated, pitch0 > 0: sige_tile_conv_strided (whose
-// own refusals come first).  pitch0 = elements per pixel of the single source (0: its channel count).
-static int tile_conv(const sige_tile_conv_t *a, const sige_conv_modulation_t *m, int pitch0, sige_stream_t stream) {
+}  // namespace sige
+
+using namespace sige;
+
+// Argument checks and launch: the window's and the modulation's own refusals come before the checks every launch makes.
+extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) {
     SIGE_REQUIRE(a != nullptr, "sige_tile_conv: null descriptor");
+    SIGE_REQUIRE(a->src_pixel_stride == 0 || a->modulation == nullptr, "sige_tile_conv: a source window cannot be modulated");
+    if (a->src_pixel_stride != 0) {
+        SIGE_REQUIRE(a->n_src == 1, "sige_tile_conv (window): one source segment (got n_src %d)", a->n_src);
+        SIGE_REQUIRE(!a->src_is_stack, "sige_tile_conv (window): the source must be a full tensor read through the tile list, not a stack");
+        SIGE_REQUIRE(a->n_src2 == 0, "sige_tile_conv (window): no fused shortcut");
+        SIGE_REQUIRE(!a->idx_per_image, "sige_tile_conv (window): per-image tile lists are not supported");
+        SIGE_REQUIRE(a->src_pixel_stride >= a->src[0].C && a->src_pixel_stride % 8 == 0,
+                     "sige_tile_conv (window): pixel stride %d must be a multiple of 8 and at least the source's %d channels", a->src_pixel_stride, a->src[0].C);
+        SIGE_REQUIRE(((uintptr_t)a->src[0].ptr & 15) == 0, "sige_tile_conv (window): source is not 16-byte aligned");
+    }
+    const sige_conv_modulation_t *m = a->modulation;
+    if (m) {
+        SIGE_REQUIRE(a->n_src == 1, "sige_tile_conv (modulation): one source segment (got n_src %d)", a->n_src);
+        SIGE_REQUIRE(!a->src_is_stack, "sige_tile_conv (modulation): the source must be a full tensor read through the tile list, not a stack");
+        SIGE_REQUIRE(a->act == SIGE_ACT_IDENTITY, "sige_tile_conv (modulation): act must be identity (negative_slope is the activation)");
+        SIGE_REQUIRE(a->n_src2 == 0, "sige_tile_conv (modulation): no fused shortcut");
+        SIGE_REQUIRE(!a->idx_per_image, "sige_tile_conv (modulation): per-image tile lists are not supported");
+        SIGE_REQUIRE(isfinite(m->negative_slope), "sige_tile_conv (modulation): negative_slope must be finite");
+    }
     SIGE_REQUIRE(a->dtype == SIGE_F16 || a->dtype == SIGE_BF16,
                  "sige_tile_conv: tensor-core path needs f16/bf16 (got dtype %d); use sige_tile_conv_generic", a->dtype);
     SIGE_REQUIRE(a->n_src == 1 || a->n_src == 2, "sige_tile_conv: n_src must be 1 or 2");
@@ -556,12 +577,12 @@ static int tile_conv(const sige_tile_conv_t *a, const sige_conv_modulation_t *m,
     if (a->N == 0) return 0;
     if (m) {
         const int cin = a->Cin;
-        SIGE_REQUIRE(m->gamma && m->beta, "sige_tile_conv_modulated: null gamma / beta");
-        SIGE_REQUIRE(((uintptr_t)m->gamma & 15) == 0 && ((uintptr_t)m->beta & 15) == 0, "sige_tile_conv_modulated: gamma / beta not 16-byte aligned");
+        SIGE_REQUIRE(m->gamma && m->beta, "sige_tile_conv (modulation): null gamma / beta");
+        SIGE_REQUIRE(((uintptr_t)m->gamma & 15) == 0 && ((uintptr_t)m->beta & 15) == 0, "sige_tile_conv (modulation): gamma / beta not 16-byte aligned");
         SIGE_REQUIRE(m->gamma_C % 8 == 0 && m->gamma_c0 % 8 == 0 && m->gamma_c0 >= 0 && m->gamma_c0 + cin <= m->gamma_C,
-                     "sige_tile_conv_modulated: gamma channel window [%d, %d) of %d channels (multiples of 8 within the buffer)", m->gamma_c0, m->gamma_c0 + cin, m->gamma_C);
+                     "sige_tile_conv (modulation): gamma channel window [%d, %d) of %d channels (multiples of 8 within the buffer)", m->gamma_c0, m->gamma_c0 + cin, m->gamma_C);
         SIGE_REQUIRE(m->beta_C % 8 == 0 && m->beta_c0 % 8 == 0 && m->beta_c0 >= 0 && m->beta_c0 + cin <= m->beta_C,
-                     "sige_tile_conv_modulated: beta channel window [%d, %d) of %d channels (multiples of 8 within the buffer)", m->beta_c0, m->beta_c0 + cin, m->beta_C);
+                     "sige_tile_conv (modulation): beta channel window [%d, %d) of %d channels (multiples of 8 within the buffer)", m->beta_c0, m->beta_c0 + cin, m->beta_C);
     }
     int csum = 0;
     bool narrow = false;   // a source whose channel count is a multiple of 8 but not of 64: partial last K chunk
@@ -614,15 +635,14 @@ static int tile_conv(const sige_tile_conv_t *a, const sige_conv_modulation_t *m,
         }
         SIGE_REQUIRE(c2 == a->Cin2 && a->w2_packed && ((uintptr_t)a->w2_packed & 15) == 0, "sige_tile_conv: shortcut channels/weights mismatch");
         SIGE_REQUIRE(!a->src_is_stack && !a->dst_is_stack, "sige_tile_conv: the fused shortcut needs full-tensor source and destination");
-        SIGE_REQUIRE((a->flags & SIGE_CONV_TC5) && tc5_supported(a, 0), "sige_tile_conv: the fused shortcut is implemented by the wgmma kernel only (3x3 stride-1 on 6x6 tiles, SIGE_CONV_TC5)");
+        SIGE_REQUIRE((a->flags & SIGE_CONV_TC5) && tc5_supported(a), "sige_tile_conv: the fused shortcut is implemented by the wgmma kernel only (3x3 stride-1 on 6x6 tiles, SIGE_CONV_TC5)");
         SIGE_REQUIRE(a->sc_flags == nullptr || a->residual != nullptr, "sige_tile_conv: sc_flags given without the cached shortcut (residual)");
     }
-    // Hopper-native path (wgmma + TMA, tile_conv_tc5.cu) when requested and the geometry fits; a modulated launch takes its MOD
-    // instantiations on the stride-1 geometries
-    if ((a->flags & SIGE_CONV_TC5) && (m ? tc5_supported_modulated(a) : tc5_supported(a, pitch0))) return tc5_launch(a, pitch0, m, (cudaStream_t)stream);
+    // Hopper-native path (wgmma + TMA, tile_conv_tc5.cu) when requested and the geometry fits
+    if ((a->flags & SIGE_CONV_TC5) && tc5_supported(a)) return tc5_launch(a, (cudaStream_t)stream);
 
     ConvParams p;
-    p.seg[0] = ConvSeg{a->src[0].ptr, pitch0 > 0 ? pitch0 : a->src[0].C, a->src[0].up};
+    p.seg[0] = ConvSeg{a->src[0].ptr, a->src_pixel_stride > 0 ? a->src_pixel_stride : a->src[0].C, a->src[0].up};
     p.seg[1] = a->n_src == 2 ? ConvSeg{a->src[1].ptr, a->src[1].C, a->src[1].up} : p.seg[0];
     p.C0 = a->src[0].C;
     p.src_is_stack = a->src_is_stack;
@@ -663,39 +683,6 @@ static int tile_conv(const sige_tile_conv_t *a, const sige_conv_modulation_t *m,
     }
     if (a->dtype == SIGE_F16) return launch_tile_conv<__half, false>(p, (cudaStream_t)stream);
     return launch_tile_conv<__nv_bfloat16, false>(p, (cudaStream_t)stream);
-}
-
-}  // namespace sige
-
-using namespace sige;
-
-extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) { return tile_conv(a, nullptr, 0, stream); }
-
-extern "C" int sige_tile_conv_strided(const sige_tile_conv_t *a, int src_pixel_stride, sige_stream_t stream) {
-    SIGE_REQUIRE(a != nullptr, "sige_tile_conv_strided: null descriptor");
-    SIGE_REQUIRE(a->n_src == 1, "sige_tile_conv_strided: one source segment (got n_src %d)", a->n_src);
-    SIGE_REQUIRE(!a->src_is_stack, "sige_tile_conv_strided: the source must be a full tensor read through the tile list, not a stack");
-    SIGE_REQUIRE(a->n_src2 == 0, "sige_tile_conv_strided: no fused shortcut");
-    SIGE_REQUIRE(!a->idx_per_image, "sige_tile_conv_strided: per-image tile lists are not supported");
-    SIGE_REQUIRE(src_pixel_stride >= a->src[0].C && src_pixel_stride % 8 == 0,
-                 "sige_tile_conv_strided: pixel stride %d must be a multiple of 8 and at least the source's %d channels", src_pixel_stride, a->src[0].C);
-    SIGE_REQUIRE(((uintptr_t)a->src[0].ptr & 15) == 0, "sige_tile_conv_strided: source is not 16-byte aligned");
-    return tile_conv(a, nullptr, src_pixel_stride, stream);
-}
-
-extern "C" int sige_tile_conv_modulated_supported(int Cin, int Cout, int k, int stride, int dtype) {
-    return (dtype == SIGE_F16 || dtype == SIGE_BF16) && Cin > 0 && Cin % 8 == 0 && Cout > 0 && Cout % 8 == 0 && k >= 1 && stride >= 1 ? 1 : 0;
-}
-
-extern "C" int sige_tile_conv_modulated(const sige_tile_conv_t *a, const sige_conv_modulation_t *m, sige_stream_t stream) {
-    SIGE_REQUIRE(a != nullptr && m != nullptr, "sige_tile_conv_modulated: null descriptor");
-    SIGE_REQUIRE(a->n_src == 1, "sige_tile_conv_modulated: one source segment (got n_src %d)", a->n_src);
-    SIGE_REQUIRE(!a->src_is_stack, "sige_tile_conv_modulated: the source must be a full tensor read through the tile list, not a stack");
-    SIGE_REQUIRE(a->act == SIGE_ACT_IDENTITY, "sige_tile_conv_modulated: act must be identity (negative_slope is the activation)");
-    SIGE_REQUIRE(a->n_src2 == 0, "sige_tile_conv_modulated: no fused shortcut");
-    SIGE_REQUIRE(!a->idx_per_image, "sige_tile_conv_modulated: per-image tile lists are not supported");
-    SIGE_REQUIRE(isfinite(m->negative_slope), "sige_tile_conv_modulated: negative_slope must be finite");
-    return tile_conv(a, m, 0, stream);
 }
 
 // conv1 -> conv2 of one residual block as one call (see include/sige_b200.h).

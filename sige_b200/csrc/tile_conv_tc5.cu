@@ -99,7 +99,7 @@ struct Params {
     int ksplit;
     int pdl;                   // launched with programmatic dependent launch: the next layer is released at the epilogue
     int is_bf16;
-    // SPADE modulation in the gather stage (MOD instantiations only, sige_tile_conv_modulated): gamma / beta are NHWC at the logical
+    // SPADE modulation in the gather stage (MOD instantiations only, sige_tile_conv_t.modulation): gamma / beta are NHWC at the logical
     // source extent with gC / bC elements per pixel, each pointing at the first channel of its window (sige_conv_modulation_t's c0);
     // slope is the leaky-ReLU slope.  The fields take the padding before `trace` and the tail up to the tensor maps' 64-byte-aligned
     // parameter offset, so every other field and both tensor maps keep their offsets.
@@ -1219,8 +1219,9 @@ static bool tc5_is_s2(const sige_tile_conv_t *a) {
 }
 
 // Can the wgmma kernel take this layer?  (3x3 stride 1 on 6x6 tiles, 1x1 on 4x4 tiles, or 3x3 stride 2 on 5x5 tiles; Cout % 64 == 0)
-// pitch0: elements per pixel of the first source (0: its channel count).
-bool tc5_supported(const sige_tile_conv_t *a, int pitch0) {
+// A modulated layer takes the stride-1 geometries only: the stride-2 one has no register-staged gather.
+bool tc5_supported(const sige_tile_conv_t *a) {
+    if (a->modulation && a->stride != 1) return false;
     const bool g3 = (a->kH == 3 && a->kW == 3 && a->stride == 1 && a->R == 6 && a->S == 6) || tc5_is_s2(a);
     const bool g1 = a->kH == 1 && a->kW == 1 && a->stride == 1 && a->R == 4 && a->S == 4;
     if (a->n_src2 > 0 && !g3) return false;
@@ -1228,7 +1229,7 @@ bool tc5_supported(const sige_tile_conv_t *a, int pitch0) {
     const long long px = a->src_is_stack ? (long long)a->B * a->N * a->R * a->S : (long long)a->B * a->H * a->W;
     long long cmax = 0;
     for (int i = 0; i < a->n_src; ++i) {
-        const int pitch = (i == 0 && pitch0 > 0) ? pitch0 : a->src[i].C;
+        const int pitch = (i == 0 && a->src_pixel_stride > 0) ? a->src_pixel_stride : a->src[i].C;
         cmax = pitch > cmax ? pitch : cmax;
     }
     if (px * cmax >= (1ll << 31)) return false;
@@ -1237,14 +1238,10 @@ bool tc5_supported(const sige_tile_conv_t *a, int pitch0) {
     return (g3 || g1) && a->Cout % 64 == 0 && a->Cin % 64 == 0 && (a->ksplit == 0 || a->ksplit == 1 || a->ksplit == 2 || a->ksplit == 4 || a->ksplit == 8);
 }
 
-// ... and a modulated one (sige_tile_conv_modulated)?  The stride-1 geometries only: the stride-2 one has no register-staged gather.
-bool tc5_supported_modulated(const sige_tile_conv_t *a) { return a->stride == 1 && tc5_supported(a, 0); }
-
-// Arguments were validated by sige_tile_conv (tile_conv_mma.cu) before this is called; m != nullptr: a modulated launch
-// (tc5_supported_modulated).
-int tc5_launch(const sige_tile_conv_t *a, int pitch0, const sige_conv_modulation_t *m, cudaStream_t st) {
+// Arguments were validated by sige_tile_conv (tile_conv_mma.cu) before this is called.
+int tc5_launch(const sige_tile_conv_t *a, cudaStream_t st) {
     tc5::Params p;
-    p.seg[0] = tc5::Seg{a->src[0].ptr, pitch0 > 0 ? pitch0 : a->src[0].C, a->src[0].up};
+    p.seg[0] = tc5::Seg{a->src[0].ptr, a->src_pixel_stride > 0 ? a->src_pixel_stride : a->src[0].C, a->src[0].up};
     p.seg[1] = a->n_src == 2 ? tc5::Seg{a->src[1].ptr, a->src[1].C, a->src[1].up} : p.seg[0];
     p.C0 = a->src[0].C;
     p.src_is_stack = a->src_is_stack;
@@ -1276,6 +1273,7 @@ int tc5_launch(const sige_tile_conv_t *a, int pitch0, const sige_conv_modulation
     p.pdl = (a->flags & SIGE_CONV_PDL) ? 1 : 0;
     p.is_bf16 = a->dtype == SIGE_BF16;
     p.trace = g_trace;
+    const sige_conv_modulation_t *m = a->modulation;
     const size_t esz = 2;                                                  // f16 / bf16
     p.gamma = m ? static_cast<const char *>(m->gamma) + (size_t)m->gamma_c0 * esz : nullptr;
     p.beta = m ? static_cast<const char *>(m->beta) + (size_t)m->beta_c0 * esz : nullptr;
@@ -1326,18 +1324,7 @@ extern "C" int sige_tile_conv_plan(const sige_tile_conv_t *a, sige_tile_conv_pla
     using namespace sige;
     SIGE_REQUIRE(a && out, "sige_tile_conv_plan: null pointer");
     out->path = 0; out->bn = 0; out->ksplit = 0; out->deep_ring = 0; out->grid_x = out->grid_y = out->grid_z = 0;
-    if ((a->flags & SIGE_CONV_TC5) && tc5_supported(a, 0)) tc5_plan(a, out);
-    else mma_plan_of(a, out);
-    return 0;
-}
-
-// The same for sige_tile_conv_modulated: the wgmma kernel's MOD instantiations take the stride-1 wgmma geometries, everything else
-// runs on mma.sync.
-extern "C" int sige_tile_conv_modulated_plan(const sige_tile_conv_t *a, sige_tile_conv_plan_t *out) {
-    using namespace sige;
-    SIGE_REQUIRE(a && out, "sige_tile_conv_modulated_plan: null pointer");
-    out->path = 0; out->bn = 0; out->ksplit = 0; out->deep_ring = 0; out->grid_x = out->grid_y = out->grid_z = 0;
-    if ((a->flags & SIGE_CONV_TC5) && tc5_supported_modulated(a)) tc5_plan(a, out);
+    if ((a->flags & SIGE_CONV_TC5) && tc5_supported(a)) tc5_plan(a, out);
     else mma_plan_of(a, out);
     return 0;
 }

@@ -39,6 +39,7 @@ inject a CPU simulator of the launch descriptors to check the lowering without a
 from __future__ import annotations
 
 import copy
+import ctypes
 import math
 from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple
 
@@ -341,9 +342,8 @@ class CudaExecutor:
         d.n_src = len(s.srcs)
         for i, (t, up) in enumerate(s.srcs):
             d.src[i].ptr, d.src[i].C, d.src[i].up = t.data_ptr(), t.shape[1], up
-        pitch = 0                           # a channel window of a wider buffer: the strided launch
         if not s.src_is_stack and len(s.srcs) == 1 and not s.srcs[0][0].is_contiguous(memory_format=torch.channels_last):
-            pitch = ops.channel_window(s.srcs[0][0])[1]
+            d.src_pixel_stride = ops.channel_window(s.srcs[0][0])[1]        # a channel window of a wider buffer
         d.B, d.H, d.W = s.B, s.H, s.W
         d.src_is_stack = 1 if s.src_is_stack else 0
         idx_t, n_per, sc_flags_t = s.idx, s.N, (None if s.shortcut is None else s.shortcut[3])
@@ -391,14 +391,12 @@ class CudaExecutor:
             a = d.aux[0]
             a.ptr, a.C, a.c0, a.scale, a.shift, a.act = d.dst, d.dC, d.dst_c0, None, None, ops._cabi.ACT_RELU
             d.dst, d.n_aux = None, 1
-        d.n_src2 = 0
-        if s.modulation is not None:       # the mma.sync kernel with SPADE's modulation in its gather stage
-            assert not pitch, s.name
+        if s.modulation is not None:       # SPADE's modulation in the gather stage
             gamma, beta, slope = s.modulation
             mod = ops.conv_modulation(gamma, beta, slope)
-            fc.desc, fc.keep = d, keep + [idx_t, mod]
-            fc.launch_fn = lambda stream, d=d, mod=mod: ops.launch_tile_conv_modulated(d, mod, stream)
-            return
+            d.modulation = ctypes.pointer(mod)
+            keep.append(mod)
+        d.n_src2 = 0
         if s.shortcut is not None:
             sc_tensors, sc_w, sc_b, sc_flags = s.shortcut
             w2 = self._pack(sc_w, s.shortcut_key)
@@ -413,9 +411,6 @@ class CudaExecutor:
             keep += [w2, b2]
         keep += [idx_t, sc_flags_t]
         fc.desc, fc.keep = d, keep
-        if pitch:
-            fc.launch_fn = lambda stream, d=d, pitch=pitch: ops.launch_tile_conv_strided(d, pitch, stream)
-            return
         fc.launch_fn = lambda stream, d=d: ops.launch_tile_conv(d, stream)
 
     def prepare_conv_in(self, rec: ConvInRec) -> Callable[[int], None]:
@@ -498,15 +493,15 @@ class CudaExecutor:
     def narrow_conv_supported(self, cin: int, cout: int, k: int, stride: int) -> bool:
         """Can sige_tile_conv run a conv whose single source has `cin` channels, a multiple of 8 but not of 64 (the mma.sync
         kernel with a partial last K chunk)?"""
-        return self.ops.tile_conv_narrow_supported(cin, cout, k, stride, self.dtype)
+        return cin % 64 != 0 and self.ops.tile_conv_supported(cin, cout, k, stride, self.dtype)
 
     def modulated_conv_supported(self, cin: int, cout: int, k: int, stride: int) -> bool:
-        """Can sige_tile_conv_modulated run a conv whose source is SPADE's modulation of `cin` channels?"""
-        return self.ops.tile_conv_modulated_supported(cin, cout, k, stride, self.dtype)
+        """Can sige_tile_conv run a conv whose source is SPADE's modulation of `cin` channels?"""
+        return self.ops.tile_conv_supported(cin, cout, k, stride, self.dtype)
 
     def strided_conv_supported(self, cin: int, cout: int, k: int, stride: int) -> bool:
-        """Can sige_tile_conv_strided run a conv whose source is a `cin`-channel window of a wider buffer?"""
-        return self.ops.tile_conv_strided_supported(cin, cout, k, stride, self.dtype)
+        """Can sige_tile_conv run a conv whose source is a `cin`-channel window of a wider buffer?"""
+        return self.ops.tile_conv_supported(cin, cout, k, stride, self.dtype)
 
     def _separable_weights(self, dw: "DWConv", pw_w: torch.Tensor, pw_b: Optional[torch.Tensor]):
         """(depthwise weight, bias with the affine folded in fp32; 1x1 weight in the step's dtype; fp32 1x1 bias), cached by the
@@ -612,7 +607,7 @@ class ModStack(Stack):
     """SPADE's modulation of three lazy Stacks cut with one tile list: the tiles of `src` (with the Gather's scale / shift) times
     (1 + the same tiles of `gamma`) plus those of `beta`, then leaky_relu(slope).  gamma / beta are channels [c0, c0 + C) of their
     buffers (C = the source's channels; c0 > 0: a torch.split window).  Only ever the source of a ConvOut: the conv's launch applies
-    it in its gather stage (sige_tile_conv_modulated), so none of the stacks is materialised."""
+    it in its gather stage (sige_tile_conv_t.modulation), so none of the stacks is materialised."""
 
     def __init__(self, x: Stack, gamma: "Buf", beta: "Buf", slope: float, gamma_c0: int = 0, beta_c0: int = 0):
         super().__init__(x.src, x.gather, x.scale, x.shift)
@@ -622,7 +617,7 @@ class ModStack(Stack):
 
 class WinStack(Stack):
     """The tiles of channels [c0, c0 + C) of a plain lazy Stack of one buffer (a torch.split part of it: SPADE's actv_0 / actv_1 /
-    actv_s).  Only ever the source of a ConvOut: the launch reads the window in place (sige_tile_conv_strided)."""
+    actv_s).  Only ever the source of a ConvOut: the launch reads the window in place (sige_tile_conv_t.src_pixel_stride)."""
 
     def __init__(self, st: Stack, c0: int, C: int):
         super().__init__(st.src, st.gather, st.scale, st.shift)

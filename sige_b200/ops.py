@@ -337,23 +337,11 @@ def tile_conv_tc_supported(x: torch.Tensor, weight: torch.Tensor, stride, dilati
     )
 
 
-def tile_conv_narrow_supported(cin: int, cout: int, k: int, stride: int, dtype: torch.dtype) -> bool:
-    """Does ``sige_tile_conv`` take a single source of `cin` channels, a multiple of 8 but not of 64?  (The mma.sync kernel with a
-    partial last K chunk; the weight is packed zero-padded to round_up(cin, 64) input channels.)"""
-    return dtype in (torch.float16, torch.bfloat16) and cin > 0 and cin % 8 == 0 and cin % 64 != 0 and cout > 0 and cout % 8 == 0 \
-        and k >= 1 and stride >= 1
-
-
-def tile_conv_modulated_supported(cin: int, cout: int, k: int, stride: int, dtype: torch.dtype) -> bool:
-    """Does ``sige_tile_conv_modulated`` (SPADE's modulation in the gather stage) take this conv?  With the wgmma flag, the wgmma
-    kernel runs the stride-1 geometries whose Cin and Cout are multiples of 64; the mma.sync kernel runs the rest."""
-    code = {torch.float16: _cabi.F16, torch.bfloat16: _cabi.BF16}.get(dtype)
-    return code is not None and bool(_cabi.lib().sige_tile_conv_modulated_supported(int(cin), int(cout), int(k), int(stride), code))
-
-
-def tile_conv_strided_supported(cin: int, cout: int, k: int, stride: int, dtype: torch.dtype) -> bool:
-    """Does ``sige_tile_conv_strided`` take a conv whose single source is a `cin`-channel window of a wider buffer?  (The window is
-    a multiple of 8 channels, like its offset and the buffer's width; one of 64 is the plain tensor-core launch, else the narrow one.)"""
+def tile_conv_supported(cin: int, cout: int, k: int, stride: int, dtype: torch.dtype) -> bool:
+    """Does ``sige_tile_conv`` take a conv of `cin` -> `cout` channels with a single source, whatever the source is: a narrow one
+    (cin a multiple of 8 but not of 64: the mma.sync kernel with a partial last K chunk, the weight packed zero-padded to
+    round_up(cin, 64) input channels), a channel window of a wider buffer, or SPADE's modulation in the gather stage?  With the wgmma
+    flag, the wgmma kernel runs the geometries it takes; the mma.sync kernel runs the rest."""
     return dtype in (torch.float16, torch.bfloat16) and cin > 0 and cin % 8 == 0 and cout > 0 and cout % 8 == 0 and k >= 1 and stride >= 1
 
 
@@ -389,17 +377,6 @@ def conv_modulation(gamma: torch.Tensor, beta: torch.Tensor, negative_slope: flo
     m.beta, m.beta_C, m.beta_c0 = b, bC, bc0 + int(beta_c0)
     m.negative_slope = float(negative_slope)
     return m
-
-
-def launch_tile_conv_modulated(desc: TileConv, mod: "_cabi.ConvModulation", stream: int) -> None:
-    _cabi.check(_cabi.lib().sige_tile_conv_modulated(byref(desc), byref(mod), stream), "sige_tile_conv_modulated")
-    _bump()
-
-
-def launch_tile_conv_strided(desc: TileConv, src_pixel_stride: int, stream: int) -> None:
-    """sige_tile_conv_strided: the single source is a channel window of a buffer with `src_pixel_stride` channels per pixel."""
-    _cabi.check(_cabi.lib().sige_tile_conv_strided(byref(desc), int(src_pixel_stride), stream), "sige_tile_conv_strided")
-    _bump()
 
 
 def tile_conv_stack(x: torch.Tensor, w_packed: torch.Tensor, bias_f32: Optional[torch.Tensor], ksize: Tuple[int, int],

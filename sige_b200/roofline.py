@@ -145,15 +145,13 @@ def measure_engine(engine, flush, reps: int = 5):
 
 
 def plan_of(fc):
-    """The launch plan (sige_tile_conv_plan_t) of a FusedConv: the kernel and grid its launch uses.  Modulated launches are planned by
-    sige_tile_conv_modulated_plan, which knows which of them run on the wgmma kernel."""
+    """The launch plan (sige_tile_conv_plan_t) of a FusedConv: the kernel and grid its launch uses."""
     import ctypes
 
     from . import _cabi
 
     pl = _cabi.TileConvPlan()
-    query = _cabi.lib().sige_tile_conv_modulated_plan if fc.spec.modulation is not None else _cabi.lib().sige_tile_conv_plan
-    _cabi.check(query(ctypes.byref(fc.desc), ctypes.byref(pl)), "tile-conv plan")
+    _cabi.check(_cabi.lib().sige_tile_conv_plan(ctypes.byref(fc.desc), ctypes.byref(pl)), "sige_tile_conv_plan")
     return pl
 
 

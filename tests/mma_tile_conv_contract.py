@@ -16,7 +16,7 @@ restatement against sige_tile_conv_plan, the case table's coverage) and tests/te
 """
 from __future__ import annotations
 
-from ctypes import byref
+from ctypes import byref, pointer
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Tuple
 
@@ -137,7 +137,7 @@ class Spec:
     residual: Optional[Tuple[int, int]] = None # (extra channels, res_c0)
     aux: Tuple[Tuple[int, int, bool, int], ...] = ()   # (extra channels, c0, affine, act) per aux destination
     mod: Optional[Tuple[int, int, int, int, float]] = None   # SPADE modulation: gamma (extra, c0), beta (extra, c0), slope
-    window: Optional[Tuple[int, int]] = None   # sige_tile_conv_strided: the source is channels [c0, c0 + Cin) of (extra + Cin)
+    window: Optional[Tuple[int, int]] = None   # src_pixel_stride: the source is channels [c0, c0 + Cin) of (extra + Cin)
     c_div_tile: bool = False                   # move the first grid tile of image 0 up / left by one pixel (stride 2)
     ksplits: Tuple[int, ...] = (0,)
     expect: str = "S"                          # the configuration the case is meant for
@@ -568,6 +568,10 @@ def descriptor(case: Case, ksplit: int = 0, flags: int = 0):
         d.aux[i].ptr, d.aux[i].C, d.aux[i].c0 = a.g.view.data_ptr(), a.g.view.shape[3], a.c0
         d.aux[i].scale, d.aux[i].shift, d.aux[i].act = _ptr(a.scale), _ptr(a.shift), a.act
     d.idx_per_image = 1 if s.per_image else 0
+    if s.window:
+        d.src_pixel_stride = case.src_bufs[0].shape[3]
+    if s.mod:
+        d.modulation = pointer(modulation(case))
     d._keep = case
     return d
 
@@ -583,13 +587,12 @@ def modulation(case: Case):
     return m
 
 
-def plan_of(d, modulated: bool = False):
-    """sige_tile_conv_plan / sige_tile_conv_modulated_plan of a descriptor."""
+def plan_of(d):
+    """sige_tile_conv_plan of a descriptor."""
     from sige_b200 import _cabi
 
     p = _cabi.TileConvPlan()
-    query = _cabi.lib().sige_tile_conv_modulated_plan if modulated else _cabi.lib().sige_tile_conv_plan
-    _cabi.check(query(byref(d), byref(p)), "tile-conv plan")
+    _cabi.check(_cabi.lib().sige_tile_conv_plan(byref(d), byref(p)), "sige_tile_conv_plan")
     return p
 
 
@@ -599,17 +602,6 @@ def plan_tuple(p):
 
 def expected_plan_tuple(p: Optional[Plan]):
     return (0, 0, 0, 0, 0, 0, 0) if p is None else (0, p.bn, p.ksplit, 0) + p.grid
-
-
-def launch(case: Case, d, stream: int) -> None:
-    from sige_b200 import ops
-
-    if case.spec.mod:
-        ops.launch_tile_conv_modulated(d, modulation(case), stream)
-    elif case.spec.window:
-        ops.launch_tile_conv_strided(d, case.src_bufs[0].shape[3], stream)
-    else:
-        ops.launch_tile_conv(d, stream)
 
 
 # ----------------------------------------------------------------------------------------------------------------------

@@ -26,12 +26,12 @@ def test_library_exports_every_declared_symbol(cabi_lib):
         assert hasattr(lib, name), "libsige_b200.so does not export %s" % name
 
 
-def test_prototype_table_matches_header(cabi_lib):
+def test_prototype_table_matches_the_abi_3_header(cabi_lib):
     from sige_b200 import _cabi
 
     assert set(_cabi.PROTOTYPES) == _declared()
     lib = _cabi.lib()
-    assert lib.sige_abi_version() == 2
+    assert lib.sige_abi_version() == 3
     assert lib.sige_built_arch() == b"sm_90a"
     assert lib.sige_activation_from_name(b"identity") == 0
     assert lib.sige_activation_from_name(b"swish") == 1

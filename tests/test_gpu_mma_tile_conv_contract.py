@@ -1,7 +1,8 @@
 """Every configuration and geometry of the mma.sync tile conv against the float64 restatement of its descriptor
 (tests/mma_tile_conv_contract.py).
 
-For each case of mc.CASES, in fp16 and bf16, at every ksplit the case lists:
+For each case of mc.CASES (those whose descriptor sets a source window or a modulation in a test of their own), in fp16 and bf16,
+at every ksplit the case lists:
   * the plan the library reports on this device equals the restated heuristic's (configuration, tiles per CTA, K split, grid) and is
     the configuration the case is meant for — a mismatch fails: the case would test something else;
   * the launch, with and without programmatic dependent launch, is within the per-element bound on every element it writes, and
@@ -20,8 +21,10 @@ DEV = "cuda:0"
 
 
 def _run(case, init, d):
+    from sige_b200 import ops
+
     kc.restore(case.buffers(), init)
-    mc.launch(case, d, torch.cuda.current_stream().cuda_stream)
+    ops.launch_tile_conv(d, torch.cuda.current_stream().cuda_stream)
     torch.cuda.synchronize()
     return kc.snapshot(case.buffers())
 
@@ -30,9 +33,24 @@ def _same(a, b):
     return all(torch.equal(kc.bits(a[k]), kc.bits(b[k])) for k in a)
 
 
+PLAIN_CASES = [s for s in mc.CASES if not (s.mod or s.window)]
+FIELD_CASES = [s for s in mc.CASES if s.mod or s.window]
+
+
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16], ids=["f16", "bf16"])
-@pytest.mark.parametrize("spec", mc.CASES, ids=lambda s: s.name)
+@pytest.mark.parametrize("spec", PLAIN_CASES, ids=lambda s: s.name)
 def test_mma_tile_conv_matches_the_float64_contract(spec, dtype):
+    _sweep(spec, dtype)
+
+
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16], ids=["f16", "bf16"])
+@pytest.mark.parametrize("spec", FIELD_CASES, ids=lambda s: s.name)
+def test_mma_tile_conv_window_and_modulation_fields_match_the_float64_contract(spec, dtype):
+    """The cases whose descriptor sets src_pixel_stride or modulation."""
+    _sweep(spec, dtype)
+
+
+def _sweep(spec, dtype):
     sms = torch.cuda.get_device_properties(DEV).multi_processor_count
     case = mc.make_case(spec, dtype, DEV)
     expects = mc.reference(case)
@@ -44,7 +62,7 @@ def test_mma_tile_conv_matches_the_float64_contract(spec, dtype):
     for ks in spec.ksplits:
         d = mc.descriptor(case, ks, padded)
         want = spec.plan(ks, sms)
-        got = mc.plan_of(d, modulated=spec.mod is not None)
+        got = mc.plan_of(d)
         label = "%s %s ksplit %d -> %s%s tpc %d grid %dx%dx%d" % ((spec.name, mc.DTYPE_NAME[dtype], ks, want.config, " MOD" if spec.mod else "",
                                                                   want.tpc) + want.grid)
         assert mc.plan_tuple(got) == mc.expected_plan_tuple(want), "%s: the library plans %s" % (label, mc.plan_tuple(got))

@@ -3,8 +3,8 @@
   * the float64 restatement agrees with the C oracle's gather -> conv2d_tiles -> scatter composite (fp32 arithmetic, so to 1e-6)
     on non-square tiles and kernels, stride 2 with a negative origin, channel windows and Cout 72, and with plain F.conv2d in
     float64 on stacks (to 1e-12);
-  * the Python restatement of the launch plan equals sige_tile_conv_plan / sige_tile_conv_modulated_plan on random descriptors
-    (without a device the library plans for 132 SMs), hand-worked points of every branch included;
+  * the Python restatement of the launch plan equals sige_tile_conv_plan on random descriptors, modulated or not (without a device
+    the library plans for 132 SMs), hand-worked points of every branch included;
   * the GPU sweep's case table reaches all 12 instantiations (f16 / bf16 x L / M / S x plain / MOD) and every required feature,
     and no case that claims a configuration could be mistaken for another from the plan's (bn, grid);
   * launches the kernel cannot run are refused before anything is launched, each with its own message;
@@ -83,7 +83,7 @@ def test_stack_reference_is_a_plain_convolution(spec):
 
 
 # ---------------------------------------------------------------------------------------------------------------- the plan
-def _host_desc(NT=16, R=6, S=6, k=(3, 3), stride=1, cin=64, cout=64, ksplit=0, B=1, flags=0):
+def _host_desc(NT=16, R=6, S=6, k=(3, 3), stride=1, cin=64, cout=64, ksplit=0, B=1, flags=0, modulated=False):
     """A descriptor whose pointers are not device memory: only argument checks and the plan may look at it."""
     from sige_b200 import _cabi
 
@@ -96,6 +96,8 @@ def _host_desc(NT=16, R=6, S=6, k=(3, 3), stride=1, cin=64, cout=64, ksplit=0, B
     d.Cin, d.Cout, d.kH, d.kW, d.stride = cin, cout, k[0], k[1], stride
     d.dst, d.dH, d.dW, d.dC = 0x50000, 64, 64, cout
     d.ksplit, d.flags = ksplit, flags
+    if modulated:
+        d.modulation = ctypes.pointer(_cabi.ConvModulation())
     return d
 
 
@@ -127,7 +129,7 @@ def test_plan_branches_by_hand(cabi_lib):
     assert both(NT=5, R=5, S=5) == mc.Plan("S", 2, 2, (3, 1, 2))
 
 
-def test_plan_equals_its_restatement_on_random_descriptors(cabi_lib):
+def test_plan_of_plain_and_modulated_descriptors_equals_its_restatement(cabi_lib):
     rng = np.random.default_rng(7)
     seen, filled = set(), 0
     for _ in range(600):
@@ -140,7 +142,8 @@ def test_plan_equals_its_restatement_on_random_descriptors(cabi_lib):
         ks = int(rng.choice([0, 0, 1, 2, 4, 8]))
         p = mc.plan(NT, R, S, kH, kW, stride, cin, cout, ks)
         for modulated in (False, True):
-            got = mc.plan_of(_host_desc(NT=NT, R=R, S=S, k=(kH, kW), stride=stride, cin=cin, cout=cout, ksplit=ks, B=B, flags=mc.PDL), modulated)
+            got = mc.plan_of(_host_desc(NT=NT, R=R, S=S, k=(kH, kW), stride=stride, cin=cin, cout=cout, ksplit=ks, B=B, flags=mc.PDL,
+                                        modulated=modulated))
             assert mc.plan_tuple(got) == mc.expected_plan_tuple(p), (NT, R, S, kH, kW, stride, cin, cout, ks)
         seen.add(None if p is None else p.config)
         filled += p is not None

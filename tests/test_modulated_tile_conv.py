@@ -1,5 +1,6 @@
-"""Modulated tile convs: sige_tile_conv_modulated applies SPADE's modulation leaky((x*scale + shift) * (1 + gamma) + beta) in the tile
-conv's gather stage, so the sub-mobile GauGAN generator's SPADE layers lower to one launch each and nothing is materialised.
+"""Modulated tile convs: sige_tile_conv with `modulation` set applies SPADE's modulation leaky((x*scale + shift) * (1 + gamma) + beta)
+in the tile conv's gather stage, so the sub-mobile GauGAN generator's SPADE layers lower to one launch each and nothing is
+materialised.
 
 CPU: the C-ABI's refusals and predicate; the float64 contract's modulated gather against the C oracle's gather -> modulate -> conv ->
 scatter composite; the sub-mobile generator lowered on the descriptor simulator with a CPU restatement of the modulated launch; the
@@ -28,7 +29,7 @@ import tile_conv_contract as TC  # noqa: E402
 
 # ---------------------------------------------------------------------------------------------------------------- C-ABI (CPU)
 def _host_desc(cin=64, cout=64, k=3, stride=1, N=16):
-    """Descriptor + modulation whose pointers are not device memory: only argument checks may look at them."""
+    """Descriptor pointing at its modulation, whose pointers are not device memory: only argument checks may look at them."""
     from sige_b200 import _cabi
 
     d = _cabi.TileConv()
@@ -42,10 +43,11 @@ def _host_desc(cin=64, cout=64, k=3, stride=1, N=16):
     d.offH = d.offW = 1 if (k == 3 and stride == 1) else 0
     m = _cabi.ConvModulation()
     m.gamma, m.gamma_C, m.beta, m.beta_C, m.negative_slope = 0x60000, cin, 0x70000, cin, 0.2
+    d.modulation = ctypes.pointer(m)
     return d, m
 
 
-def test_modulated_refusals_come_before_any_cuda_call(cabi_lib):
+def test_modulation_field_refusals_come_before_any_cuda_call(cabi_lib):
     """Each refusal returns non-zero with its own message (a descriptor that passed the checks would fail at the device
     instead, with a different message: there is no device here)."""
     from sige_b200 import _cabi
@@ -55,7 +57,7 @@ def test_modulated_refusals_come_before_any_cuda_call(cabi_lib):
     def refused(change, what):
         d, m = _host_desc()
         change(d, m)
-        assert lib.sige_tile_conv_modulated(ctypes.byref(d), ctypes.byref(m), None) != 0
+        assert lib.sige_tile_conv(ctypes.byref(d), None) != 0
         assert what in lib.sige_last_error(), (what, lib.sige_last_error())
 
     def two_sources(d, m):
@@ -81,26 +83,32 @@ def test_modulated_refusals_come_before_any_cuda_call(cabi_lib):
     refused(setter(beta_c0=-8, beta_C=64), b"beta channel window")
     refused(setter(gamma=0x60008), b"16-byte aligned")
     refused(setter(beta=None), b"null gamma / beta")
-    d, m = _host_desc()
-    assert lib.sige_tile_conv_modulated(None, ctypes.byref(m), None) != 0 and b"null" in lib.sige_last_error()
-    assert lib.sige_tile_conv_modulated(ctypes.byref(d), None, None) != 0 and b"null" in lib.sige_last_error()
+    refused(setter(src_pixel_stride=128), b"a source window cannot be modulated")
+    assert lib.sige_tile_conv(None, None) != 0 and b"null" in lib.sige_last_error()
     d, m = _host_desc(N=0)
     m.beta = None
-    assert lib.sige_tile_conv_modulated(ctypes.byref(d), ctypes.byref(m), None) == 0       # N == 0: no-op
+    assert lib.sige_tile_conv(ctypes.byref(d), None) == 0       # N == 0: no-op
 
 
-def test_modulated_predicate_and_prototypes(cabi_lib):
+def test_tile_conv_supported_and_the_refusal_of_what_it_rejects(cabi_lib):
+    """ops.tile_conv_supported takes every modulated conv of the table, and sige_tile_conv refuses, before any CUDA call, each
+    modulated descriptor the predicate rejects."""
     import test_cabi_symbols as TS
-    from sige_b200 import _cabi
+    from sige_b200 import _cabi, ops
 
     lib = _cabi.lib()
-    assert lib.sige_abi_version() == 2 and set(_cabi.PROTOTYPES) == TS._declared()
-    assert {"sige_tile_conv_modulated", "sige_tile_conv_modulated_supported"} <= TS._declared()
-    ok = lib.sige_tile_conv_modulated_supported
+    assert lib.sige_abi_version() == 3 and set(_cabi.PROTOTYPES) == TS._declared()
+    ok = ops.tile_conv_supported
     for cin in (8, 16, 40, 64, 96, 136, 256, 512, 768):
         for k, s in ((3, 1), (1, 1), (3, 2)):
-            assert ok(cin, 64, k, s, _cabi.F16) == 1 and ok(cin, 48, k, s, _cabi.BF16) == 1
-    assert ok(36, 64, 3, 1, _cabi.F16) == 0 and ok(64, 60, 3, 1, _cabi.F16) == 0 and ok(64, 64, 3, 1, _cabi.F32) == 0
+            assert ok(cin, 64, k, s, torch.float16) and ok(cin, 48, k, s, torch.bfloat16)
+    for cin, cout, dtype, code, why in ((36, 64, torch.float16, _cabi.F16, b"source 0 has 36 channels"),
+                                        (64, 60, torch.float16, _cabi.F16, b"Cout (60) must be a multiple of 8"),
+                                        (64, 64, torch.float32, _cabi.F32, b"needs f16/bf16")):
+        assert not ok(cin, cout, 3, 1, dtype)
+        d, m = _host_desc(cin=cin, cout=cout)
+        d.dtype, m.gamma_C, m.beta_C = code, 64, 64
+        assert lib.sige_tile_conv(ctypes.byref(d), None) != 0 and why in lib.sige_last_error(), lib.sige_last_error()
 
 
 # ---------------------------------------------------------------------------------------------------------------- contract (CPU)
@@ -214,14 +222,14 @@ def test_modulated_reference_matches_oracle(oracle, spec, mod):
 # ---------------------------------------------------------------------------------------------------------------- lowering (CPU)
 def _mod_sim():
     """(ModulatedSim, NarrowSim): the descriptor simulator of test_narrow_tile_conv.py with and without a CPU restatement of
-    sige_tile_conv_modulated."""
+    the modulated sige_tile_conv launch."""
     import test_narrow_tile_conv as TN
 
     NarrowSim, _ = TN._narrow_sim()
 
     class ModulatedSim(NarrowSim):
         def modulated_conv_supported(self, cin, cout, k, stride):
-            """sige_tile_conv_modulated_supported(): Cin and Cout multiples of 8."""
+            """ops.tile_conv_supported(): Cin and Cout multiples of 8."""
             return cin % 8 == 0 and cout % 8 == 0
 
         def prepare_conv(self, fc):
@@ -411,16 +419,13 @@ def _mod_case(spec, mod, dtype, dev) -> ModCase:
 
 
 def _launch(mc: ModCase, ksplit, flags, mod=True):
-    """The modulated launch of `mc`, or (mod=False) the plain sige_tile_conv launch of the same descriptor."""
+    """The modulated launch of `mc`, or (mod=False) the plain launch of the same descriptor."""
     from sige_b200 import _cabi
 
     d = TC.descriptor(mc.case, ksplit=ksplit, flags=flags)
-    stream = torch.cuda.current_stream().cuda_stream
     if mod:
-        m = modulation(mc)
-        _cabi.check(_cabi.lib().sige_tile_conv_modulated(ctypes.byref(d), ctypes.byref(m), stream), "sige_tile_conv_modulated")
-    else:
-        _cabi.check(_cabi.lib().sige_tile_conv(ctypes.byref(d), stream), "sige_tile_conv")
+        d.modulation = ctypes.pointer(modulation(mc))
+    _cabi.check(_cabi.lib().sige_tile_conv(ctypes.byref(d), torch.cuda.current_stream().cuda_stream), "sige_tile_conv")
     torch.cuda.synchronize()
 
 
@@ -431,7 +436,7 @@ def _ksplits(spec):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
-def test_modulated_tile_conv_against_the_float64_contract(dtype):
+def test_modulation_field_against_the_float64_contract(dtype):
     """Every modulated case, at every split the plan allows, with and without PDL: within the contract's bound and every element
     it does not write bitwise unchanged."""
     dev = torch.device("cuda:0")
@@ -456,7 +461,7 @@ def test_modulated_tile_conv_against_the_float64_contract(dtype):
 @pytest.mark.gpu
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("cin,k", [(40, 3), (64, 3), (512, 3), (96, 1), (256, 1)])
-def test_zero_modulation_equals_the_plain_launch(dtype, cin, k):
+def test_zero_modulation_field_equals_the_plain_launch(dtype, cin, k):
     """gamma = beta = 0 and slope 1: bitwise the existing mma.sync launch with the same scale / shift pre-op."""
     dev = torch.device("cuda:0")
     spec = TC.Spec("zero%d_k%d" % (cin, k), B=1, H=30, W=38, srcs=((cin, 0),), Cout=64, k=k, counts=(40,), preop="shared", seed=cin + k)

@@ -1,13 +1,13 @@
 """The SPADE GauGAN generator's sparse SPADE layers as modulated tile convs on channel windows.
 
 The full SPADE (reference gaugan/models/sige_normalization.py:51,75-86) has ONE gamma/beta conv whose input is a torch.split window of
-the block's shared activation and whose output is split into gamma and beta.  sige_tile_conv_strided reads such a window in place;
-the lowering runs `mlp_gamma_beta` on it and hands the conv that reads the SPADE gamma / beta as windows of one buffer
-(sige_tile_conv_modulated), so nothing is materialised and the compiled step takes the next label edit in place.
+the block's shared activation and whose output is split into gamma and beta.  sige_tile_conv reads such a window in place
+(src_pixel_stride); the lowering runs `mlp_gamma_beta` on it and hands the conv that reads the SPADE gamma / beta as windows of one
+buffer (modulation), so nothing is materialised and the compiled step takes the next label edit in place.
 
 CPU: the in-tree generator against the reference's golden; launch counts before / after on the descriptor simulator (the in-tree file
-and, when installed, the reference's); the DDPM and sub-mobile steps unchanged by the new rule; rebind on the simulator; the new entry
-point's refusals and predicate.
+and, when installed, the reference's); the DDPM and sub-mobile steps unchanged by the new rule; rebind on the simulator; the window's
+refusals, predicate and plan.
 GPU: the strided launch bitwise equal to the plain launch on a compacted copy (wgmma and mma.sync geometries, every split, PDL,
 padded lists, NaN outside the window); the modulated launch with gamma / beta windows bitwise equal to compacted copies; the fused
 fp16 miniature against the golden; the next edit by rebind and set_masks_async."""
@@ -38,7 +38,7 @@ def _sims():
 
     class StridedSim(ModulatedSim):
         def strided_conv_supported(self, cin, cout, k, stride):
-            """sige_tile_conv_strided: a window of cin % 8 == 0 channels, Cout % 8 == 0."""
+            """ops.tile_conv_supported(): a window of cin % 8 == 0 channels, Cout % 8 == 0."""
             return cin % 8 == 0 and cout % 8 == 0
 
     return StridedSim, ModulatedSim
@@ -246,7 +246,7 @@ def _host_desc(cin=128, cout=256, k=3, N=16):
     return d
 
 
-def test_strided_refusals_come_before_any_cuda_call(cabi_lib):
+def test_window_field_refusals_come_before_any_cuda_call(cabi_lib):
     """Each refusal returns non-zero with its own message (a descriptor that passed the checks would fail at the device instead,
     with a different message: there is no device here)."""
     from sige_b200 import _cabi
@@ -255,8 +255,9 @@ def test_strided_refusals_come_before_any_cuda_call(cabi_lib):
 
     def refused(change, what, pitch=384):
         d = _host_desc()
+        d.src_pixel_stride = pitch
         change(d)
-        assert lib.sige_tile_conv_strided(ctypes.byref(d), pitch, None) != 0
+        assert lib.sige_tile_conv(ctypes.byref(d), None) != 0
         assert what in lib.sige_last_error(), (what, lib.sige_last_error())
 
     def two_sources(d):
@@ -271,30 +272,49 @@ def test_strided_refusals_come_before_any_cuda_call(cabi_lib):
     refused(lambda d: setattr(d, "idx_per_image", 1), b"per-image")
     refused(lambda d: None, b"pixel stride", pitch=120)
     refused(lambda d: None, b"pixel stride", pitch=132)
-    refused(lambda d: None, b"pixel stride", pitch=0)
+    refused(lambda d: None, b"pixel stride", pitch=-8)
     refused(lambda d: setattr(d.src[0], "ptr", 0x10008), b"16-byte aligned")
-    assert lib.sige_tile_conv_strided(None, 256, None) != 0 and b"null" in lib.sige_last_error()
     d = _host_desc(N=0)
-    assert lib.sige_tile_conv_strided(ctypes.byref(d), 256, None) == 0          # N == 0: no-op
+    d.src_pixel_stride = 256
+    assert lib.sige_tile_conv(ctypes.byref(d), None) == 0          # N == 0: no-op
     d = _host_desc()
+    d.src_pixel_stride = 256
     d.src[0].C = 12
-    assert lib.sige_tile_conv_strided(ctypes.byref(d), 256, None) != 0           # and otherwise sige_tile_conv's contract
+    assert lib.sige_tile_conv(ctypes.byref(d), None) != 0           # and otherwise the contract of every launch
     assert b"multiple of 8" in lib.sige_last_error()
 
 
-def test_strided_predicate_and_channel_windows(cabi_lib):
+def test_window_is_planned_with_its_pixel_stride(cabi_lib):
+    """The wgmma kernel keeps 32-bit element offsets into its source, so a window of a buffer of 2^31 elements or more runs on
+    mma.sync however narrow the window is; the plan sees the pixel stride the launch uses and reports that kernel."""
+    import mma_tile_conv_contract as MC
+    from sige_b200 import _cabi
+
+    def plan(pitch):
+        d = _host_desc()
+        d.H = d.W = d.dH = d.dW = 2048                       # 2^22 pixels
+        d.src_pixel_stride = pitch
+        p = _cabi.TileConvPlan()
+        assert _cabi.lib().sige_tile_conv_plan(ctypes.byref(d), ctypes.byref(p)) == 0
+        return p
+
+    assert plan(0).path == 1 and plan(384).path == 1         # 2^29 and 1.5 * 2^30 elements
+    assert MC.plan_tuple(plan(512)) == MC.expected_plan_tuple(MC.plan(16, 6, 6, 3, 3, 1, 128, 256, 0))
+
+
+def test_window_predicate_and_channel_windows(cabi_lib):
     import test_cabi_symbols as TS
     from sige_b200 import _cabi, ops
     from sige_b200.fused import CudaExecutor
 
-    assert _cabi.lib().sige_abi_version() == 2
-    assert set(_cabi.PROTOTYPES) == TS._declared() and "sige_tile_conv_strided" in _cabi.PROTOTYPES
+    assert _cabi.lib().sige_abi_version() == 3
+    assert set(_cabi.PROTOTYPES) == TS._declared()
     ex = CudaExecutor(torch.device("cpu"), torch.float16)
     for cin in (8, 40, 64, 128, 192):
         for k, s in ((3, 1), (1, 1), (3, 2)):
-            assert ex.strided_conv_supported(cin, 256, k, s) and ops.tile_conv_strided_supported(cin, 48, k, s, torch.bfloat16)
+            assert ex.strided_conv_supported(cin, 256, k, s) and ops.tile_conv_supported(cin, 48, k, s, torch.bfloat16)
     assert not ex.strided_conv_supported(36, 256, 3, 1) and not ex.strided_conv_supported(128, 60, 3, 1)
-    assert not ops.tile_conv_strided_supported(128, 256, 3, 1, torch.float32)
+    assert not ops.tile_conv_supported(128, 256, 3, 1, torch.float32)
     buf = torch.empty(2, 384, 5, 7, dtype=torch.float16).contiguous(memory_format=torch.channels_last)
     for c0, c1 in ((0, 384), (0, 128), (128, 256), (256, 384)):
         base, pitch, first = ops.channel_window(buf[:, c0:c1])
@@ -342,7 +362,7 @@ def _ksplits(spec):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
-def test_strided_launch_equals_the_plain_launch_on_a_compacted_copy(dtype):
+def test_window_field_launch_equals_the_plain_launch_on_a_compacted_copy(dtype):
     """Every window case on the wgmma kernel (cp.async copy gather and register-staged gather) and on the mma.sync kernel (narrow
     sources included), at every split, with and without PDL and padded lists: bitwise the plain launch on the compacted window.
     The channels outside the window are NaN, so a read of any of them would show; every element the launch does not write keeps
@@ -366,10 +386,8 @@ def test_strided_launch_equals_the_plain_launch_on_a_compacted_copy(dtype):
                         buf.copy_(init[name])
                     d = TC.descriptor(case, ksplit=ks, flags=flags)
                     if strided:
-                        d.src[0].ptr = wide[..., c0:].data_ptr()
-                        _cabi.check(lib.sige_tile_conv_strided(ctypes.byref(d), pitch, stream), "sige_tile_conv_strided")
-                    else:
-                        _cabi.check(lib.sige_tile_conv(ctypes.byref(d), stream), "sige_tile_conv")
+                        d.src[0].ptr, d.src_pixel_stride = wide[..., c0:].data_ptr(), pitch
+                    _cabi.check(lib.sige_tile_conv(ctypes.byref(d), stream), "sige_tile_conv")
                     torch.cuda.synchronize()
                     outs.append({k: v.clone() for k, v in case.buffers().items()})
                 for name in init:
@@ -385,7 +403,7 @@ def test_strided_launch_equals_the_plain_launch_on_a_compacted_copy(dtype):
 @pytest.mark.gpu
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("cin,k,slope", [(128, 3, 0.2), (64, 3, 0.2), (256, 1, 1.0), (40, 3, 0.2)])
-def test_modulated_launch_with_gamma_beta_windows_equals_compacted_copies(dtype, cin, k, slope):
+def test_modulation_field_with_gamma_beta_windows_equals_compacted_copies(dtype, cin, k, slope):
     """gamma and beta as the two channel halves of ONE buffer (torch.split(gamma_beta, C)), passed as views: bitwise the same launch
     with gamma and beta copied into buffers of their own."""
     import test_modulated_tile_conv as TM
@@ -406,8 +424,8 @@ def test_modulated_launch_with_gamma_beta_windows_equals_compacted_copies(dtype,
         for g, b in ((gamma_c, beta_c), (gamma_w, beta_w)):
             case.dst.copy_(init)
             d = TC.descriptor(case, ksplit=ks, flags=TC.PDL | TC.PADDED)
-            m = ops.conv_modulation(g, b, slope)
-            _cabi.check(_cabi.lib().sige_tile_conv_modulated(ctypes.byref(d), ctypes.byref(m), stream), "sige_tile_conv_modulated")
+            d.modulation = ctypes.pointer(ops.conv_modulation(g, b, slope))
+            _cabi.check(_cabi.lib().sige_tile_conv(ctypes.byref(d), stream), "sige_tile_conv")
             torch.cuda.synchronize()
             outs.append(case.dst.clone())
         assert torch.equal(outs[-2].view(torch.int16), outs[-1].view(torch.int16)), ks

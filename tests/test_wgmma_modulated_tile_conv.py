@@ -1,10 +1,10 @@
-"""Modulated tile convs on the wgmma kernel: with SIGE_CONV_TC5, sige_tile_conv_modulated runs the stride-1 wgmma geometries (3x3 on
+"""Modulated tile convs on the wgmma kernel: with SIGE_CONV_TC5, a modulated sige_tile_conv runs the stride-1 wgmma geometries (3x3 on
 6x6 tiles, 1x1 on 4x4 tiles, Cin and Cout multiples of 64) on the MOD instantiations of tile_conv_tc5_kernel, whose register-staged
 gather applies SPADE's modulation leaky((x*scale + shift) * (1 + gamma) + beta).  Everything else stays on the mma.sync kernel.
 
-CPU (host-only planning: the plan of an H100 80GB HBM3, as in test_tile_conv_contract.py): sige_tile_conv_modulated_plan gives the
-intended instantiation for every case and split of the table below, the table reaches all 12 MOD instantiations, and the launches
-that stay on mma.sync plan it.
+CPU (host-only planning: the plan of an H100 80GB HBM3, as in test_tile_conv_contract.py): sige_tile_conv_plan of a modulated
+descriptor gives the intended instantiation for every case and split of the table below, the table reaches all 12 MOD
+instantiations, and the launches that stay on mma.sync plan it.
 GPU: every case against the float64 contract (tests/test_modulated_tile_conv.py's mod_reference), with the plan on the device checked;
 gamma = beta = 0 with slope 1 equals the plain wgmma launch bitwise; the SPADE generator miniature runs its wide modulated launches on
 wgmma."""
@@ -53,11 +53,12 @@ MOD_INSTANTIATIONS = sorted(
 
 
 def modulated_plan(d):
+    """sige_tile_conv_plan of a copy of `d` whose modulation is set (the plan never reads it)."""
     from sige_b200 import _cabi
 
-    p = _cabi.TileConvPlan()
-    _cabi.check(_cabi.lib().sige_tile_conv_modulated_plan(ctypes.byref(d), ctypes.byref(p)), "sige_tile_conv_modulated_plan")
-    return p
+    m = type(d).from_buffer_copy(d)
+    m.modulation = ctypes.pointer(_cabi.ConvModulation())
+    return TC.plan_of(m)
 
 
 def instantiation(spec, dtype, plan):
@@ -101,20 +102,20 @@ def table_plans(cabi_lib):
     return _table_plans()
 
 
-def test_modulated_case_plans_are_the_intended_ones(table_plans):
+def test_modulated_descriptor_plans_are_the_intended_ones(table_plans):
     for spec, _, dtype, i, ks, plan, key in table_plans:
         assert key == intended(spec, dtype, i), "%s %s ksplit %d: plan %s -> %s, intended %s" % (
             spec.name, TC.DTYPE_NAME[dtype], ks, TC.plan_str(plan), key, intended(spec, dtype, i))
         assert plan.ksplit == spec.expect[i][1]
 
 
-def test_modulated_case_table_reaches_every_mod_instantiation(table_plans):
+def test_modulated_descriptor_plans_reach_every_mod_instantiation(table_plans):
     keys = {key for *_, key in table_plans if key is not None}
     assert len(MOD_INSTANTIATIONS) == 12
     assert sorted(keys) == MOD_INSTANTIATIONS, "missing: %s" % sorted(set(MOD_INSTANTIATIONS) - keys)
 
 
-def test_modulated_case_table_covers_every_feature_wide_and_narrow(table_plans):
+def test_modulated_descriptor_plans_cover_every_feature_wide_and_narrow(table_plans):
     seen = set()
     for spec, mod, _, _, _, plan, _ in table_plans:
         seen |= {(f, "wide" if plan.bn == 128 else "narrow") for f in mod_features(spec, mod)}
@@ -134,10 +135,10 @@ def test_modulated_case_table_sizes_do_not_depend_on_the_h100_variant():
                 assert m_blocks * spec.Cout // 64 <= 100, spec.name
 
 
-def test_launches_that_stay_on_mma_sync_report_its_plan(cabi_lib):
-    """No flag, a narrow Cin, a Cout that is not a multiple of 64, stride 2: sige_tile_conv_modulated_plan says mma.sync (path 0) with
+def test_modulated_descriptors_that_stay_on_mma_sync_plan_it(cabi_lib):
+    """No flag, a narrow Cin, a Cout that is not a multiple of 64, stride 2: the plan of a modulated descriptor says mma.sync (path 0) with
     that kernel's configuration and grid (restated in tests/mma_tile_conv_contract.py); the wgmma geometries with the flag plan wgmma
-    exactly as sige_tile_conv_plan does."""
+    exactly as the unmodulated descriptor does."""
     def plans(spec, flags):
         d = TC.descriptor(TC.make_case(spec, torch.float16, "cpu"), 0, flags)
         return modulated_plan(d), TC.plan_of(d)
@@ -159,13 +160,13 @@ def test_launches_that_stay_on_mma_sync_report_its_plan(cabi_lib):
     assert plain.path == 1 and mod.path == 0
 
 
-def test_modulated_plan_prototype(cabi_lib):
+def test_one_plan_query_for_modulated_descriptors(cabi_lib):
     import test_cabi_symbols as TS
     from sige_b200 import _cabi
 
-    assert "sige_tile_conv_modulated_plan" in TS._declared() and set(_cabi.PROTOTYPES) == TS._declared()
-    assert _cabi.lib().sige_abi_version() == 2
-    assert _cabi.lib().sige_tile_conv_modulated_plan(None, None) != 0 and b"null" in _cabi.lib().sige_last_error()
+    assert set(_cabi.PROTOTYPES) == TS._declared()
+    assert _cabi.lib().sige_abi_version() == 3
+    assert _cabi.lib().sige_tile_conv_plan(None, None) != 0 and b"null" in _cabi.lib().sige_last_error()
 
 
 # ---------------------------------------------------------------------------------------------------------------- kernel (GPU)
@@ -175,7 +176,7 @@ def _device_plan_key(mc, ks, flags):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
-def test_wgmma_modulated_tile_conv_against_the_float64_contract(dtype):
+def test_wgmma_modulation_field_against_the_float64_contract(dtype):
     """Every case, at every split of the table, with and without PDL (and PADDED where the list is padded): the plan on this device is
     the intended MOD instantiation, every written element is within the contract's bound and every other element is unchanged."""
     dev = torch.device("cuda:0")
@@ -202,7 +203,7 @@ def test_wgmma_modulated_tile_conv_against_the_float64_contract(dtype):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
-def test_zero_modulation_equals_the_plain_wgmma_launch(dtype):
+def test_zero_modulation_field_equals_the_plain_wgmma_launch(dtype):
     """gamma = beta = 0 and slope 1: bitwise the plain wgmma launch with the same scale / shift pre-op (both run the register-staged
     gather of the same plan): 3x3 and 1x1, BN 64 and 128, split and un-split, up-sampled sources."""
     dev = torch.device("cuda:0")
