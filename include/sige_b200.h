@@ -276,6 +276,21 @@ typedef struct {
  * CTAs' worth — CTAs made only of padding exit at once.  (Without the flag padding entries are still harmless: they read zeros
  * and write nothing; the flag only buys the early exit, at the price of one index load on every CTA's prologue.) */
 #define SIGE_CONV_PADDED 4
+/* With SIGE_CONV_PDL on the wgmma kernel: release the next launch right after this launch's own dependency has resolved, instead
+ * of at the epilogue, so that the next launch's CTAs take the SMs this one leaves idle and gather their early chunks (below)
+ * during this launch's mainloop.  Meant for the predecessor of a launch with early source groups. */
+#define SIGE_CONV_EARLY_RELEASE 8
+/* Early source groups (wgmma kernel, with SIGE_CONV_PDL): source groups the launch may read before its dependency on the preceding
+ * launch of the stream resolves — src[0], src[1], all of src2 (the fused shortcut).  Their K chunks are gathered and multiplied
+ * while the preceding launch is still running; each rank of a split takes an even share of them, then an even share of the rest.
+ * Set one only for a group that the preceding launch does not write (nor the pre-op's scale / shift, nor the modulation's gamma /
+ * beta, for the src groups), and only when the preceding launch is a sige_tile_conv on the wgmma kernel: such a launch waits for
+ * ITS predecessor before it releases its dependents, so every launch before it has completed.  None set = wait before the first
+ * gather.  The sum is the same up to the order of the K chunks; the mma.sync kernel and the stride-2 geometry ignore them (they
+ * wait first). */
+#define SIGE_CONV_EARLY_SRC0 16
+#define SIGE_CONV_EARLY_SRC1 32
+#define SIGE_CONV_EARLY_SHORTCUT 64
 /* Origin of a padding entry of a per-image tile list (both coordinates). */
 #define SIGE_TILE_NONE (-30000)
 
@@ -450,10 +465,10 @@ int sige_tile_writeback(const sige_writeback_entry_t *entries, int n_entries, si
 /* diagnostics                                                                */
 /* ------------------------------------------------------------------------- */
 /* In-kernel timeline: while `buf` (device int64, 16 slots per CTA of the NEXT sige_tile_conv launch that takes the wgmma
- * path) is set, that launch stamps %globaltimer per CTA — slot 0 entry, 3 dependency released + loads issued, 4 halo stored,
+ * path) is set, that launch stamps %globaltimer per CTA — slot 0 entry, 3 dependency resolved (griddepcontrol.wait returned), 4 halo stored,
  * 5/6 MMA issue begin/end, 7 accumulators out of registers, 8/9 every partial row present (split-K: exchange landed),
  * 10 stores of thread 0 issued, 11 exit (every thread's stores issued); slot 12 holds the number of halo fills of the
- * CTA's K slice (a count, not a time).  The pointer is baked into the launch's
+ * CTA's K slice (a count, not a time); slot 13 the early chunks of the slice gathered (SIGE_CONV_EARLY_*; 0 without any).  The pointer is baked into the launch's
  * kernel parameters (so it survives CUDA-graph capture); call again (NULL to stop) before the next launch.  bench.py derives
  * the in-step roofline from these stamps; returns 0. */
 int sige_debug_set_trace(void *buf);

@@ -23,6 +23,8 @@ ACT_IDENTITY, ACT_SWISH, ACT_RELU = 0, 1, 2
 CONV_PDL = 1
 CONV_TC5 = 2
 CONV_PADDED = 4
+CONV_EARLY_RELEASE = 8
+CONV_EARLY_SRC0, CONV_EARLY_SRC1, CONV_EARLY_SHORTCUT = 16, 32, 64      # early source groups: (mask & 7) << 4
 TILE_NONE = -30000
 
 

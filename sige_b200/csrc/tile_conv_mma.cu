@@ -126,7 +126,11 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
     const int tile0 = blockIdx.x * p.tpc;          // first tile of this CTA
     const int n0 = blockIdx.y * BN;                // first output channel of this CTA
     // fixed-capacity tile lists: a CTA whose first tile is SIGE_TILE_NONE padding has nothing to do (see tile_conv_tc5.cu)
-    if (p.padded && __ldg(p.idx + 2 * tile0) <= SIGE_TILE_NONE) return;
+    // (it still waits for the previous launch first: no launch may complete before its predecessor, see tile_conv_tc5.cu)
+    if (p.padded && __ldg(p.idx + 2 * tile0) <= SIGE_TILE_NONE) {
+        if (p.pdl) pdl_acquire();
+        return;
+    }
     const int ntile = min(p.tpc, p.NT - tile0);    // tiles actually present
     const int NC = (p.Cin + KC - 1) / KC;          // K chunks (the last one partial on a narrow source)
     const int J = NC * p.taps;                     // (chunk, tap) steps of the whole K loop

@@ -98,6 +98,8 @@ struct Params {
     int idx_per_image;         // 1: idx / sc_flags hold B*N entries (row b*N + i = tile i of image b), else N shared by all images
     int ksplit;
     int pdl;                   // launched with programmatic dependent launch: the next layer is released at the epilogue
+    int early_release;         // SIGE_CONV_EARLY_RELEASE: released right after this launch's own dependency has resolved instead
+    int early;                 // SIGE_CONV_EARLY_* >> 4: source groups whose chunks are gathered before the dependency resolves (KOrder)
     int is_bf16;
     // SPADE modulation in the gather stage (MOD instantiations only, sige_tile_conv_t.modulation): gamma / beta are NHWC at the logical
     // source extent with gC / bC elements per pixel, each pointing at the first channel of its window (sige_conv_modulation_t's c0);
@@ -342,9 +344,59 @@ __device__ __forceinline__ long long gtime() {
         if (p.trace) p.trace[((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 16 + (slot)] = gtime(); \
     } while (0)
 
-// K slice of rank kr of a split-K launch: ring steps [k_slice(J, kr, ks), k_slice(J, kr + 1, ks)), an even split (the host
-// picks the halo layout from the same partition, see split_halo_fills)
+// even split of n ring steps over ks ranks: rank kr takes [k_slice(n, kr, ks), k_slice(n, kr + 1, ks))
 __host__ __device__ __forceinline__ int k_slice(int J, int kr, int ks) { return (int)(((long long)J * kr) / ks); }
+
+// K order and partition of a launch.  The ring steps fall into three source groups, each a run of whole 64-channel chunks in the
+// natural order: main chunks of src[0], main chunks of src[1], fused-shortcut chunks (src2).  The groups whose bit is set in
+// `early` (the SIGE_CONV_EARLY_* flags) come first, then the others, each group keeping its order; rank kr of a split takes an even
+// share of the early steps followed by an even share of the late ones, so the work left after the dependency resolves is
+// balanced.  early == 0 is the natural order and the even split of k_slice.  The kernel, the halo-layout choice
+// (split_halo_fills) and decide() all use this one partition.
+struct KOrder {
+    int NC, spc, J_main, J;
+    int b0, early, E;                                      // b0: ring steps of src[0] (the groups are [0, b0), [b0, J_main), [J_main, J))
+    __host__ __device__ KOrder(int Cin, int C0, int Cin2, int spc_, int early_) {
+        NC = Cin / KC;
+        spc = spc_;
+        J_main = NC * spc;
+        J = J_main + Cin2 / KC;
+        b0 = C0 < Cin ? C0 / KC * spc : J_main;
+        early = early_ & 7;
+        E = ((early & 1) ? b0 : 0) + ((early & 2) ? J_main - b0 : 0) + ((early & 4) ? J - J_main : 0);
+    }
+    // ring position q -> step j of the natural order
+    __host__ __device__ int step(int q) const {
+        const int want = q < E ? 1 : 0;                    // early groups first, then the others
+        if (!want) q -= E;
+        if (((early >> 0) & 1) == want) { if (q < b0) return q; q -= b0; }
+        if (((early >> 1) & 1) == want) { if (q < J_main - b0) return b0 + q; q -= J_main - b0; }
+        return J_main + q;
+    }
+    __host__ __device__ int chunk(int j) const { return j < J_main ? j / spc : NC + (j - J_main); }
+};
+// The K slice of rank kr: `ne` early ring positions from eb, then the late ones from lb; n in all.  Slice step i sits at ring
+// position pos(i).  A chunk's steps are never split between the early and the late part.
+struct KSlice {
+    int eb, ne, lb, n;
+    __host__ __device__ KSlice(const KOrder &o, int kr, int ks) {
+        eb = k_slice(o.E, kr, ks);
+        ne = k_slice(o.E, kr + 1, ks) - eb;
+        lb = o.E + k_slice(o.J - o.E, kr, ks);
+        n = ne + (o.E + k_slice(o.J - o.E, kr + 1, ks) - lb);
+    }
+    __host__ __device__ int pos(int i) const { return i < ne ? eb + i : lb + (i - ne); }
+    // halo fills (distinct chunks) of the slice
+    __host__ __device__ int fills(const KOrder &o) const {
+        int f = 0, prev = -1;
+        for (int i = 0; i < n; ++i) {
+            const int c = o.chunk(o.step(pos(i)));
+            if (c != prev) ++f;
+            prev = c;
+        }
+        return f;
+    }
+};
 
 // ASYNC: the gather is a pure copy (no pre-op: the producer of the source already applied it) and is done with cp.async.
 // DB: the double-buffered split-K layout (Cfg).
@@ -380,19 +432,31 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
     const int tile0 = blockIdx.x * TILES;
     // fixed-capacity tile lists (one image): real tiles are packed at the front, the rest are SIGE_TILE_NONE.  A CTA (and with it
     // its whole split-K cluster: same tile0) whose first tile is padding has nothing to read or write.
-    if (p.padded && __ldg(p.idx + 2 * tile0) <= SIGE_TILE_NONE) return;
+    // Early chunks (p.early) read buffers that the preceding launch does not write, before griddepcontrol.wait.  That is sound
+    // because every CTA of every launch waits before it releases its dependents and before it exits (here, in the producers and
+    // at the epilogue): when this launch starts, every CTA of the preceding launch has passed its wait, so the launch before that
+    // has completed and its writes are visible — and no launch completes before its own predecessor, so all earlier ones have too.
+    if (p.padded && __ldg(p.idx + 2 * tile0) <= SIGE_TILE_NONE) {
+        if (p.pdl) pdl_acquire();
+        return;
+    }
     const int n0 = blockIdx.y * BN;
     const int ntile = min(TILES, p.NT - tile0);
     const int NC = p.Cin / KC;
     const int J_main = NC * SPC;                   // ring steps of the main conv (a step = TPS taps of one 64-channel chunk)
-    const int NC2 = (TAPS == 9 && !S2) ? p.Cin2 / KC : 0;  // fused 1x1 shortcut: one step (the centre tap) per chunk of ITS input
-    const int J = J_main + NC2;
     const int kr = blockIdx.z;
-    const int j_begin = k_slice(J, kr, p.ksplit), j_end = k_slice(J, kr + 1, p.ksplit);
-    // halo-buffer chunks in processing order: main chunks 0..NC-1, then shortcut chunks NC..NC+NC2-1
+    // halo-buffer chunks: main chunks 0..NC-1, then fused 1x1 shortcut chunks NC..NC+NC2-1 (one step, the centre tap, per chunk
+    // of ITS input); this rank's steps in processing order: ko.step(ks.pos(i)), i < ks.n
+    const KOrder ko(p.Cin, p.C0, (TAPS == 9 && !S2) ? p.Cin2 : 0, SPC, S2 ? 0 : p.early);
+    const KSlice ks(ko, kr, p.ksplit);
     auto chunk_of = [&](int j) { return j < J_main ? j / SPC : NC + (j - J_main); };
-    const int c_first = chunk_of(j_begin), c_last = chunk_of(j_end - 1);
-    if (tid == 0 && p.trace) p.trace[((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 16 + 12] = c_last - c_first + 1;   // halo fills
+    auto step_at = [&](int i) { return ko.step(ks.pos(i)); };
+    // slice step i (step j) starts a chunk: the step after the last one of that chunk in this slice (or ks.n)
+    auto chunk_end = [&](int i, int j) {
+        const int rest = j < J_main ? SPC - (j - (j / SPC) * SPC) : 1;
+        return min(i + rest, i < ks.ne ? ks.ne : ks.n);
+    };
+    if (tid == 0 && p.trace) p.trace[((blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * 16 + 12] = ks.fills(ko);   // halo fills
     int32_t *s_idx = reinterpret_cast<int32_t *>(smem + C::OFF_CONST);          // [TILES][2] tile origins of this CTA
     unsigned char *s_flags = smem + C::OFF_FLAGS;                               // [TILES] 1 = evaluate the fused shortcut on this tile
     float *s_const = reinterpret_cast<float *>(smem + C::OFF_VEC);              // bias | aux0 scale | aux0 shift | aux1 scale | aux1 shift | bias2
@@ -472,12 +536,13 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
         // ================= TMA producer: weights =================
         if (lane == 0) {
             int s = 0, k = 0;                                          // ring stage and lap
-            int c = j_begin < J_main ? j_begin / SPC : 0, st = j_begin < J_main ? j_begin - c * SPC : 0;
-            for (int j = j_begin; j < j_end; ++j) {
-                if (DB && j == j_begin + NSTB) {
+            for (int i = 0; i < ks.n; ++i) {
+                const int j = step_at(i);
+                if (DB && i == NSTB) {
                     // the ring is full: pull the rest of the slice into L2 now (this overlaps the previous layer under PDL),
                     // so that a two-stage ring refills from L2 rather than HBM
-                    for (int jj = j; jj < j_end; ++jj) {
+                    for (int ii = i; ii < ks.n; ++ii) {
+                        const int jj = step_at(ii);
                         if (jj < J_main) {
                             const int cj = jj / SPC, row0 = ((jj - cj * SPC) * TPS * NC + cj) * p.Cout + n0;
 #pragma unroll
@@ -491,10 +556,10 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
                 const uint32_t dst = sbase + C::OFF_B + s * C::B_STAGE_BYTES;
                 if (j < J_main) {
                     mbar_expect_tx(B_FULL(s), C::B_STAGE_BYTES);
+                    const int c = j / SPC, st = j - c * SPC;
                     const int row0 = (st * TPS * NC + c) * p.Cout + n0;      // weight rows of tap st*TPS, chunk c
 #pragma unroll
                     for (int t = 0; t < TPS; ++t) tma_load_2d(dst + t * C::B_TILE_BYTES, &wmap, 0, row0 + t * NC * p.Cout, B_FULL(s));
-                    if (++st == SPC) { st = 0; ++c; }
                 } else {                                               // shortcut weights [Cin2/64][Cout][64]
                     mbar_expect_tx(B_FULL(s), C::B_TILE_BYTES);
                     tma_load_2d(dst, &wmap2, 0, (j - J_main) * p.Cout + n0, B_FULL(s));
@@ -514,15 +579,16 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
         const uint32_t a_lo0 = desc_lo(sbase + C::OFF_A + wg * (64 * 128)), b_lo0 = desc_lo(sbase + C::OFF_B);
         uint32_t accum = 0;
         int ab = 0, ause = 0;             // halo buffer index and how many times it has been used
-        int st = (j_begin < J_main) ? j_begin % SPC : 0, s = 0, k = 0;
+        int s = 0, k = 0;
         int pend = -1;                    // weight stage of the previous step, not yet released
-        for (int j = j_begin; j < j_end; ++j) {
+        for (int i = 0; i < ks.n; ++i) {
+            const int j = step_at(i);
             const bool is_sc = j >= J_main;
-            if (is_sc) st = 0;
-            if (j == j_begin || st == 0) {                        // a new chunk starts: wait for its halo buffer
+            const int st = is_sc ? 0 : j - (j / SPC) * SPC;
+            if (i == 0 || i == ks.ne || st == 0) {                // a new chunk starts: wait for its halo buffer
                 mbar_wait(A_FULL(ab), (ause / NAB) & 1);
                 fence_proxy_async();          // gathered data (generic proxy writes) -> visible to the tensor core's async proxy
-                if (j == j_begin && tid == 0) SIGE_TRACE(5);
+                if (i == 0 && tid == 0) SIGE_TRACE(5);
             }
             mbar_wait(B_FULL(s), k & 1);
             const uint32_t b_step = b_lo0 + s * (C::B_STAGE_BYTES >> 4);
@@ -534,7 +600,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
                 else if (TPS == 3) a_step += st * ((32 * 128) >> 4);                           // ky = st, kx = t
                 else { const int ky = st / 3; a_step += ky * ((32 * 128) >> 4) + (st - 3 * ky) * (A_COPY_BYTES >> 4); }
             }
-            const bool chunk_done = is_sc || st == SPC - 1 || j == j_end - 1;
+            const bool chunk_done = is_sc || st == SPC - 1 || i == ks.n - 1 || i == ks.ne - 1;
             fence_acc(acc);
             wgmma_fence();
 #pragma unroll
@@ -563,7 +629,6 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
             __syncwarp();
             accum = 1;
             if (chunk_done) { ++ause; ab = ause % NAB; }
-            if (++st == SPC) st = 0;
             if (++s == NSTB) { s = 0; ++k; }
         }
         wgmma_wait<0>();
@@ -572,6 +637,17 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
     } else {
         // ================= A-operand producers: gather + pre-op + swizzled stores =================
         const int ptid = tid - NCONS;
+        // griddepcontrol.wait right before the first late chunk's gather (slice step ks.ne), or after the last chunk when the whole
+        // slice is early (see the invariant at the padding exit); slot 13 = the early chunks are gathered, slot 3 = the dependency
+        // has resolved
+        auto acquire = [&]() {
+            if (ptid == 0 && ks.ne > 0) SIGE_TRACE(13);
+            if (p.pdl) {
+                pdl_acquire();
+                if (p.early_release) pdl_release();
+            }
+            if (ptid == 0) SIGE_TRACE(3);
+        };
         if constexpr (S2) {
             // ---- stride-2 geometry: 32 tiles x 5x5 halo pixels x 8 units = 6400 sixteen-byte copies per chunk, pure copy with
             //      cp.async straight into the plane layout described at S2_TILES.  Thread -> (tile = ptid / 8, unit = ptid % 8), and
@@ -593,11 +669,12 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
             const uint32_t d_ox0 = sbase + C::OFF_A + (tl * 2) * 128 + ((u ^ ((tl * 2) & 7)) << 4);
             const uint32_t d_ox1 = sbase + C::OFF_A + (tl * 2 + 1) * 128 + ((u ^ ((tl * 2 + 1) & 7)) << 4);
             if (ptid == 0) SIGE_TRACE(2);
-            if (p.pdl) pdl_acquire();   // activations of the previous layer are complete
             int ause = 0;
-            for (int c = c_first; c <= c_last; ++c) {
+            for (int i = 0, next; i < ks.n; i = next) {                   // (no fused shortcut, no early chunks: KOrder)
+                const int j = step_at(i), c = chunk_of(j);
+                next = chunk_end(i, j);
+                if (i == 0) acquire();                                    // activations of the previous layer are complete
                 mbar_wait(A_EMPTY(0), (ause & 1) ^ 1);                    // the MMAs that read the (single) halo buffer have retired
-                if (ptid == 0 && c == c_first) SIGE_TRACE(3);
                 const int cbase = c * KC;
                 const int sg = cbase >= p.C0 ? 1 : 0;
                 const Seg &seg = p.seg[sg];
@@ -623,9 +700,10 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
                     }
                 }
                 cp_async_arrive(A_FULL(0));
-                if (ptid == 0 && c == c_first) SIGE_TRACE(4);
+                if (ptid == 0 && i == 0) SIGE_TRACE(4);
                 ++ause;
             }
+            if (ks.n == 0) acquire();
         } else {
         // per-thread gather list (fixed for the whole kernel)
         int g_xyt[LOADS];     // x | y << 4 | tile << 8 of the halo pixel this load feeds
@@ -667,6 +745,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
             const int y = rem / R, x = rem - y * R;
             g_xyt[k] = x | (y << 4) | (tl << 8);
         }
+        const int c_first = ks.n > 0 ? chunk_of(step_at(0)) : 0;
         resolve(c_first < NC && c_first * KC >= p.C0 ? 1 : 0);
         if (ptid == 0) SIGE_TRACE(2);   // bookkeeping (idx loads) done
         uint4 regs[LOADS];
@@ -854,37 +933,51 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
                 }
                 cp_async_arrive(full_bar);
             };
-            if (p.pdl) pdl_acquire();   // activations of the previous layer are complete
             int ab = 0, ause = 0;
-            for (int c = c_first; c <= c_last; ++c) {
+            for (int i = 0, next; i < ks.n; i = next) {
+                const int j = step_at(i), c = chunk_of(j);
+                next = chunk_end(i, j);
+                if (i == ks.ne) acquire();                                // activations of the previous layer are complete
                 mbar_wait(A_EMPTY(ab), ((ause / NAB) & 1) ^ 1);           // the MMAs that read this buffer have retired
-                if (ptid == 0 && c == c_first) SIGE_TRACE(3);
                 copy_chunk(c, smem + C::OFF_A + ab * A_BUF_BYTES, A_FULL(ab));
-                if (ptid == 0 && c == c_first) SIGE_TRACE(4);
+                if (ptid == 0 && i == 0) SIGE_TRACE(4);
                 ++ause;
                 ab = ause % NAB;
             }
+            if (ks.ne == ks.n) acquire();
         } else {
-        if (p.pdl) pdl_acquire();   // activations of the previous layer are complete
-        issue_any(c_first);
+        if (ks.n > 0) {
+            if (ks.ne == 0) acquire();                                // activations of the previous layer are complete
+            issue_any(c_first);
+        }
         int ab = 0, ause = 0;
-        for (int c = c_first; c <= c_last; ++c) {
+        for (int i = 0; i < ks.n;) {
+            const int j = step_at(i), c = chunk_of(j), next = chunk_end(i, j);
             mbar_wait(A_EMPTY(ab), ((ause / NAB) & 1) ^ 1);           // the MMAs that read this buffer have retired
-            if (ptid == 0 && c == c_first) SIGE_TRACE(3);
             if (c < NC) store(c, smem + C::OFF_A + ab * A_BUF_BYTES); else store2(smem + C::OFF_A + ab * A_BUF_BYTES);
-            if (ptid == 0 && c == c_first) SIGE_TRACE(4);
+            if (ptid == 0 && i == 0) SIGE_TRACE(4);
             fence_proxy_async();                                      // generic-proxy stores -> visible to the tensor core
             mbar_arrive(A_FULL(ab));
-            if (c < c_last) issue_any(c + 1);
+            if (next < ks.n) {
+                if (next == ks.ne) acquire();
+                issue_any(chunk_of(step_at(next)));
+            }
+            i = next;
             ++ause;
             ab = ause % NAB;
         }
+        if (ks.ne == ks.n) acquire();
         }
         }   // !S2
     }
 
     // ---------------- epilogue ----------------
-    if (p.pdl) pdl_release();             // the next layer's prologue may overlap this epilogue
+    // the next layer's prologue may overlap this epilogue.  A thread waits before it releases: the first release of a CTA is what
+    // counts, and the weight-loading warp can get here before the producers' wait has returned.
+    if (p.pdl) {
+        pdl_acquire();
+        pdl_release();
+    }
     float *cst = reinterpret_cast<float *>(smem + C::OFF_A);
     // v[8] (fp32 conv result of 8 consecutive channels starting at n) -> +bias, +residual -> dst and aux destinations
     auto emit = [&](long long pixel, int tl, int n, float (&v)[8]) {
@@ -1094,7 +1187,8 @@ static Machine machine() {
     return cache[dev];
 }
 
-static Plan decide(long long NT, int Cin, int Cout, int taps, int Cin2, int ksplit_req, bool s2 = false) {
+// C0, early: channels of src[0] and the SIGE_CONV_EARLY_* mask, for the K partition (KOrder)
+static Plan decide(long long NT, int Cin, int C0, int Cout, int taps, int Cin2, int early, int ksplit_req, bool s2 = false) {
     Plan pl;
     const long long m_blocks = ceil_div(NT, s2 ? S2_TILES : TILES);
     // BN = 128 when that still fills the machine — or when the narrow tiling would need more waves of one-per-SM CTAs
@@ -1107,7 +1201,13 @@ static Plan decide(long long NT, int Cin, int Cout, int taps, int Cin2, int kspl
     pl.bn = wide ? 128 : 64;
     const bool split_ok = pl.bn == 64;                       // Cfg::kSplitOk
     const int tps = (taps == 9 && pl.bn == 64) ? 3 : 1;     // Cfg::TPS
-    const int J = (Cin / KC) * (taps / tps) + (taps == 9 ? Cin2 / KC : 0);        // ring steps
+    const KOrder ko(Cin, C0, (taps == 9 && !s2) ? Cin2 : 0, taps / tps, s2 ? 0 : early);
+    const int J = ko.J;                                      // ring steps
+    auto shortest = [&](int k) {                             // steps of the shortest K slice of a k-way split
+        int m = J;
+        for (int kr = 0; kr < k; ++kr) m = min(m, KSlice(ko, kr, k).n);
+        return m;
+    };
     const long long base = m_blocks * (Cout / pl.bn);
     int ks = ksplit_req;
     if (ks <= 0) {
@@ -1115,7 +1215,7 @@ static Plan decide(long long NT, int Cin, int Cout, int taps, int Cin2, int kspl
         constexpr int kMinTaps = 3;
         const int *kMaxCtas = mc.max_ctas;
         ks = 1;
-        while (split_ok && ks < 8 && base * (ks * 2) <= kMaxCtas[ks * 2] && (J * tps) / (ks * 2) >= kMinTaps) ks *= 2;
+        while (split_ok && ks < 8 && base * (ks * 2) <= kMaxCtas[ks * 2] && shortest(ks * 2) * tps >= kMinTaps) ks *= 2;
     }
     if (ks > J || !split_ok) ks = 1;
     pl.ksplit = ks;
@@ -1185,16 +1285,12 @@ static int launch(Params &p, const void *w_packed, const void *w2_packed, cudaSt
     return launch_v<T, BN, TAPS, DEEP, false, false, DB>(p, w_packed, w2_packed, st);
 }
 
-// Halo fills of the longest K slice of a split narrow 3x3 launch (the kernel's partition: k_slice, chunk_of).  One fill: the
+// Halo fills of the longest K slice of a split narrow 3x3 launch (the kernel's partition: KOrder, KSlice).  One fill: the
 // single-buffered layout (its deep weight ring has the whole slice in flight); more: the double-buffered one.
-static int split_halo_fills(int Cin, int Cin2, int ks) {
-    const int NC = Cin / KC, J_main = NC * 3, J = J_main + Cin2 / KC;
-    auto chunk_of = [&](int j) { return j < J_main ? j / 3 : NC + (j - J_main); };
+static int split_halo_fills(int Cin, int C0, int Cin2, int early, int ks) {
+    const KOrder ko(Cin, C0, Cin2, 3, early);
     int most = 0;
-    for (int kr = 0; kr < ks; ++kr) {
-        const int b = k_slice(J, kr, ks), e = k_slice(J, kr + 1, ks);
-        if (e > b && chunk_of(e - 1) - chunk_of(b) + 1 > most) most = chunk_of(e - 1) - chunk_of(b) + 1;
-    }
+    for (int kr = 0; kr < ks; ++kr) most = max(most, KSlice(ko, kr, ks).fills(ko));
     return most;
 }
 static int g_split_halo_buffers = 0;     // sige_debug_set_split_halo_buffers
@@ -1271,6 +1367,8 @@ int tc5_launch(const sige_tile_conv_t *a, cudaStream_t st) {
     p.padded = ((a->flags & SIGE_CONV_PADDED) && a->B == 1 && a->idx && !a->src_is_stack && !a->dst_is_stack) ? 1 : 0;
     p.ksplit = a->ksplit;
     p.pdl = (a->flags & SIGE_CONV_PDL) ? 1 : 0;
+    p.early_release = (a->flags & SIGE_CONV_EARLY_RELEASE) ? 1 : 0;
+    p.early = (a->flags >> 4) & 7;                                      // SIGE_CONV_EARLY_SRC0 | _SRC1 | _SHORTCUT
     p.is_bf16 = a->dtype == SIGE_BF16;
     p.trace = g_trace;
     const sige_conv_modulation_t *m = a->modulation;
@@ -1281,14 +1379,14 @@ int tc5_launch(const sige_tile_conv_t *a, cudaStream_t st) {
     p.bC = m ? m->beta_C : 0;
     p.slope = m ? m->negative_slope : 1.f;
     const bool s2 = !m && tc5_is_s2(a);
-    const tc5::Plan pl = tc5::decide(p.NT, p.Cin, p.Cout, p.taps, p.Cin2, a->ksplit, s2);
+    const tc5::Plan pl = tc5::decide(p.NT, p.Cin, p.C0, p.Cout, p.taps, p.Cin2, p.early, a->ksplit, s2);
     p.ksplit = pl.ksplit;
     if (s2) {
         if (a->dtype == SIGE_F16) return tc5::launch_v<__half, 64, 9, false, true, true>(p, a->w_packed, a->w2_packed, st);
         return tc5::launch_v<__nv_bfloat16, 64, 9, false, true, true>(p, a->w_packed, a->w2_packed, st);
     }
     const bool wide = pl.bn == 128, three = p.taps == 9;
-    const int nab = tc5::g_split_halo_buffers ? tc5::g_split_halo_buffers : (tc5::split_halo_fills(p.Cin, p.Cin2, p.ksplit) > 1 ? 2 : 1);
+    const int nab = tc5::g_split_halo_buffers ? tc5::g_split_halo_buffers : (tc5::split_halo_fills(p.Cin, p.C0, p.Cin2, p.early, p.ksplit) > 1 ? 2 : 1);
     const bool db = pl.deep && nab == 2;
 #define SIGE_TC5(T)                                                                              \
     (wide ? (three ? tc5::launch<T, 128, 9>(p, a->w_packed, a->w2_packed, st) : tc5::launch<T, 128, 1>(p, a->w_packed, a->w2_packed, st)) \
@@ -1309,7 +1407,8 @@ static void tc5_plan(const sige_tile_conv_t *a, sige_tile_conv_plan_t *out) {
     using namespace sige;
     const long long NT = (long long)a->B * a->N;
     const bool s2 = tc5_is_s2(a);
-    const tc5::Plan pl = tc5::decide(NT, a->Cin, a->Cout, a->kH * a->kW, a->n_src2 > 0 ? a->Cin2 : 0, a->ksplit, s2);
+    const int Cin2 = a->n_src2 > 0 ? a->Cin2 : 0;
+    const tc5::Plan pl = tc5::decide(NT, a->Cin, a->src[0].C, a->Cout, a->kH * a->kW, Cin2, (a->flags >> 4) & 7, a->ksplit, s2);
     out->path = 1;
     out->bn = pl.bn;
     out->ksplit = pl.ksplit;

@@ -128,6 +128,8 @@ class ConvSpec:
         self.pdl = False
         self.tc5 = False
         self.ksplit = 0
+        self.early = 0                                       # early source groups: SIGE_CONV_EARLY_* >> 4 (Lowering._early_masks)
+        self.early_release = False                           # SIGE_CONV_EARLY_RELEASE: the next launch has early source groups
 
     @property
     def Cin(self) -> int:
@@ -322,7 +324,7 @@ class CudaExecutor:
 
     def prepare_conv(self, fc: FusedConv) -> None:
         ops = self.ops
-        from ._cabi import CONV_PADDED, CONV_PDL, CONV_TC5
+        from ._cabi import CONV_EARLY_RELEASE, CONV_PADDED, CONV_PDL, CONV_TC5
 
         s = fc.spec
         w, b = s.weight, s.bias
@@ -375,7 +377,7 @@ class CudaExecutor:
         else:
             d.residual, d.rC, d.res_c0 = None, 0, 0
         d.ksplit = s.ksplit
-        d.flags = (CONV_PDL if s.pdl else 0) | (CONV_TC5 if s.tc5 else 0)
+        d.flags = (CONV_PDL if s.pdl else 0) | (CONV_TC5 if s.tc5 else 0) | (CONV_EARLY_RELEASE if s.early_release else 0) | (s.early << 4)
         if s.slot is not None and s.tile_img is None and s.B == 1 and s.slot.cap - s.slot.n >= 8:
             d.flags |= CONV_PADDED          # whole CTAs of padding exist (capacity headroom): let them exit at once
         d.n_aux = len(s.aux)
@@ -412,6 +414,12 @@ class CudaExecutor:
         keep += [idx_t, sc_flags_t]
         fc.desc, fc.keep = d, keep
         fc.launch_fn = lambda stream, d=d: ops.launch_tile_conv(d, stream)
+
+    def takes_wgmma(self, fc: FusedConv) -> bool:
+        """Whether the prepared launch runs on the wgmma kernel (sige_tile_conv_plan)."""
+        pl = self.ops._cabi.TileConvPlan()
+        self.ops._cabi.check(self.ops._cabi.lib().sige_tile_conv_plan(ctypes.byref(fc.desc), ctypes.byref(pl)), "sige_tile_conv_plan")
+        return pl.path == 1
 
     def prepare_conv_in(self, rec: ConvInRec) -> Callable[[int], None]:
         ops = self.ops
@@ -2477,10 +2485,54 @@ class Lowering:
             s = fc.spec
             if s.dst is not None and not s.aux:
                 _ = s.dst.raw             # a value nobody transformed: keep the raw destination
+        self._early_masks()
+        for fc in self.fused:
             self.ex.prepare_conv(fc)
+        takes_wgmma = getattr(self.ex, "takes_wgmma", None)
+        if takes_wgmma is not None:
+            for fc in self.fused:
+                prev = self._conv_at.get(fc.pos - 1)
+                if fc.spec.early and not takes_wgmma(prev):          # (the mma.sync kernel releases before it waits)
+                    fc.spec.early, prev.spec.early_release = 0, False
+                    fc.desc.flags &= ~(7 << 4)
+                    prev.desc.flags &= ~self.ex.ops._cabi.CONV_EARLY_RELEASE
         for prep in self._pending_prepare:
             prep()
         self._build_sparse_update()
+
+    def _early_masks(self) -> None:
+        """The early source groups of every launch (SIGE_CONV_EARLY_SRC0 / _SRC1 / _SHORTCUT, kept as bits 0..2 in ConvSpec.early):
+        the source groups that the immediately preceding step does not write.  Only when that step is a tile conv meant for the wgmma kernel
+        (it waits for its own predecessor before it releases this launch; the attention, glue and mma.sync kernels release first)
+        and both launches use programmatic dependent launch.  The predecessor of a launch with a mask releases it as soon as its
+        own dependency has resolved (SIGE_CONV_EARLY_RELEASE).  Masks depend on buffers and launch order only, not on tiles, so
+        `rebind` keeps them; the sparse_update epilogue leaves them 0."""
+        self._conv_at = {fc.pos: fc for fc in self.fused}
+
+        def key(t):
+            return t.untyped_storage().data_ptr()
+
+        for fc in self.fused:
+            s = fc.spec
+            prev = self._conv_at.get(fc.pos - 1)
+            if not (s.pdl and s.tc5 and prev is not None and prev.spec.pdl and prev.spec.tc5):
+                continue
+            p = prev.spec
+            written = {key(v) for (v, _, _, _) in p.aux}
+            if p.dst_stack is not None:
+                written.add(key(p.dst_stack))
+            if p.dst is not None and p.dst.has_raw:
+                written.add(key(p.dst.raw))
+            pre = [t for t in (s.scale, s.shift) if t is not None] + (list(s.modulation[:2]) if s.modulation is not None else [])
+            groups = [[t] + pre for t, _ in s.srcs[:2]]
+            if s.shortcut is not None:
+                groups += [[]] * (2 - len(groups)) + [list(s.shortcut[0])]
+            mask = 0
+            for g, reads in enumerate(groups):
+                if reads and not any(key(t) in written for t in reads):
+                    mask |= 1 << g
+            if mask:
+                s.early, p.early_release = mask, True
 
     # ------------------------------------------------------------------ sparse_update epilogue
     def _sparse_update_refusal(self) -> Optional[str]:
@@ -2506,6 +2558,7 @@ class Lowering:
 
     def _relaunch(self, spec: ConvSpec, name: str) -> FusedConv:
         spec.name, spec.pdl = name, False          # (the epilogue's first launch follows another graph)
+        spec.early, spec.early_release = 0, False
         fc = FusedConv(spec)
         self.ex.prepare_conv(fc)
         self.epilogue_fused.append(fc)
