@@ -80,6 +80,18 @@ int sige_activation_from_name(const char *name);
 int sige_reduce_mask(const uint8_t *mask, int H, int W, int R, int S, int strideH, int strideW,
                      int padH, int padW, int32_t *idx_out, int capacity, int32_t *count_out,
                      sige_stream_t stream);
+/*
+ * E masks of one geometry, uint8 [E, H, W], in ONE launch (one CTA per mask, each the
+ * ordered compaction of sige_reduce_mask): image e's tiles go to rows e*cap + i of
+ * idx_out [E*cap, 2] (the per-image layout of sige_tile_conv_t.idx_per_image) in the
+ * same order as sige_reduce_mask, SIGE_TILE_NONE fills the rest of each image's rows.
+ * counts_out[e] (device int32) = the number of active tiles of image e.  An image with
+ * more than cap keeps its first cap tiles and bit 0 of *status (device int32) is set;
+ * the word is only ever OR-ed, never cleared.  E == 0 is a no-op.
+ */
+int sige_reduce_mask_batched(const uint8_t *masks, int E, int H, int W, int R, int S, int strideH,
+                             int strideW, int padH, int padW, int32_t *idx_out, int cap,
+                             int32_t *counts_out, int32_t *status, sige_stream_t stream);
 /* host helper: number of candidate tiles (upper bound for `capacity`) */
 int sige_reduce_mask_capacity(int H, int W, int R, int S, int strideH, int strideW, int padH,
                               int padW);
@@ -272,9 +284,12 @@ typedef struct {
 /* Use the wgmma / TMA kernel when the geometry allows (3x3 s1 on 6x6 tiles, 1x1 on 4x4 tiles,
  * Cout % 64 == 0); otherwise the mma.sync kernel runs. */
 #define SIGE_CONV_TC5 2
-/* `idx` is a fixed-capacity list (B == 1): real tiles packed at the front, SIGE_TILE_NONE entries behind them, possibly whole
- * CTAs' worth — CTAs made only of padding exit at once.  (Without the flag padding entries are still harmless: they read zeros
- * and write nothing; the flag only buys the early exit, at the price of one index load on every CTA's prologue.) */
+/* `idx` is a fixed-capacity list (B == 1), or B of them (idx_per_image == 1): real tiles packed at the front of each list,
+ * SIGE_TILE_NONE entries behind them, possibly whole CTAs' worth — CTAs made only of padding exit at once.  With per-image lists
+ * the flag takes effect only when N is a multiple of the kernel's tiles per CTA (8 for the stride-1 geometries of either kernel,
+ * 32 for the wgmma stride-2 one, the plan's tiles per CTA on the mma.sync kernel), so that no CTA holds tiles of two images.
+ * (Without the flag padding entries are still harmless: they read zeros and write nothing; the flag only buys the early exit,
+ * at the price of one index load on every CTA's prologue.) */
 #define SIGE_CONV_PADDED 4
 /* With SIGE_CONV_PDL on the wgmma kernel: release the next launch right after this launch's own dependency has resolved, instead
  * of at the epilogue, so that the next launch's CTAs take the SMs this one leaves idle and gather their early chunks (below)

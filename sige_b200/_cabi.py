@@ -126,6 +126,7 @@ PROTOTYPES = {
     "sige_built_arch": (c_char_p, []),
     "sige_activation_from_name": (_I, [c_char_p]),
     "sige_reduce_mask": (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _I, _P, _P]),
+    "sige_reduce_mask_batched": (_I, [_P] + [_I] * 9 + [_P, _I, _P, _P, _P]),
     "sige_reduce_mask_capacity": (_I, [_I] * 8),
     "sige_gather": (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _I, _BP, _BP, _I, _I, _P, _P]),
     "sige_gather_upsampled": (_I, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P, _I, _BP, _BP, _I, _I, _P, _P]),

@@ -64,7 +64,7 @@ struct ConvParams {
     int src_is_stack;
     const int32_t *idx;
     int N, NT;              // tiles per batch element, total tiles (B*N)
-    int padded;             // SIGE_CONV_PADDED (B == 1): whole CTAs of padding may follow the real tiles
+    int padded;             // SIGE_CONV_PADDED: whole CTAs of padding may follow the real tiles (of each image)
     int idx_per_image;      // 1: idx holds B*N entries (row b*N + i = tile i of image b), else N shared by all images
     int R, S, RS;
     const float *scale, *shift;
@@ -505,6 +505,7 @@ static int launch_cfg(ConvParams &p, const MmaPlan &pl, cudaStream_t st) {
         attr_dev = dev;
     }
     p.tpc = pl.tpc;
+    if (p.NT > p.N && p.N % pl.tpc) p.padded = 0;       // B > 1: a CTA must not hold tiles of two images
     p.ksplit = pl.ksplit;
     const dim3 grid(pl.grid_x, pl.grid_y, pl.ksplit);
     const cudaError_t e = launch_ex(kern, grid, dim3(Cfg::NTHREADS), Cfg::SMEM_BYTES, st, p.pdl != 0, dim3(1, 1, p.ksplit), p);
@@ -656,7 +657,8 @@ extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) {
     p.N = a->N;
     p.NT = a->B * a->N;
     p.idx_per_image = a->idx_per_image ? 1 : 0;
-    p.padded = ((a->flags & SIGE_CONV_PADDED) && a->B == 1 && a->idx && !a->src_is_stack && !a->dst_is_stack) ? 1 : 0;
+    // (per-image lists: launch_cfg keeps the flag only when a list is a whole number of CTAs, see tile_conv_tc5.cu)
+    p.padded = ((a->flags & SIGE_CONV_PADDED) && a->idx && !a->src_is_stack && !a->dst_is_stack && (a->B == 1 || a->idx_per_image)) ? 1 : 0;
     p.R = a->R; p.S = a->S; p.RS = a->R * a->S;
     p.scale = a->scale; p.shift = a->shift; p.affine_bstride = a->affine_bstride; p.act = a->act;
     p.w = a->w_packed; p.bias = a->bias;

@@ -94,7 +94,7 @@ struct Params {
     int C0_2, Cin2;
     const float *bias2;
     const unsigned char *sc_flags;
-    int padded;                // SIGE_CONV_PADDED: whole CTAs of SIGE_TILE_NONE padding may follow the real tiles (B == 1)
+    int padded;                // SIGE_CONV_PADDED: whole CTAs of SIGE_TILE_NONE padding may follow the real tiles (of each image)
     int idx_per_image;         // 1: idx / sc_flags hold B*N entries (row b*N + i = tile i of image b), else N shared by all images
     int ksplit;
     int pdl;                   // launched with programmatic dependent launch: the next layer is released at the epilogue
@@ -430,7 +430,7 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int tile0 = blockIdx.x * TILES;
-    // fixed-capacity tile lists (one image): real tiles are packed at the front, the rest are SIGE_TILE_NONE.  A CTA (and with it
+    // fixed-capacity tile lists (one per image): real tiles are packed at the front, the rest are SIGE_TILE_NONE.  A CTA (and with it
     // its whole split-K cluster: same tile0) whose first tile is padding has nothing to read or write.
     // Early chunks (p.early) read buffers that the preceding launch does not write, before griddepcontrol.wait.  That is sound
     // because every CTA of every launch waits before it releases its dependents and before it exits (here, in the producers and
@@ -1364,7 +1364,6 @@ int tc5_launch(const sige_tile_conv_t *a, cudaStream_t st) {
     p.bias2 = a->n_src2 > 0 ? a->bias2 : nullptr;
     p.sc_flags = a->n_src2 > 0 ? a->sc_flags : nullptr;
     p.idx_per_image = a->idx_per_image ? 1 : 0;
-    p.padded = ((a->flags & SIGE_CONV_PADDED) && a->B == 1 && a->idx && !a->src_is_stack && !a->dst_is_stack) ? 1 : 0;
     p.ksplit = a->ksplit;
     p.pdl = (a->flags & SIGE_CONV_PDL) ? 1 : 0;
     p.early_release = (a->flags & SIGE_CONV_EARLY_RELEASE) ? 1 : 0;
@@ -1379,6 +1378,10 @@ int tc5_launch(const sige_tile_conv_t *a, cudaStream_t st) {
     p.bC = m ? m->beta_C : 0;
     p.slope = m ? m->negative_slope : 1.f;
     const bool s2 = !m && tc5_is_s2(a);
+    // a CTA's first index row is row tile0 of `idx`: one list (B == 1), or per-image lists whose length is a whole number of CTAs
+    // (no CTA then holds tiles of two images, so padding behind one image's tiles fills whole CTAs)
+    p.padded = ((a->flags & SIGE_CONV_PADDED) && a->idx && !a->src_is_stack && !a->dst_is_stack &&
+                (a->B == 1 || (a->idx_per_image && a->N % (s2 ? tc5::S2_TILES : tc5::TILES) == 0))) ? 1 : 0;
     const tc5::Plan pl = tc5::decide(p.NT, p.Cin, p.C0, p.Cout, p.taps, p.Cin2, p.early, a->ksplit, s2);
     p.ksplit = pl.ksplit;
     if (s2) {

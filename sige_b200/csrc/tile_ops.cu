@@ -279,11 +279,11 @@ __global__ void scatter_gather_nhwc_kernel(long long total, TileGeom g, int Rx, 
 // reduce_mask  (reference sige/utils.py:8-37) — device-side, ordered compaction.
 // One CTA walks the pooled grid in row-major chunks of blockDim.x candidates; each
 // thread tests its R x S window, a ballot + warp-total scan gives the rank, so the
-// output order equals torch.nonzero's row-major order bit for bit.
+// output order equals torch.nonzero's row-major order bit for bit.  Writes the first
+// `capacity` origins and returns the number of active tiles (to every thread).
 // ----------------------------------------------------------------------------
-__global__ void reduce_mask_kernel(const uint8_t *__restrict__ mask, int H, int W, int R, int S, int strideH,
-                                   int strideW, int padH, int padW, int nI, int nJ, int32_t *__restrict__ out,
-                                   int capacity, int32_t *__restrict__ count) {
+__device__ int reduce_mask_cta(const uint8_t *__restrict__ mask, int H, int W, int R, int S, int strideH, int strideW,
+                               int padH, int padW, int nI, int nJ, int32_t *__restrict__ out, int capacity) {
     __shared__ int warp_tot[32];
     __shared__ int base_s;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
@@ -323,7 +323,29 @@ __global__ void reduce_mask_kernel(const uint8_t *__restrict__ mask, int H, int 
         if (threadIdx.x == 0) base_s = base + chunk;
         __syncthreads();
     }
-    if (threadIdx.x == 0) *count = base_s;
+    return base_s;
+}
+
+__global__ void reduce_mask_kernel(const uint8_t *__restrict__ mask, int H, int W, int R, int S, int strideH,
+                                   int strideW, int padH, int padW, int nI, int nJ, int32_t *__restrict__ out,
+                                   int capacity, int32_t *__restrict__ count) {
+    const int total = reduce_mask_cta(mask, H, W, R, S, strideH, strideW, padH, padW, nI, nJ, out, capacity);
+    if (threadIdx.x == 0) *count = total;
+}
+
+// E masks of one geometry, one CTA per mask: image e's list goes to rows e*cap .. e*cap + cap - 1 (the per-image layout of
+// sige_tile_conv_t.idx_per_image), SIGE_TILE_NONE behind its tiles.
+__global__ void reduce_mask_batched_kernel(const uint8_t *__restrict__ masks, int H, int W, int R, int S, int strideH,
+                                           int strideW, int padH, int padW, int nI, int nJ, int32_t *__restrict__ out,
+                                           int cap, int32_t *__restrict__ counts, int32_t *__restrict__ status) {
+    const int e = blockIdx.x;
+    int32_t *seg = out + 2LL * e * cap;
+    const int total = reduce_mask_cta(masks + (long long)e * H * W, H, W, R, S, strideH, strideW, padH, padW, nI, nJ, seg, cap);
+    for (int i = 2 * min(total, cap) + threadIdx.x; i < 2 * cap; i += blockDim.x) seg[i] = SIGE_TILE_NONE;
+    if (threadIdx.x == 0) {
+        counts[e] = total;
+        if (total > cap) atomicOr(status, 1);
+    }
 }
 
 // ----------------------------------------------------------------------------
@@ -463,6 +485,22 @@ int sige_reduce_mask(const uint8_t *mask, int H, int W, int R, int S, int stride
     reduce_mask_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(mask, H, W, R, S, strideH, strideW, padH, padW, nI, nJ,
                                                              idx_out, capacity, count_out);
     return check_launch("sige_reduce_mask");
+}
+
+int sige_reduce_mask_batched(const uint8_t *masks, int E, int H, int W, int R, int S, int strideH, int strideW, int padH,
+                             int padW, int32_t *idx_out, int cap, int32_t *counts_out, int32_t *status,
+                             sige_stream_t stream) {
+    SIGE_REQUIRE(E >= 0 && cap >= 0, "sige_reduce_mask_batched: negative E (%d) or cap (%d)", E, cap);
+    if (E == 0) return 0;
+    SIGE_REQUIRE(masks && counts_out && status, "sige_reduce_mask_batched: null pointer");
+    SIGE_REQUIRE(H > 0 && W > 0 && R > 0 && S > 0 && strideH > 0 && strideW > 0 && padH >= 0 && padW >= 0,
+                 "sige_reduce_mask_batched: bad geometry H=%d W=%d R=%d S=%d stride=(%d,%d) pad=(%d,%d)", H, W, R, S,
+                 strideH, strideW, padH, padW);
+    SIGE_REQUIRE(cap == 0 || idx_out, "sige_reduce_mask_batched: idx_out is null with cap %d", cap);
+    const int nI = (H + padH) / strideH + 1, nJ = (W + padW) / strideW + 1;
+    reduce_mask_batched_kernel<<<E, 1024, 0, (cudaStream_t)stream>>>(masks, H, W, R, S, strideH, strideW, padH, padW, nI,
+                                                                     nJ, idx_out, cap, counts_out, status);
+    return check_launch("sige_reduce_mask_batched");
 }
 
 int sige_gather(const void *x, int dtype, int layout, int B, int C, int H, int W, int R, int S, const int32_t *idx,

@@ -102,8 +102,8 @@ class ConvSpec:
         self.B = 1
         self.H = self.W = 0
         self.idx: Optional[torch.Tensor] = None
-        self.tile_img: Optional[torch.Tensor] = None         # int32 [N]: a batch of independent edits (idx = concatenated lists)
-        self.slot: Optional["IdxSlot"] = None                # fixed-capacity index buffer (N = capacity, slot.n tiles are real)
+        self.tile_img: Optional[torch.Tensor] = None         # int32 [N]: a batch of independent edits (image of each row of idx)
+        self.slot: Optional["IdxSlot"] = None                # fixed-capacity index buffer (N = capacity, or E * capacity for a batch)
         self.N = 0
         self.block = 0
         self.scale: Optional[torch.Tensor] = None            # fp32 [Cin] or [B, Cin]
@@ -168,9 +168,8 @@ class FusedConv:
     @property
     def tiles(self) -> int:
         s = self.spec
-        if s.tile_img is not None:
-            return s.N
-        return s.B * (s.slot.n if s.slot is not None else s.N)
+        n = s.slot.n if s.slot is not None else s.N
+        return n if s.tile_img is not None else s.B * n         # (a batch's lists hold the tiles of every edit)
 
     @property
     def out_elems(self) -> int:
@@ -204,29 +203,58 @@ class FusedConv:
 class IdxSlot:
     """A tile list with a fixed capacity: the launches hold this buffer's address and N = capacity; entries beyond the current
     count are SIGE_TILE_NONE origins (such a tile reads zeros and writes nothing, include/sige_b200.h).  A new mask whose lists
-    fit is installed by rewriting the buffers in place (`FusedStep.rebind`): no re-trace, no re-capture."""
+    fit is installed by rewriting the buffers in place (`FusedStep.rebind`): no re-trace, no re-capture.
+
+    A batch of E independent edits (the Gather has `tile_images`) gets one list of `cap` rows per edit: `buf` is [E*cap, 2], row
+    e*cap + i = tile i of edit e (the per-image layout of sige_tile_conv_t.idx_per_image and of `sige_reduce_mask_batched`), and
+    `tile_img` is the constant image index row // cap of every row.  `cap` is the longest list at build time, or with headroom
+    that times (1 + headroom) rounded up to a multiple of 8, so that padding fills whole CTAs (SIGE_CONV_PADDED)."""
 
     def __init__(self, gather, dev, headroom: float = 0.0):
         from ._cabi import TILE_NONE
 
         self.gather = gather
-        idx = gather.active_indices.to(dev)
-        self.n = int(idx.shape[0])
-        self.cap = max(8, (int(math.ceil(self.n * (1.0 + headroom))) + 7) // 8 * 8)
-        self.buf = torch.full((self.cap, 2), TILE_NONE, dtype=torch.int32, device=dev)
-        self.buf[:self.n] = idx
         self.none = TILE_NONE
+        timg = getattr(gather, "tile_images", None)
+        self.E = 1 if timg is None else int(gather.num_edits)
+        self.tile_img: Optional[torch.Tensor] = None
+        if timg is None:
+            self.cap = max(8, (int(math.ceil(int(gather.active_indices.shape[0]) * (1.0 + headroom))) + 7) // 8 * 8)
+        else:
+            top = int(self._counts().max())
+            self.cap = top if headroom <= 0 else (int(math.ceil(top * (1.0 + headroom))) + 7) // 8 * 8
+            self.tile_img = (torch.arange(self.E * self.cap, dtype=torch.int32) // max(self.cap, 1)).to(dev)
+        self.padded = headroom > 0          # batches: whole CTAs of padding may follow each edit's tiles
+        self.buf = torch.full((self.E * self.cap, 2), TILE_NONE, dtype=torch.int32, device=dev)
+        self.reload()
+
+    def _counts(self) -> torch.Tensor:
+        """Tiles per edit of the gather's current lists (a batch)."""
+        g = self.gather
+        return torch.bincount(g.tile_images.long().cpu(), minlength=int(g.num_edits))
 
     def fits(self) -> bool:
         g = self.gather
-        return getattr(g, "tile_images", None) is None and g.active_indices is not None and int(g.active_indices.shape[0]) <= self.cap \
-            and int(g.active_indices.shape[0]) > 0
+        timg = getattr(g, "tile_images", None)
+        if g.active_indices is None or int(g.active_indices.shape[0]) == 0 or (timg is None) != (self.tile_img is None):
+            return False
+        if timg is None:
+            return int(g.active_indices.shape[0]) <= self.cap
+        return int(g.num_edits) == self.E and int(self._counts().max()) <= self.cap
 
     def reload(self) -> None:
         idx = self.gather.active_indices.to(self.buf.device)
         self.n = int(idx.shape[0])
-        self.buf[:self.n] = idx
-        self.buf[self.n:] = self.none
+        if self.tile_img is None:
+            self.buf[:self.n] = idx
+            self.buf[self.n:] = self.none
+            return
+        img = self.gather.tile_images.to(self.buf.device).long()           # the concatenated lists are in edit order
+        counts = torch.bincount(img, minlength=self.E)
+        starts = torch.cumsum(counts, 0) - counts
+        rows = img * self.cap + (torch.arange(self.n, device=img.device) - starts[img])
+        self.buf.fill_(self.none)
+        self.buf[rows] = idx
 
     def install_device(self, out: torch.Tensor, count: torch.Tensor, status: torch.Tensor) -> None:
         """Install the result of `sige_reduce_mask` (`out` [candidates, 2] of which the first `count` rows are real, `count` a
@@ -240,6 +268,37 @@ class IdxSlot:
         self.buf.copy_(torch.where(rows < count.view(1, 1), src, torch.full_like(src, self.none)))
         status.bitwise_or_((count > cap).to(torch.int32))
         self.n = cap           # the real count is only known on the device: host-side code treats every entry as potentially real
+
+    def install_batched_device(self, masks: torch.Tensor, status: torch.Tensor) -> None:
+        """Reduce the [E, H, W] CUDA masks of a batch straight into `buf` (one `sige_reduce_mask_batched` launch): each edit's
+        first min(count, cap) origins, SIGE_TILE_NONE behind them; bit 0 of `status` (device int32) if an edit's list did not fit."""
+        from . import ops
+
+        g = self.gather
+        ops.reduce_mask_batched_cuda(masks, g.block_size, g.block_stride, g.offset, self.cap, out=self.buf, status=status)
+        self.n = self.E * self.cap
+
+
+def _shortcut_flags(ms: IdxSlot, off: int, ss: IdxSlot, soff: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The fused 1x1 shortcut's flags of a main conv's list `ms` (origin offset `off`) against the shortcut's list `ss`: uint8,
+    one per row of ms.buf, 1 where the row is a real tile whose centre 4x4 tile is in the shortcut's list of the same edit; and
+    an int32 [1] that is 1 when some shortcut tile is no such centre (it left the main conv's grid).  Device tensor arithmetic
+    only, sorted per edit — no host synchronisation (torch.isin would synchronise)."""
+    E, width = ms.E, 1 << 16
+    mi, si = ms.buf.view(E, ms.cap, 2).long(), ss.buf.view(E, ss.cap, 2).long()
+    real_m, real_s = mi[..., 0] > ms.none, si[..., 0] > ss.none
+    main_key = torch.where(real_m, (mi[..., 0] + off) * width + (mi[..., 1] + off), torch.full_like(mi[..., 0], -1))
+    sc_key = torch.where(real_s, (si[..., 0] + soff) * width + (si[..., 1] + soff), torch.full_like(si[..., 0], -2))
+
+    def member(keys, pool):          # [E, n] keys found in the same edit's row of pool [E, m]
+        if pool.shape[1] == 0:
+            return torch.zeros_like(keys, dtype=torch.bool)
+        srt = torch.sort(pool, dim=1).values
+        return srt.gather(1, torch.searchsorted(srt, keys).clamp(max=srt.shape[1] - 1)) == keys
+
+    flags = (member(main_key, sc_key) & real_m).to(torch.uint8).view(-1)
+    stray = (~member(sc_key, main_key) & real_s).any().to(torch.int32).view(1)
+    return flags, stray
 
 
 class ConvInRec:
@@ -299,29 +358,6 @@ class CudaExecutor:
             _PACKED[k] = (weakref.ref(param), param._version, wp)
         return wp
 
-    def per_image_tiles(self, idx: torch.Tensor, tile_img: torch.Tensor, batch: int, flags: Optional[torch.Tensor] = None):
-        """(idx [N, 2] concatenated per-edit lists, tile_img [N]) -> the C-ABI's per-image layout: ([B*Nmax, 2] with row
-        b*Nmax + i = tile i of image b, padded with SIGE_TILE_NONE; Nmax; flags padded with 0)."""
-        from ._cabi import TILE_NONE
-
-        key = (idx.data_ptr(), tile_img.data_ptr(), int(idx.shape[0]), batch)
-        memo = self.__dict__.setdefault("_per_image", {})
-        if key not in memo:
-            img = tile_img.long()
-            counts = torch.bincount(img, minlength=batch)
-            nmax = max(1, int(counts.max()))
-            starts = torch.cumsum(counts, 0) - counts
-            rows = img * nmax + (torch.arange(img.numel(), device=img.device) - starts[img])
-            padded = torch.full((batch * nmax, 2), TILE_NONE, dtype=torch.int32, device=idx.device)
-            padded[rows] = idx
-            memo[key] = (padded.contiguous(), nmax, rows, idx, tile_img)
-        padded, nmax, rows = memo[key][:3]
-        pflags = None
-        if flags is not None:
-            pflags = torch.zeros((batch * nmax,), dtype=torch.uint8, device=idx.device)
-            pflags[rows] = flags
-        return padded, nmax, pflags
-
     def prepare_conv(self, fc: FusedConv) -> None:
         ops = self.ops
         from ._cabi import CONV_EARLY_RELEASE, CONV_PADDED, CONV_PDL, CONV_TC5
@@ -348,13 +384,12 @@ class CudaExecutor:
             d.src_pixel_stride = ops.channel_window(s.srcs[0][0])[1]        # a channel window of a wider buffer
         d.B, d.H, d.W = s.B, s.H, s.W
         d.src_is_stack = 1 if s.src_is_stack else 0
-        idx_t, n_per, sc_flags_t = s.idx, s.N, (None if s.shortcut is None else s.shortcut[3])
+        idx_t, sc_flags_t = s.idx, (None if s.shortcut is None else s.shortcut[3])
         d.idx_per_image = 0
-        if s.tile_img is not None:           # batch of independent edits -> padded per-image tile lists
-            idx_t, n_per, sc_flags_t = self.per_image_tiles(s.idx, s.tile_img, s.B, sc_flags_t)
-            d.idx_per_image = 1
+        d.N = s.N
+        if s.tile_img is not None:           # batch of independent edits: the slot's per-image lists, `cap` rows per edit
+            d.idx_per_image, d.N = 1, s.slot.cap
         d.idx = None if idx_t is None else idx_t.data_ptr()
-        d.N = n_per
         d.R = d.S = s.block
         d.scale = None if s.scale is None else s.scale.data_ptr()
         d.shift = None if s.shift is None else s.shift.data_ptr()
@@ -378,7 +413,7 @@ class CudaExecutor:
             d.residual, d.rC, d.res_c0 = None, 0, 0
         d.ksplit = s.ksplit
         d.flags = (CONV_PDL if s.pdl else 0) | (CONV_TC5 if s.tc5 else 0) | (CONV_EARLY_RELEASE if s.early_release else 0) | (s.early << 4)
-        if s.slot is not None and s.tile_img is None and s.B == 1 and s.slot.cap - s.slot.n >= 8:
+        if s.slot is not None and (s.slot.padded if s.tile_img is not None else (s.B == 1 and s.slot.cap - s.slot.n >= 8)):
             d.flags |= CONV_PADDED          # whole CTAs of padding exist (capacity headroom): let them exit at once
         d.n_aux = len(s.aux)
         keep = [wp, b32]
@@ -427,10 +462,7 @@ class CudaExecutor:
         b = None if rec.bias is None else rec.bias.detach().to(self.dtype).contiguous()
         aux = [ops.conv_aux(v, sc, sh, act) for (v, sc, sh, act) in rec.aux]
         out = rec.out.raw
-        tiles, per_image = rec.tiles, False
-        if rec.tiles is not None and rec.tile_img is not None:
-            tiles, _, _ = self.per_image_tiles(rec.tiles, rec.tile_img, rec.x.shape[0])
-            per_image = True
+        tiles, per_image = rec.tiles, rec.tiles is not None and rec.tile_img is not None      # (a batch: a slot's per-image lists)
 
         def run(_stream):
             ops.conv_in_nhwc(rec.x, w, b, out=out, aux=aux, tiles=tiles, tile_size=rec.tile_size, tiles_per_image=per_image)
@@ -492,6 +524,12 @@ class CudaExecutor:
 
     def writeback_supported(self) -> bool:
         """Can the step copy its output tiles into the module caches (sige_tile_writeback: sparse_update on the fused path)?"""
+        return True
+
+    def batch_slots_supported(self) -> bool:
+        """Can the launches of a batch of edits read its per-edit fixed-capacity lists (`IdxSlot` of a batch: each edit's rows end
+        in SIGE_TILE_NONE padding)?  Then a new batch is installed in place (`FusedStep.rebind`); without it a batch's launches get
+        the concatenated lists with a per-row image index, and a new batch recompiles."""
         return True
 
     def prepare_writeback(self, entries) -> Callable[[int], None]:
@@ -843,6 +881,8 @@ class Lowering:
         installed in place by `FusedStep.rebind`; CTAs made only of padding exit at once)."""
         self.tape, self.ex, self.dtype, self.dev = tape, executor, dtype, device
         self.headroom = float(headroom)
+        ok = getattr(executor, "batch_slots_supported", None)
+        self.batch_slots = ok is not None and ok()
         self.module_names = module_names or {}
         self.pdl, self.tc5, self.producer_preop, self.fuse_shortcut = pdl, tc5, producer_preop, fuse_shortcut
         self.fused_attention, self.sparse_stem, self.ksplit = fused_attention, sparse_stem, ksplit
@@ -1172,12 +1212,13 @@ class Lowering:
             pre = pre or Pre()
             pre.mod = ((st.gamma, st.gamma_c0), (st.beta, st.beta_c0), st.slope)
         timg = getattr(g, "tile_images", None)
-        if timg is None and int(g.active_indices.shape[0]) > 0 and not exact:
-            idx = self.slot(g).buf            # fixed capacity, padded with SIGE_TILE_NONE (see IdxSlot)
+        if int(g.active_indices.shape[0]) > 0 and not exact and (timg is None or self.batch_slots):
+            sl = self.slot(g)                 # fixed capacity, padded with SIGE_TILE_NONE (see IdxSlot)
+            idx, timg = sl.buf, sl.tile_img
         else:
             idx = g.active_indices.to(self.dev)
-        return (st.src.segs, pre, st.src.HW, idx, int(g.block_size[0]), int(g.offset[0]), None,
-                None if timg is None else timg.to(self.dev))
+            timg = None if timg is None else timg.to(self.dev)
+        return (st.src.segs, pre, st.src.HW, idx, int(g.block_size[0]), int(g.offset[0]), None, timg)
 
     def _chan_vec(self, t: Optional[torch.Tensor], f: Full) -> Optional[torch.Tensor]:
         """(1|B, C, 1, 1) broadcast operand -> fp32 [C] (or [B, C]) vector."""
@@ -1975,13 +2016,12 @@ class Lowering:
                 and int(sc.weight.shape[1]) % 64 == 0 and int(co.weight.shape[1]) % 64 == 0)
         name = self._module_name(node)
         if fuse:
-            flags = torch.isin(main_key, sc_key).to(torch.uint8).contiguous()
-            if mg.tile_images is None:          # fixed-capacity form (IdxSlot): padded entries carry flag 0
-                ms, ss = self.slot(mg), self.slot(sg)
-                fbuf = torch.zeros((ms.cap,), dtype=torch.uint8, device=self.dev)
-                fbuf[:ms.n] = flags
-                self.flag_recipes.append((fbuf, ms, off, ss, soff))
-                flags = fbuf
+            if mg.tile_images is None or self.batch_slots:
+                ms, ss = self.slot(mg), self.slot(sg)      # one flag per row of the main conv's list; padding rows carry flag 0
+                flags = _shortcut_flags(ms, off, ss, soff)[0].contiguous()
+                self.flag_recipes.append((flags, ms, off, ss, soff))
+            else:                                      # one flag per row of the concatenated lists of a batch
+                flags = torch.isin(main_key, sc_key).to(torch.uint8).contiguous()
             shortcut = ([b for b, _ in sc_full.segs], sc.weight, sc.bias, flags)
             n_fused = len(self.fused)
             self._tile_emit(node, co, dst, residual=skip, shortcut=shortcut, name=name)
@@ -2743,8 +2783,9 @@ class FusedStep:
     def rebind(self) -> bool:
         """Install the model's CURRENT tile lists (after a new ``set_masks``) into this compiled step without re-tracing or
         re-capturing: possible when every list fits the capacity it was built with and nothing outside the fused launches
-        holds a tile list (no eager operator-module fallbacks, no batch of edits).  Index buffers and shortcut flags are
-        rewritten in place and every cached buffer goes back to the original activations; the CUDA graph stays valid."""
+        holds a tile list (no eager operator-module fallbacks).  A batch of edits takes a new batch of the same size whose every
+        per-edit list fits.  Index buffers and shortcut flags are rewritten in place and every cached buffer goes back to the
+        original activations; the CUDA graph stays valid."""
         low = self.low
         if any(n.startswith(("sige.", "gather(")) for n in self.eager_nodes) or not low.slots:
             return False
@@ -2753,26 +2794,23 @@ class FusedStep:
         with torch.no_grad():
             for sl in low.slots.values():
                 sl.reload()
-            width = 1 << 16
             for (fbuf, ms, off, ss, soff) in low.flag_recipes:
-                mi, si = ms.buf[:ms.n].long(), ss.buf[:ss.n].long()
-                main_key = (mi[:, 0] + off) * width + (mi[:, 1] + off)
-                sc_key = (si[:, 0] + soff) * width + (si[:, 1] + soff)
-                if not bool(torch.isin(sc_key, main_key).all()):
+                flags, stray = _shortcut_flags(ms, off, ss, soff)
+                if bool(stray):
                     return False            # the shortcut's tiles left the main conv's grid: a different program
-                fbuf.zero_()
-                fbuf[:ms.n] = torch.isin(main_key, sc_key).to(torch.uint8)
+                fbuf.copy_(flags)
             for b in low.cached_bufs:
                 b.restore()
         return True
 
     def rebind_device(self, masks) -> bool:
-        """`rebind` without a host synchronisation (SURVEY section 8f-4): the mask reductions (`sige_reduce_mask`) run on the device
-        and their results go straight into the fixed-capacity tile lists the captured launches read — count and all stay in HBM,
-        nothing is copied back, so the call only ENQUEUES work (a handful of small kernels) and the next replay sees the new edit.
+        """`rebind` without a host synchronisation (SURVEY section 8f-4): the mask reductions (`sige_reduce_mask`, or one
+        `sige_reduce_mask_batched` per geometry for the [E, H, W] masks of a batch of edits) run on the device and their results
+        go straight into the fixed-capacity tile lists the captured launches read — counts and all stay in HBM, nothing is copied
+        back, so the call only ENQUEUES work (a handful of small kernels) and the next replay sees the new edit.
         Whether every list fit its capacity is recorded in `self.async_status` (device int32: bit 0 = a list overflowed and was
         truncated, bit 1 = a fused shortcut's tiles left the main conv's grid); `async_ok()` reads it (that one does synchronise).
-        Returns False — nothing changed — when this step cannot be re-bound in place at all."""
+        Returns False — nothing changed — when this step cannot be re-bound in place at all (a batch of another size included)."""
         from . import ops
 
         low = self.low
@@ -2781,7 +2819,8 @@ class FusedStep:
         for sl in low.slots.values():
             g = sl.gather
             m = masks.get(tuple(g.input_res)) if g.input_res is not None else None
-            if getattr(g, "tile_images", None) is not None or m is None or not m.is_cuda or m.dim() != 2:
+            want = 2 if sl.tile_img is None else 3
+            if m is None or not m.is_cuda or m.dim() != want or (want == 3 and int(m.shape[0]) != sl.E):
                 return False
         with torch.no_grad():
             if getattr(self, "async_status", None) is None:
@@ -2792,21 +2831,24 @@ class FusedStep:
                 g = sl.gather
                 res = tuple(g.input_res)
                 key = (res, tuple(g.block_size), tuple(g.block_stride), tuple(g.offset))
+                m = masks[res]
+                if sl.tile_img is not None:
+                    key = key + (sl.cap,)
+                    if key in memo:
+                        sl.buf.copy_(memo[key].buf)
+                        sl.n = memo[key].n
+                    else:
+                        sl.install_batched_device((m > 0.5) if m.is_floating_point() else (m != 0), self.async_status)
+                        memo[key] = sl
+                    continue
                 if key not in memo:
-                    m = masks[res]
                     m = (m > 0.5) if m.is_floating_point() else (m != 0)          # same binarisation as masks.reduce_mask
                     memo[key] = ops.reduce_mask_cuda_launch(m, g.block_size, g.block_stride, g.offset)
                 sl.install_device(*memo[key], self.async_status)
-            width = 1 << 16
             for (fbuf, ms, off, ss, soff) in low.flag_recipes:
-                mi, si = ms.buf.long(), ss.buf.long()
-                real_m, real_s = mi[:, 0] > ms.none, si[:, 0] > ss.none
-                main_key = torch.where(real_m, (mi[:, 0] + off) * width + (mi[:, 1] + off), torch.full_like(mi[:, 0], -1))
-                sc_key = torch.where(real_s, (si[:, 0] + soff) * width + (si[:, 1] + soff), torch.full_like(si[:, 0], -2))
-                eq = main_key.view(-1, 1) == sc_key.view(1, -1)       # (torch.isin synchronises; the lists are a few hundred entries)
-                fbuf.copy_((eq.any(1) & real_m).to(torch.uint8))
-                stray = (~eq.any(0) & real_s).any().to(torch.int32) * 2
-                self.async_status.bitwise_or_(stray.view(1))
+                flags, stray = _shortcut_flags(ms, off, ss, soff)
+                fbuf.copy_(flags)
+                self.async_status.bitwise_or_(stray * 2)
             for b in low.cached_bufs:
                 b.restore()
         return True

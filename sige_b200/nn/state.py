@@ -167,9 +167,10 @@ class SIGEModel(nn.Module):
         """`set_masks` for the NEXT edit without a host synchronisation (an extension; SURVEY section 8f-4): when a compiled fused
         step exists whose tile lists are fixed-capacity device buffers (`set_fused(headroom=...)` sizes them), the new pyramid is
         reduced on the device straight into those buffers (`FusedStep.rebind_device`) — the host never learns the tile counts, no
-        re-trace, no re-capture, only enqueued work.  Returns True when that happened; `masks_async_ok()` tells (with a sync,
-        whenever the caller can afford one) whether every list fit.  Otherwise — no compiled step yet, a batch of edits, eager
-        operator-module fallbacks in the step, CPU masks — falls back to the synchronous `set_masks` and returns False.
+        re-trace, no re-capture, only enqueued work.  A batch of edits ([E, H, W] masks, the same E as the compiled step) takes
+        one `sige_reduce_mask_batched` launch per geometry.  Returns True when that happened; `masks_async_ok()` tells (with a
+        sync, whenever the caller can afford one) whether every list fit.  Otherwise — no compiled step yet, a batch of another
+        size, eager operator-module fallbacks in the step, CPU masks — falls back to the synchronous `set_masks` and returns False.
         The operator modules' own `active_indices` are brought up to date lazily (by a synchronous `set_masks`) if a later call
         cannot use the compiled step."""
         d = self.__dict__

@@ -147,6 +147,35 @@ def reduce_mask_cuda_launch(mask: torch.Tensor, block_size, stride, padding):
     return out, count
 
 
+def reduce_mask_batched_cuda(masks: torch.Tensor, block_size, stride, padding, cap: int, out: Optional[torch.Tensor] = None,
+                             status: Optional[torch.Tensor] = None):
+    """bool/uint8 [E, H, W] CUDA masks of one geometry -> (int32 [E*cap, 2] per-image tile lists, row e*cap + i = tile i of
+    edit e, SIGE_TILE_NONE behind each edit's tiles; int32 [E] device counts; int32 [1] device status, bit 0 = some edit had
+    more than `cap` tiles and was truncated), as ONE launch of `sige_reduce_mask_batched`, without synchronising.  `out` and
+    `status` may be given (the status word is OR-ed into, not cleared)."""
+    _require_cuda(masks, out, status)
+    if masks.dim() != 3:
+        raise ValueError("reduce_mask_batched_cuda expects [E, H, W] masks")
+    E, H, W = masks.shape
+    m8 = (masks.to(torch.uint8) if masks.dtype != torch.uint8 else masks).contiguous()
+    if out is None:
+        out = torch.empty((E * cap, 2), dtype=torch.int32, device=masks.device)
+    if out.dtype != torch.int32 or tuple(out.shape) != (E * cap, 2) or not out.is_contiguous():
+        raise ValueError("reduce_mask_batched_cuda: out must be a contiguous int32 [E*cap, 2] tensor")
+    if status is None:
+        status = torch.zeros((1,), dtype=torch.int32, device=masks.device)
+    counts = torch.empty((E,), dtype=torch.int32, device=masks.device)
+    with torch.cuda.device(masks.device):
+        _cabi.check(
+            _cabi.lib().sige_reduce_mask_batched(m8.data_ptr(), E, H, W, block_size[0], block_size[1], stride[0], stride[1],
+                                                 padding[0], padding[1], out.data_ptr(), cap, counts.data_ptr(), status.data_ptr(),
+                                                 _stream(masks)),
+            "sige_reduce_mask_batched",
+        )
+    _bump()
+    return out, counts, status
+
+
 def reduce_mask_cuda(mask: torch.Tensor, block_size, stride, padding) -> torch.Tensor:
     """bool/uint8 [H,W] CUDA mask -> int32 [N,2] active tile origins, row-major, bit-exact."""
     out, count = reduce_mask_cuda_launch(mask, block_size, stride, padding)
