@@ -141,14 +141,17 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
 
     // ---------------- halo loader bookkeeping (fixed per thread) ----------------
     // unit q -> (pixel, 16B unit u); pixel -> (tile_local, y, x)
-    int ld_pix[LOADS];     // pixel index in the (logical) source image, or -1 (zero)
+    // (hh << 16) | ww of the pixel in the (logical) source image, unsigned so that rows 32768 and beyond stay valid: with
+    // H, W < 65536 every pixel packs to at most 0xfffefffe, so NO_PIX (zero fill: outside the image or no tile) is never one
+    constexpr unsigned NO_PIX = 0xffffffffu;
+    unsigned ld_pix[LOADS];
     int ld_img[LOADS];     // image (batch or stack row) index
     int ld_smem[LOADS];    // byte offset in the halo buffer, -1 = no work
     int ld_ab[LOADS];      // affine batch row
 #pragma unroll
     for (int k = 0; k < LOADS; ++k) {
         const int q = tid + k * NTHREADS;
-        ld_smem[k] = -1; ld_pix[k] = -1; ld_img[k] = 0; ld_ab[k] = 0;
+        ld_smem[k] = -1; ld_pix[k] = NO_PIX; ld_img[k] = 0; ld_ab[k] = 0;
         if (q < p.tpc * p.RS * 8) {
             const int pix = q >> 3, u = q & 7;
             const int tl = pix / p.RS, rem = pix - tl * p.RS;
@@ -162,7 +165,7 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
                     hh += __ldg(p.idx + 2 * n); ww += __ldg(p.idx + 2 * n + 1); img = b;
                 }
                 ld_img[k] = img; ld_ab[k] = b;
-                if (hh >= 0 && hh < p.H && ww >= 0 && ww < p.W) ld_pix[k] = (hh << 16) | ww;
+                if (hh >= 0 && hh < p.H && ww >= 0 && ww < p.W) ld_pix[k] = ((unsigned)hh << 16) | (unsigned)ww;
             }
         }
     }
@@ -178,8 +181,8 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
         for (int k = 0; k < LOADS; ++k) {
             ld_reg[k] = make_uint4(0, 0, 0, 0);
             const int u = (tid + k * NTHREADS) & 7;
-            if (ld_smem[k] >= 0 && ld_pix[k] >= 0 && cbase + u * 8 < p.Cin) {   // channels >= Cin: zero
-                const int hh = (ld_pix[k] >> 16) >> seg.up, ww = (ld_pix[k] & 0xffff) >> seg.up;
+            if (ld_smem[k] >= 0 && ld_pix[k] != NO_PIX && cbase + u * 8 < p.Cin) {   // channels >= Cin: zero
+                const int hh = (int)(ld_pix[k] >> 16) >> seg.up, ww = (int)(ld_pix[k] & 0xffff) >> seg.up;
                 const T *src = reinterpret_cast<const T *>(seg.ptr) +
                                (((long long)ld_img[k] * Hs + hh) * Ws + ww) * seg.pitch + cl + u * 8;
                 ld_reg[k] = __ldg(reinterpret_cast<const uint4 *>(src));
@@ -193,7 +196,7 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
             if (ld_smem[k] < 0) continue;
             uint4 v = ld_reg[k];
             const int ch = c * KC + ((tid + k * NTHREADS) & 7) * 8;
-            if (pre && ld_pix[k] >= 0 && ch < p.Cin) {   // scale / shift hold Cin entries: padding units stay zero
+            if (pre && ld_pix[k] != NO_PIX && ch < p.Cin) {   // scale / shift hold Cin entries: padding units stay zero
                 T *e = reinterpret_cast<T *>(&v);
                 float sc[8], sh[8];
 #pragma unroll

@@ -672,9 +672,9 @@ def output_pixels(case: Case, t, img, org, floor_division: bool = False):
     return ob[:, None, None].expand(shape), oh[:, :, None].expand(shape), ow[:, None, :].expand(shape), ok
 
 
-def reference(case: Case, floor_division: bool = False) -> List[kc.Expect]:
-    """`floor_division` computes the output origin with floor instead of C division: a deliberately wrong contract, for the
-    tests that show `check` tells the two apart."""
+def tile_values(case: Case, floor_division: bool = False):
+    """(v, bound, OB, OH, OW, ok): the launch's result before rounding, [NT, Ro, So, Cout] in float64, its per-element bound,
+    and where every output pixel goes (see output_pixels).  Only the tiles are gathered, so the buffers may be any size."""
     s = case.spec
     dev = case.w.device
     u = kc.ROUNDOFF[case.dtype]
@@ -695,7 +695,16 @@ def reference(case: Case, floor_division: bool = False) -> List[kc.Expect]:
         c0 = s.residual[1]
         r = case.residual[OB, OH.clamp(0, case.residual.shape[1] - 1), OW.clamp(0, case.residual.shape[2] - 1)][..., c0:c0 + s.Cout].double()
         v, mag = v + r, mag + r.abs()
-    bound = u * v.abs() + ACC * mag + pre + ABS
+    return v, u * v.abs() + ACC * mag + pre + ABS, OB, OH, OW, ok
+
+
+def reference(case: Case, floor_division: bool = False) -> List[kc.Expect]:
+    """`floor_division` computes the output origin with floor instead of C division: a deliberately wrong contract, for the
+    tests that show `check` tells the two apart."""
+    s = case.spec
+    dev = case.w.device
+    u = kc.ROUNDOFF[case.dtype]
+    v, bound, OB, OH, OW, ok = tile_values(case, floor_division)
     ob, oh, ow = OB[ok], OH[ok], OW[ok]
     shape = (s.NT, s.Ro, s.So) if s.dst_stack else (s.B, s.dH, s.dW)
     lin = (ob * shape[1] + oh) * shape[2] + ow
