@@ -477,6 +477,34 @@ typedef struct {
 int sige_tile_writeback(const sige_writeback_entry_t *entries, int n_entries, sige_stream_t stream);
 
 /* ------------------------------------------------------------------------- */
+/* cache load: the cached buffers of a fused step from the module caches     */
+/* ------------------------------------------------------------------------- */
+/* Entry e reads `src`, a cache [src_batch, C, H, W] (dense in src_layout, f32 / f16 / bf16), once, and writes
+ *   raw          NHWC [E, H, W, C] in `dtype`: the cache rounded to nearest (NULL: none);
+ *   view[k].dst  NHWC [E, H, W, C] in `dtype`: act(cache * scale[c] + shift[c]) for k < n_views, scale / shift fp32 [C] or NULL,
+ *                act SIGE_ACT_IDENTITY or SIGE_ACT_SWISH.
+ * A source of one image (src_batch == 1) is written to all E images; otherwise src_batch == E and image i goes to image i.
+ * Arithmetic in fp32, each operation rounded (no contraction): z * scale, then + shift, then swish as z * (1 / (1 + expf(-z))).
+ * C a multiple of 8, destinations 16-byte aligned and not overlapping any source.  At most SIGE_CACHE_LOAD_MAX_ENTRIES entries
+ * per call (the table travels in the launch's parameters); every entry is validated before any device call; n_entries == 0
+ * does nothing. */
+#define SIGE_CACHE_LOAD_MAX_ENTRIES 64
+typedef struct {
+    void *dst;
+    const float *scale, *shift;
+    int act;
+} sige_cache_view_t;
+typedef struct {
+    const void *src;
+    int src_dtype, src_layout, src_batch;
+    int C, H, W, E;
+    void *raw;
+    int n_views;
+    sige_cache_view_t view[2];
+} sige_cache_load_entry_t;
+int sige_cache_load(const sige_cache_load_entry_t *entries, int n_entries, int dtype, sige_stream_t stream);
+
+/* ------------------------------------------------------------------------- */
 /* diagnostics                                                                */
 /* ------------------------------------------------------------------------- */
 /* In-kernel timeline: while `buf` (device int64, 16 slots per CTA of the NEXT sige_tile_conv launch that takes the wgmma

@@ -85,6 +85,18 @@ class WritebackEntry(Structure):
 WRITEBACK_MAX_ENTRIES = 64
 
 
+class CacheView(Structure):
+    _fields_ = [("dst", c_void_p), ("scale", c_void_p), ("shift", c_void_p), ("act", c_int)]
+
+
+class CacheLoadEntry(Structure):
+    _fields_ = [("src", c_void_p), ("src_dtype", c_int), ("src_layout", c_int), ("src_batch", c_int), ("C", c_int), ("H", c_int), ("W", c_int),
+                ("E", c_int), ("raw", c_void_p), ("n_views", c_int), ("view", CacheView * 2)]
+
+
+CACHE_LOAD_MAX_ENTRIES = 64
+
+
 class TileConv(Structure):
     _fields_ = [
         ("dtype", c_int),
@@ -152,6 +164,7 @@ PROTOTYPES = {
     "sige_separable_conv_supported": (_I, [_I, _I, _I, _I]),
     "sige_separable_conv": (_I, [POINTER(SeparableConv), _P]),
     "sige_tile_writeback": (_I, [POINTER(WritebackEntry), _I, _P]),
+    "sige_cache_load": (_I, [POINTER(CacheLoadEntry), _I, _I, _P]),
     "sige_debug_set_trace": (_I, [_P]),
     "sige_debug_set_split_halo_buffers": (_I, [_I]),
 }

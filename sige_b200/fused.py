@@ -72,7 +72,11 @@ class Buf:
     def raw(self) -> torch.Tensor:
         if self._raw is None:
             if self.cached_init is not None:
-                self._raw = self.owner.clone_cache(self.cached_init, self.shape[0])
+                if self.owner.loads(self) and not self.owner.built:
+                    self._raw = self.owner.empty(*self.shape)        # filled when the lowering ends (Lowering.load_caches)
+                else:
+                    self._raw = self.owner.clone_cache(self.cached_init, self.shape[0])
+                self.owner.loader = None
             else:
                 self._raw = self.owner.empty(*self.shape)
         return self._raw
@@ -82,7 +86,8 @@ class Buf:
         return self._raw is not None
 
     def restore(self) -> None:
-        """Back to the cached original values (a new edit starts from them): raw copy and every transformed view."""
+        """Back to the cached original values (a new edit starts from them): raw copy and every transformed view.  The torch
+        restatement of `sige_cache_load`, for executors without it and caches it does not take."""
         if self.cached_init is None:
             return
         if self._raw is not None:
@@ -90,6 +95,15 @@ class Buf:
             self._raw.copy_(c if c.shape[0] == self.shape[0] else c.expand(self.shape[0], *c.shape[1:]))
         for (v, sc, sh, act) in self.view_inits:
             self.owner.init_view(v, self.cached_init, sc, sh, act)
+
+
+class Derived:
+    """A tensor the program reads that was derived from tensors taken from outside the tape (module caches, dense-pass
+    statistics, parameters): ``out = fn(*srcs)``.  `FusedStep.refresh` re-runs ``fn`` on the sources' current values and
+    copies the result into ``out``'s storage, which every launch keeps reading.  ``fn`` None: the sources are read as they are."""
+
+    def __init__(self, fn: Optional[Callable], srcs: Sequence, out):
+        self.fn, self.srcs, self.out = fn, tuple(srcs), out
 
 
 class ConvSpec:
@@ -113,6 +127,7 @@ class ConvSpec:
         self.weight: Optional[torch.Tensor] = None           # fp32 OIHW (after exact folds)
         self.bias: Optional[torch.Tensor] = None             # fp32 [Cout] or None
         self.weight_key = None                               # cache key of the packed form
+        self.refold = False                                  # weight / bias fold dense-pass statistics (`Lowering.derive`)
         self.out_row_scale: Optional[Tuple[int, float]] = None
         self.k = 1
         self.stride = 1
@@ -536,6 +551,36 @@ class CudaExecutor:
         """One `sige_tile_writeback` over (src buffer, module cache, tile list, off, stride, output tile) entries."""
         return self.ops.tile_writeback_launcher(entries)
 
+    def cache_load_supported(self, cache: Optional[torch.Tensor] = None) -> bool:
+        """Can `sige_cache_load` fill a cached buffer from this module cache (a dense 4-D f32 / f16 / bf16 CUDA tensor, C a
+        multiple of 8)?  Without an argument: does the executor have the launch at all?"""
+        return cache is None or (cache.is_cuda and cache.dim() == 4 and int(cache.shape[1]) % 8 == 0 and cache.dtype in self.ops._DTYPES
+                                 and self.ops.layout_of(cache) >= 0)
+
+    def prepare_cache_load(self, entries) -> Callable[[int], None]:
+        """One `sige_cache_load` over (module cache, raw buffer or None, [(view, scale, shift, act)]) entries."""
+        return self.ops.cache_load_launcher(entries, self.dtype)
+
+    def repack_conv(self, fc: FusedConv) -> None:
+        """Enqueue the packing of a prepared launch's `spec.weight` / `spec.bias`, recomputed in place (`FusedStep.refresh`),
+        into the packed buffers its descriptor points at."""
+        s = fc.spec
+        w, b = s.weight, s.bias
+        if s.out_row_scale is not None:
+            rows, f = s.out_row_scale
+            w = w.clone()
+            w[:rows] *= f
+            if b is not None:
+                b = b.clone()
+                b[:rows] *= f
+        pad_cin = (s.Cin + 63) // 64 * 64 if s.Cin % 64 else 0
+        if pad_cin > w.shape[1]:
+            w = F.pad(w, (0, 0, 0, 0, 0, pad_cin - w.shape[1]))
+        wp, b32 = fc.keep[0], fc.keep[1]
+        self.ops.pack_conv_weight(w.contiguous(), self.dtype, out=wp)
+        if b32 is not None and b32 is not b:
+            b32.copy_(b)
+
     def narrow_conv_supported(self, cin: int, cout: int, k: int, stride: int) -> bool:
         """Can sige_tile_conv run a conv whose single source has `cin` channels, a multiple of 8 but not of 64 (the mma.sync
         kernel with a partial last K chunk)?"""
@@ -863,6 +908,21 @@ def _is_const(o) -> bool:
     return isinstance(o, torch.Tensor) and not isinstance(o, LazyTensor)
 
 
+def _fold_affine(weight: torch.Tensor, bias: Optional[torch.Tensor], f_scale: Optional[torch.Tensor], f_shift: Optional[torch.Tensor],
+                 cin_pad: int) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """fp32 (weight, bias) of a 1x1 conv with the per-input-channel affine x * f_scale + f_shift folded in (exact: no halo),
+    `cin_pad` zero input channels appended."""
+    w32 = weight.detach().float()
+    b32 = None if bias is None else bias.detach().float()
+    if f_shift is not None:
+        b32 = (torch.zeros(w32.shape[0], device=w32.device) if b32 is None else b32) + (w32[:, :, 0, 0] @ f_shift.to(w32.device))
+    if f_scale is not None:
+        w32 = w32 * f_scale.to(w32.device).view(1, -1, 1, 1)
+    if cin_pad:
+        w32 = F.pad(w32, (0, 0, 0, 0, 0, cin_pad))
+    return w32, b32
+
+
 def _pair(v) -> Tuple[int, int]:
     if isinstance(v, (tuple, list)):
         return (int(v[0]), int(v[-1]))
@@ -913,6 +973,11 @@ class Lowering:
         self._alias_of: Dict[int, LazyTensor] = {}
         self.uses: Dict[int, int] = {}
         self._keepalive: List = []
+        self.derived: List[Derived] = []       # every tensor taken from outside the tape, and what the program made of it
+        self.eager_state: List[str] = []       # eager operator-module calls that read module caches themselves
+        self.cache_load = getattr(executor, "cache_load_supported", None)
+        self.loader = None                     # (prepared sige_cache_load, buffers it does not take) of load_caches
+        self.built = False
         for lt, t in zip(tape.inputs, static_inputs):
             self.env[id(lt)] = RealT(t)
         self._count_uses(outputs)
@@ -920,6 +985,9 @@ class Lowering:
             self._lower(node)
         self.outputs = lazy._tree_map(lambda o: self._output(o) if isinstance(o, LazyTensor) else o, outputs)
         self._post()
+        self.built = True
+        if self.cache_load is not None:
+            self.load_caches(torch.cuda.current_stream(self.dev).cuda_stream if self.dev.type == "cuda" else 0)
 
     # ------------------------------------------------------------------ helpers: memory
     def empty(self, b: int, c: int, h: int, w: int) -> torch.Tensor:
@@ -943,13 +1011,49 @@ class Lowering:
         self.cached_bufs.append(b)
         return b
 
+    def loads(self, buf: Buf) -> bool:
+        """Does the executor's one-launch cache load (`sige_cache_load`) fill this cached buffer?"""
+        return self.cache_load is not None and self.cache_load(buf.cached_init)
+
+    def load_caches(self, stream: int) -> None:
+        """Every cached buffer (raw copy and transformed views) from its cache, as the step starts a new edit: one
+        `sige_cache_load` for the caches the executor takes, the torch chain (`Buf.restore`) for the others."""
+        if self.loader is None:
+            entries, rest = [], []
+            for b in self.cached_bufs:
+                if not self.loads(b):
+                    rest.append(b)
+                elif b.has_raw or b.view_inits:
+                    entries.append((b.cached_init, b._raw, [(v, sc, sh, act) for (v, sc, sh, act) in b.view_inits]))
+            self.loader = (self.ex.prepare_cache_load(entries) if entries else None, rest)
+        run, rest = self.loader
+        if run is not None:
+            run(stream)
+        for b in rest:
+            b.restore()
+
+    def derive(self, fn: Optional[Callable], *srcs):
+        """``fn(*srcs)`` for a tensor the program reads that is made from tensors taken from outside the tape; ``fn`` None:
+        ``srcs`` are read as they are (nothing is returned).  Recorded (`Derived`) so that `FusedStep.refresh` can recompute it
+        into the same storage after a dense pass.  A result that aliases a source is copied: the program owns its storage."""
+        out = fn(*srcs) if fn is not None else None
+        ptrs = {t.untyped_storage().data_ptr() for t in srcs if isinstance(t, torch.Tensor)}
+
+        def own(t):
+            return t.clone() if isinstance(t, torch.Tensor) and t.untyped_storage().data_ptr() in ptrs else t
+
+        out = tuple(own(t) for t in out) if isinstance(out, tuple) else own(out)
+        self.derived.append(Derived(fn, srcs, out))
+        return out
+
     def vec(self, v: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
         """fp32 contiguous copy of a per-channel vector (kept alive; one copy per distinct source)."""
         if v is None:
             return None
         key = (v.data_ptr(), v.numel(), v._version, tuple(v.shape), tuple(v.stride()))
         if key not in self._vecs:
-            self._vecs[key] = (v.detach().to(self.dev).reshape(-1).float().contiguous(), v)
+            dev = self.dev
+            self._vecs[key] = (self.derive(lambda t: t.detach().to(dev).reshape(-1).float().contiguous(), v), v)
         return self._vecs[key][0]
 
     def all_tiles(self, h: int, w: int, off: int) -> torch.Tensor:
@@ -992,8 +1096,10 @@ class Lowering:
         sh = None if shift is None else shift.contiguous()
         v = self.empty(b, c, h, w)
         if buf.cached_init is not None:
-            self.init_view(v, buf.cached_init, sc, sh, act)
+            if self.built or not self.loads(buf):
+                self.init_view(v, buf.cached_init, sc, sh, act)
             buf.view_inits.append((v, sc, sh, act))
+            self.loader = None
         else:
             v.zero_()
         for pr in buf.producers:
@@ -1036,20 +1142,19 @@ class Lowering:
             B, n = segs[0][0].shape[0], int(idx.shape[0])
         s = ConvSpec()
         s.name = name
-        w32 = weight.detach().float()
-        b32 = None if bias is None else bias.detach().float()
         key = (weight, "w")
         if weight_fold is not None:        # exact fold of a per-input-channel affine (no activation) into a 1x1 conv
-            f_scale, f_shift = weight_fold
-            assert w32.shape[2] == 1 and w32.shape[3] == 1
-            if f_shift is not None:
-                b32 = (torch.zeros(w32.shape[0], device=w32.device) if b32 is None else b32) + (w32[:, :, 0, 0] @ f_shift.to(w32.device))
-            if f_scale is not None:
-                w32 = w32 * f_scale.to(w32.device).view(1, -1, 1, 1)
+            assert weight.shape[2] == 1 and weight.shape[3] == 1
+            w32, b32 = self.derive(_fold_affine, weight, bias, weight_fold[0], weight_fold[1], cin_pad)
             key = None                      # folded with per-image statistics: never cached
+            s.refold = True
             self._keepalive.append(weight_fold)
-        if cin_pad:
-            w32 = F.pad(w32, (0, 0, 0, 0, 0, cin_pad))
+        else:
+            self.derive(None, weight, bias)
+            w32 = weight.detach().float()
+            b32 = None if bias is None else bias.detach().float()
+            if cin_pad:
+                w32 = F.pad(w32, (0, 0, 0, 0, 0, cin_pad))
         s.weight, s.bias, s.weight_key = w32, b32, key
         s.epilogue_act = epilogue or "identity"
         s.k, s.stride, s.off, s.block = int(weight.shape[2]), stride, off, block
@@ -1110,6 +1215,7 @@ class Lowering:
             sc_bufs, sc_w, sc_b, sc_flags = shortcut
             for b_ in sc_bufs:
                 b_.readers.append((idx, block, 0, tile_img))      # the fused shortcut reads the centre 4x4 of conv2's 6x6 tiles
+            self.derive(None, sc_w, sc_b)
             s.shortcut = ([b_.raw for b_ in sc_bufs], sc_w.detach().float(), None if sc_b is None else sc_b.detach().float(), sc_flags)
             s.shortcut_key = (sc_w, "w")
         fc = FusedConv(s)
@@ -1226,7 +1332,7 @@ class Lowering:
             return None
         C = f.C
         if t.numel() == 1:
-            return self.vec(t).expand(C).contiguous()
+            return self.derive(lambda u: u.expand(C).contiguous(), self.vec(t))
         if t.dim() == 4 and t.shape[2] == 1 and t.shape[3] == 1 and t.shape[1] == C:
             if t.shape[0] == 1:
                 return self.vec(t)
@@ -1346,7 +1452,10 @@ class Lowering:
         idx = g.active_indices.to(self.dev)
         n = int(idx.shape[0])
         out = torch.empty((x.shape[0] * n, x.shape[1], g.block_size[0], g.block_size[1]), dtype=self.dtype, device=self.dev, memory_format=torch.channels_last)
-        ex, scale, shift = self.ex, st.scale, st.shift
+        dev = self.dev
+        ex = self.ex
+        # the gather's broadcast operands (dense-pass statistics, often): owned copies, so that a refresh rewrites what it reads
+        scale, shift = (None if v is None else self.derive(lambda u: u.detach().to(dev).clone(), v) for v in (st.scale, st.shift))
 
         def run(_stream):
             out.copy_(ex.gather(x, g.block_size, idx, scale, shift, g.activation_name, g.activation_first, up))
@@ -1398,6 +1507,18 @@ class Lowering:
         lazy._tree_map(bind, node.args)
         lazy._tree_map(bind, node.kwargs)
         is_module_call = isinstance(node.op, str)
+        consts: List[torch.Tensor] = []
+
+        def const(o):
+            if _is_const(o):
+                consts.append(o)
+            return o
+
+        lazy._tree_map(const, node.args)
+        lazy._tree_map(const, node.kwargs)
+        self.derive(None, *consts)       # (an eager node's arguments are frozen in the captured graph)
+        if is_module_call and node.name not in ("sige.conv", "sige.gather"):
+            self.eager_state.append(node.name)
         if not is_module_call and node.name in _VIEW_OPS and self._static_view(node, getters):
             return
         outs = []
@@ -1535,6 +1656,7 @@ class Lowering:
         """`src`: the conv's source when it is not x's symbolic value (a ModStack)."""
         if not (_is_const(weight) and (bias is None or _is_const(bias))) or weight.dim() != 4:
             return False
+        self.derive(None, weight, bias)
         k, s, p = _pair(weight.shape[2:]), _pair(stride), (_pair(padding) if not isinstance(padding, str) else None)
         if p is None or k[0] != k[1] or s[0] != s[1] or p[0] != p[1] or _pair(dilation) != (1, 1) or groups != 1:
             return False
@@ -1810,12 +1932,13 @@ class Lowering:
             return False
         if not (c.numel() == 1 or (c.dim() == 4 and tuple(c.shape) == (1, v.C, 1, 1))):
             return False
+        self.derive(None, c)            # (folded into the separable launch's weights by the executor)
         cv = self.vec(c).expand(v.C) if c.numel() == 1 else self.vec(c)
         if is_mul:
-            scale = cv if v.scale is None else v.scale * cv
-            shift = None if v.shift is None else v.shift * cv
+            scale = cv if v.scale is None else self.derive(torch.mul, v.scale, cv)
+            shift = None if v.shift is None else self.derive(torch.mul, v.shift, cv)
         else:
-            scale, shift = v.scale, (cv if v.shift is None else v.shift + cv)
+            scale, shift = v.scale, (cv if v.shift is None else self.derive(torch.add, v.shift, cv))
         self.env[id(node.outs[0])] = DWConv(v.src, v.c0, v.weight, v.bias, scale, shift, v.consts + (c,))
         return True
 
@@ -2062,10 +2185,10 @@ class Lowering:
         if pre.act:
             return None
         if is_mul:
-            pre.scale = cv if pre.scale is None else pre.scale * cv
-            pre.shift = None if pre.shift is None else pre.shift * cv
+            pre.scale = cv if pre.scale is None else self.derive(torch.mul, pre.scale, cv)
+            pre.shift = None if pre.shift is None else self.derive(torch.mul, pre.shift, cv)
         else:
-            pre.shift = cv if pre.shift is None else pre.shift + cv
+            pre.shift = cv if pre.shift is None else self.derive(torch.add, pre.shift, cv)
         return Full(list(v.segs), pre, None)
 
     def _h_mul(self, node: Node):
@@ -2291,6 +2414,7 @@ class Lowering:
             buf = f.single
         if buf is None or not (a["weight"] is None or _is_const(a["weight"])) or not (a["bias"] is None or _is_const(a["bias"])):
             return False
+        self.derive(None, a["weight"], a["bias"])
         self.env[id(node.outs[0])] = GNVal(buf, int(a["num_groups"]), a["weight"], a["bias"], float(a["eps"]))
         return True
 
@@ -2386,7 +2510,8 @@ class Lowering:
         def rt(t):
             if isinstance(t, LazyTensor):
                 return self.runtime_tensor(t)
-            c = t.detach().to(self.dev).to(self.dtype).contiguous()       # cached keys / values: constants of this step
+            dev, dt = self.dev, self.dtype
+            c = self.derive(lambda u: u.detach().to(dev).to(dt).contiguous(), t)       # cached keys / values: constants of this step
             self._keepalive.append(c)
             return c
 
@@ -2721,6 +2846,11 @@ class FusedStep:
         # sparse_update (the reference's apply step): whether this step can write its results back into the module caches
         self.sparse_update_reason: Optional[str] = self.low.sparse_update_reason
         self.sparse_update_supported = self.sparse_update_reason is None
+        # refresh (a new dense pass taken in place): why this step cannot (None: it can), and where the model keeps the current value
+        # of every tensor the program took from outside the tape
+        self.refresh_reason: Optional[str] = None
+        self.locations: Dict[int, Tuple] = {}
+        self._locate()
         self.graph = None
         self.epilogue_graph = None
         self.launches_per_step = 0
@@ -2731,8 +2861,11 @@ class FusedStep:
         self._run(self.steps)
         return self.outputs
 
+    def _stream(self) -> int:
+        return torch.cuda.current_stream(self.dev).cuda_stream if self.dev.type == "cuda" else 0
+
     def _run(self, steps) -> None:
-        stream = torch.cuda.current_stream(self.dev).cuda_stream if self.dev.type == "cuda" else 0
+        stream = self._stream()
         with torch.no_grad():
             for _kind, fn in steps:
                 fn(stream)
@@ -2799,8 +2932,7 @@ class FusedStep:
                 if bool(stray):
                     return False            # the shortcut's tiles left the main conv's grid: a different program
                 fbuf.copy_(flags)
-            for b in low.cached_bufs:
-                b.restore()
+            low.load_caches(self._stream())
         return True
 
     def rebind_device(self, masks) -> bool:
@@ -2849,8 +2981,129 @@ class FusedStep:
                 flags, stray = _shortcut_flags(ms, off, ss, soff)
                 fbuf.copy_(flags)
                 self.async_status.bitwise_or_(stray * 2)
-            for b in low.cached_bufs:
-                b.restore()
+            low.load_caches(self._stream())
+        return True
+
+    def _locate(self) -> None:
+        """Find, for every tensor the program took from outside the tape (module caches, dense-pass statistics, the sources of
+        `Lowering.derive`), the module attribute that holds it: a tensor, or a dict / list of tensors one level deep
+        (``scale1s[cache_id]``, ``original_outputs[cache_id]``), matched by storage.  Parameters and registered buffers need no
+        location.  Sets `refresh_reason` when the step cannot be refreshed."""
+        low, model = self.low, self.model
+        if low.eager_state:
+            self.refresh_reason = "eager operator modules read their caches inside the captured graph (%s)" % ", ".join(low.eager_state)
+            return
+        fixed = {t.untyped_storage().data_ptr() for t in list(model.parameters()) + list(model.buffers())}
+        made = {id(t) for d in low.derived for t in (d.out if isinstance(d.out, tuple) else (d.out,)) if isinstance(t, torch.Tensor)}
+        holders: Dict[int, List] = {}
+        for name, m in model.named_modules():
+            for attr, val in vars(m).items():
+                if attr in ("_parameters", "_buffers", "_modules"):
+                    continue
+                items = ([(None, val)] if isinstance(val, torch.Tensor) else list(val.items()) if isinstance(val, dict)
+                         else list(enumerate(val)) if isinstance(val, list) else [])
+                for key, t in items:
+                    if isinstance(t, torch.Tensor) and not isinstance(t, LazyTensor):
+                        holders.setdefault(t.untyped_storage().data_ptr(), []).append((name, attr, key, t))
+
+        def locate(t: torch.Tensor) -> Optional[str]:
+            if id(t) in self.locations:
+                return None
+            lo, hi = t.storage_offset(), t.storage_offset() + sum((n - 1) * st for n, st in zip(t.shape, t.stride()))
+            for (name, attr, key, base) in holders.get(t.untyped_storage().data_ptr(), []):
+                blo = base.storage_offset()
+                bhi = blo + sum((n - 1) * st for n, st in zip(base.shape, base.stride()))
+                if base.dtype == t.dtype and blo <= lo and hi <= bhi:
+                    self.locations[id(t)] = (name, attr, key, base.dtype, base.device, tuple(base.shape), tuple(base.stride()),
+                                             lo - blo, tuple(t.shape), tuple(t.stride()))
+                    return None
+            return "a %s tensor the forward read is held by no module" % (tuple(t.shape),)
+
+        reasons = [locate(b.cached_init) for b in low.cached_bufs]
+        for d in low.derived:
+            for t in d.srcs:
+                if not isinstance(t, torch.Tensor) or id(t) in made or t.untyped_storage().data_ptr() in fixed:
+                    continue
+                reasons.append("a %s tensor taken from outside the tape is read as it is" % (tuple(t.shape),) if d.fn is None else locate(t))
+        if any(f.spec.refold for f in low.fused) and getattr(self.ex, "repack_conv", None) is None:
+            reasons.append("the executor cannot re-pack folded weights")
+        self.refresh_reason = next((r for r in reasons if r is not None), None)
+        if self.refresh_reason is not None:
+            self.locations = {}
+        low._vecs.clear()         # (the memo of the lowering held the sources)
+
+    def _resolve(self) -> Tuple[Optional[Dict[int, torch.Tensor]], Optional[str]]:
+        """(the model's current tensor at every location, None) when each has the recorded dtype, device, shape, stride and view
+        geometry; else (None, why not)."""
+        mods = dict(self.model.named_modules())
+        new: Dict[int, torch.Tensor] = {}
+        for tid, (name, attr, key, dt, dev, shape, stride, rel, vshape, vstride) in self.locations.items():
+            m = mods.get(name)
+            c = None if m is None else vars(m).get(attr)
+            where = "%s.%s%s" % (name, attr, "" if key is None else "[%r]" % (key,))
+            try:
+                base = c if key is None else c[key]
+            except (KeyError, IndexError, TypeError):
+                return None, "%s is gone" % where
+            if not isinstance(base, torch.Tensor) or isinstance(base, LazyTensor):
+                return None, "%s is no longer a tensor" % where
+            if base.dtype != dt or base.device != dev or tuple(base.shape) != shape or tuple(base.stride()) != stride:
+                return None, "%s is now a %s %s tensor of shape %s, stride %s (the step was built for %s %s, %s, %s)" % (
+                    where, base.dtype, base.device, tuple(base.shape), tuple(base.stride()), dt, dev, shape, stride)
+            new[tid] = base.as_strided(vshape, vstride, base.storage_offset() + rel)
+        return new, None
+
+    def refresh(self, load: bool = True) -> bool:
+        """Take the model's CURRENT caches and dense-pass statistics (after a new ``full``-mode pass on an original image) into
+        this compiled step in place, without re-tracing or re-capturing: every recorded derivation is recomputed into the
+        storage the launches read (per-channel vectors, weights with statistics folded in, re-packed), every cached buffer is
+        reloaded from its new cache (one `sige_cache_load`) and the write-back targets the new caches.  Only enqueued work: no
+        host synchronisation.  The CUDA graph, descriptors and split-K plans stay as captured.  Returns False — nothing
+        changed — when `refresh_reason` is set, when a location no longer holds a tensor of the recorded geometry, or when the
+        step writes back and the new caches cannot take its tiles; the last two set `refresh_reason` too (the caller recompiles).
+        ``load`` False: the cached buffers are left for the caller to reload (`rebind` follows, which reloads them)."""
+        if self.refresh_reason is not None:
+            return False
+        new, why = self._resolve()
+        if new is None:
+            self.refresh_reason = why
+            return False
+        low = self.low
+        old = [b.cached_init for b in low.cached_bufs]
+        for b in low.cached_bufs:
+            b.cached_init = new[id(b.cached_init)]
+        refusal = low._sparse_update_refusal() if self.sparse_update_supported else None
+        if refusal is not None:
+            for b, c in zip(low.cached_bufs, old):
+                b.cached_init = c
+            self.refresh_reason = "the new caches cannot take the write-back: %s" % refusal
+            return False
+        with torch.no_grad():
+            live = set(new)
+            for d in low.derived:
+                if d.fn is None or not any(isinstance(t, torch.Tensor) and id(t) in live for t in d.srcs):
+                    continue
+                srcs = tuple(new.get(id(t), t) if isinstance(t, torch.Tensor) else t for t in d.srcs)
+                val = d.fn(*srcs)
+                outs, vals = (d.out, val) if isinstance(d.out, tuple) else ((d.out,), (val,))
+                for o, v in zip(outs, vals):
+                    if o is not None:
+                        o.copy_(v)
+                        live.add(id(o))
+                d.srcs = srcs
+            for fc in low.fused + low.epilogue_fused:
+                if fc.spec.refold and id(fc.spec.weight) in live:
+                    self.ex.repack_conv(fc)
+            low.loader = None
+            if load:
+                low.load_caches(self._stream())
+            if self.sparse_update_supported:
+                low.epilogue = [e for e in low.epilogue if e[0] != "writeback"]
+                entries = [(buf.raw, buf.cached_init, slot.buf, off, stride, ro) for (buf, slot, off, stride, ro) in low.cache_writers]
+                if entries:
+                    low.epilogue.append(("writeback", self.ex.prepare_writeback(entries)))
+                self.epilogue_graph = None
+        self.locations = {id(new[k]): loc for k, loc in self.locations.items()}
         return True
 
     def async_ok(self) -> bool:

@@ -253,12 +253,15 @@ class SIGEModel(nn.Module):
             self._sync_async_masks()          # lists installed on the device only: a different call signature needs the modules' lists
             key = (d.get("timestamp", 0), _cache_generation[0], d.get("_sige_cache_id", 0), sig)
         if key not in steps:
-            # same caches, same arguments, NEW masks: try to install the new tile lists into the compiled step in place
-            for k in [k for k in steps if k[1:] == key[1:] and k[0] != key[0]]:
+            # same cache id, same arguments, a NEW dense pass (new caches and statistics) and / or NEW masks: take them into the
+            # compiled step in place (FusedStep.refresh, then FusedStep.rebind)
+            for k in [k for k in steps if k[2:] == key[2:] and k[:2] != key[:2]]:
                 st = steps.pop(k)
-                if st is not None and st.rebind():
-                    steps[key] = st
-                    break
+                # (a rebind reloads the cached buffers itself: the refresh before it leaves them)
+                if st is None or (k[1] != key[1] and not st.refresh(load=k[0] == key[0])) or (k[0] != key[0] and not st.rebind()):
+                    continue
+                steps[key] = st
+                break
         if key not in steps:
             for k in [k for k in steps if k[0] != key[0] or k[1] != key[1]]:
                 del steps[k]           # older masks / older caches: their buffers are garbage now

@@ -333,14 +333,17 @@ def scatter_gather(x, y, bsize_h: int, bsize_w: int, active_indices, scatter_map
 # --------------------------------------------------------------------------------------
 # a3: tile convolution
 # --------------------------------------------------------------------------------------
-def pack_conv_weight(weight: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
+def pack_conv_weight(weight: torch.Tensor, dtype: torch.dtype, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """OIHW -> packed weights in `dtype` (f16/bf16) for the tensor-core kernels.  The returned tensor has the
     bookkeeping shape (kH*kW, Cout, Cin); its memory order is [tap][Cin/64][Cout][64] (contiguous slabs per
-    (tap, 64-channel chunk)) when Cin % 64 == 0."""
+    (tap, 64-channel chunk)) when Cin % 64 == 0.  `out`: an earlier result of the same shape and dtype, overwritten in place."""
     _require_cuda(weight)
     w = weight.detach().contiguous()
     Cout, Cin, kH, kW = w.shape
-    out = torch.empty((kH * kW, Cout, Cin), dtype=dtype, device=w.device)
+    if out is None:
+        out = torch.empty((kH * kW, Cout, Cin), dtype=dtype, device=w.device)
+    elif tuple(out.shape) != (kH * kW, Cout, Cin) or out.dtype != dtype or not out.is_contiguous() or out.device != w.device:
+        raise ValueError("pack_conv_weight: out must be a contiguous %s tensor of shape %s" % (dtype, (kH * kW, Cout, Cin)))
     with torch.cuda.device(w.device):
         _cabi.check(
             _cabi.lib().sige_pack_conv_weight(w.data_ptr(), _dt(w), Cout, Cin, kH, kW, out.data_ptr(), _DTYPES[dtype], _stream(w)),
@@ -807,6 +810,71 @@ def tile_writeback_launcher(entries):
             _bump()
 
     return run
+
+
+def cache_load_launcher(entries, dtype: torch.dtype):
+    """Prepare `sige_cache_load` over ``entries`` and return ``run(stream)``, which enqueues it (one launch per
+    SIGE_CACHE_LOAD_MAX_ENTRIES entries).  Entry = (src, raw, views): ``src`` a module cache [1 or E, C, H, W], NCHW- or
+    NHWC-dense, f32 / f16 / bf16; ``raw`` None or a channels-last [E, C, H, W] buffer in ``dtype`` that receives the cache;
+    ``views`` up to two (dst, scale, shift, act): dst like raw, receiving act(src * scale + shift) with fp32 [C] scale / shift
+    (or None) and act "identity" or "swish".  The tensors are not copied: the launch reads them as they are when it runs."""
+    from ._cabi import CACHE_LOAD_MAX_ENTRIES, CacheLoadEntry
+
+    if dtype not in (torch.float16, torch.bfloat16):
+        raise ValueError("cache_load: the destinations are f16 or bf16, not %s" % dtype)
+    rows, keep, dev = [], [], None
+    for k, (src, raw, views) in enumerate(entries):
+        views = list(views)
+        _require_cuda(src, raw, *[t for v in views for t in v[:3]])
+        lo = layout_of(src) if src.dim() == 4 else -1
+        if lo < 0 or src.dtype not in _DTYPES:
+            raise ValueError("cache_load: entry %d: src must be an NCHW- or NHWC-dense 4-D f32 / f16 / bf16 tensor" % k)
+        dsts = ([raw] if raw is not None else []) + [v[0] for v in views]
+        if not dsts or len(views) > 2:
+            raise ValueError("cache_load: entry %d: a raw destination and / or one or two views" % k)
+        E, C, H, W = (int(d) for d in dsts[0].shape)
+        if int(src.shape[0]) not in (1, E) or tuple(src.shape[1:]) != (C, H, W) or C % 8:
+            raise ValueError("cache_load: entry %d: src %s does not match destinations %s (C a multiple of 8)" % (k, tuple(src.shape), tuple(dsts[0].shape)))
+        for d in dsts:
+            if tuple(d.shape) != (E, C, H, W) or d.dtype != dtype or not d.is_contiguous(memory_format=torch.channels_last) or d.data_ptr() % 16:
+                raise ValueError("cache_load: entry %d: destinations must be channels-last %s [E, C, H, W] buffers, 16-byte aligned" % (k, dtype))
+        e = CacheLoadEntry()
+        e.src, e.src_dtype, e.src_layout, e.src_batch = src.data_ptr(), _dt(src), lo, int(src.shape[0])
+        e.C, e.H, e.W, e.E = C, H, W, E
+        e.raw = None if raw is None else raw.data_ptr()
+        e.n_views = len(views)
+        for i, (dst, sc, sh, act) in enumerate(views):
+            for v in (sc, sh):
+                if v is not None and (v.dtype != torch.float32 or v.numel() != C or not v.is_contiguous()):
+                    raise ValueError("cache_load: entry %d: view %d: scale / shift must be contiguous fp32 [C]" % (k, i))
+            ev = e.view[i]
+            ev.dst, ev.act = dst.data_ptr(), _act(act)
+            ev.scale = None if sc is None else sc.data_ptr()
+            ev.shift = None if sh is None else sh.data_ptr()
+        dev = dev or src.device
+        rows.append(e)
+        keep.append((src, raw, views))
+    tables = []
+    for s in range(0, len(rows), CACHE_LOAD_MAX_ENTRIES):
+        part = rows[s:s + CACHE_LOAD_MAX_ENTRIES]
+        tables.append(((CacheLoadEntry * len(part))(*part), len(part)))
+    dt = _DTYPES[dtype]
+
+    def run(stream: int) -> None:
+        _ = keep
+        for table, n in tables:
+            with torch.cuda.device(dev):
+                _cabi.check(_cabi.lib().sige_cache_load(table, n, dt, stream), "sige_cache_load")
+            _bump()
+
+    return run
+
+
+def cache_load(entries, dtype: torch.dtype) -> None:
+    """`cache_load_launcher(entries, dtype)` enqueued once on the current stream."""
+    entries = list(entries)
+    if entries:
+        cache_load_launcher(entries, dtype)(_stream(entries[0][0]))
 
 
 def tile_writeback(entries) -> None:
