@@ -92,7 +92,8 @@ int sige_reduce_mask(const uint8_t *mask, int H, int W, int R, int S, int stride
 int sige_reduce_mask_batched(const uint8_t *masks, int E, int H, int W, int R, int S, int strideH,
                              int strideW, int padH, int padW, int32_t *idx_out, int cap,
                              int32_t *counts_out, int32_t *status, sige_stream_t stream);
-/* host helper: number of candidate tiles (upper bound for `capacity`) */
+/* host helper: number of candidate tiles (upper bound for `capacity`).  A geometry of 2^31 or more candidates, which
+ * sige_reduce_mask and sige_reduce_mask_batched refuse, returns -1 and sets the error. */
 int sige_reduce_mask_capacity(int H, int W, int R, int S, int strideH, int strideW, int padH,
                               int padW);
 
@@ -364,7 +365,8 @@ int sige_conv_in_nhwc_tiles(const void *x, const void *w, const void *bias, void
                             int H, int W, int Cin, int Cout, const int32_t *idx, int n_tiles, int R, int S,
                             int idx_per_image, int n_aux, const sige_conv_aux_t *aux, sige_stream_t stream);
 /* GroupNorm statistics folded to per-channel fp32 (scale, shift) [B, C]: GroupNorm(x) == x*scale + shift.
- * Deterministic two-stage reduction; `workspace` holds sige_group_norm_fold_workspace(B, C) floats. */
+ * Deterministic two-stage reduction; `workspace` holds sige_group_norm_fold_workspace(B, C) floats, which is -1 (and the
+ * error is set) when that count exceeds 2^31 - 1.  H * W < 2^31. */
 int sige_group_norm_fold_workspace(int B, int C);
 int sige_group_norm_fold(const void *x, int dtype, int B, int H, int W, int C, int groups, float eps,
                          const void *gamma, const void *beta, float *scale, float *shift,

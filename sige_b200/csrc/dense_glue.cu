@@ -62,7 +62,7 @@ __global__ void __launch_bounds__(256) conv_in_kernel(const T *__restrict__ x, c
     __syncthreads();
     pdl_acquire();
     const int WQ = W / 4;
-    const int total = B * H * WQ * OV;      // < 2^31 (checked on the host)
+    const int total = B * H * WQ * OV;      // < 2^29 (checked on the host), so the int loop index below cannot wrap
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
         const int ov = i % OV;
         int q = i / OV;
@@ -163,15 +163,16 @@ __global__ void __launch_bounds__(256) conv_in_tiles_kernel(const T *__restrict_
     pdl_release();
     __syncthreads();
     pdl_acquire();
-    const int total = NT * R * S * OV;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-        const int ov = i % OV;
-        int q = i / OV;
+    const int total = NT * R * S * OV;      // < 2^31 - 1 (checked on the host)
+    // long long: the last stride past `total` can pass 2^31
+    for (long long i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
+        const int ov = (int)i % OV;
+        int q = (int)i / OV;
         const int xx = q % S; q /= S;
         const int yy = q % R;
         const int t = q / R;
         const int b = t / n_tiles, tt = idx_per_image ? t : t - b * n_tiles;      // per-image lists: row b*n_tiles + i
-        const int hh = __ldg(idx + 2 * tt) + yy, ww = __ldg(idx + 2 * tt + 1) + xx;
+        const int hh = __ldg(idx + 2LL * tt) + yy, ww = __ldg(idx + 2LL * tt + 1) + xx;
         if (hh < 0 || hh >= H || ww < 0 || ww >= W) continue;
         float acc[8];
 #pragma unroll
@@ -225,8 +226,9 @@ __global__ void __launch_bounds__(256) gn_partial_kernel(const T *__restrict__ x
     const int slots = blockDim.x / CV;
     const int cv = threadIdx.x % CV, slot = threadIdx.x / CV;
     const int b = blockIdx.y;
-    const int per = (HW + nblk - 1) / nblk;
-    const int p0 = blockIdx.x * per, p1 = min(HW, p0 + per);
+    // HW < 2^31 (checked on the host); the pixel positions are long long because the last CTA's range and loop steps may pass it
+    const int per = HW / nblk + (HW % nblk != 0);
+    const long long p0 = (long long)blockIdx.x * per, p1 = min((long long)HW, p0 + per);
     pdl_release();
     pdl_acquire();
     float s[8], q[8];
@@ -234,11 +236,11 @@ __global__ void __launch_bounds__(256) gn_partial_kernel(const T *__restrict__ x
     for (int z = 0; z < 8; ++z) { s[z] = 0.f; q[z] = 0.f; }
     if (slot < slots) {
         constexpr int GB = 8;     // loads in flight per thread (same summation order as a plain loop)
-        for (int pb = p0 + slot; pb < p1; pb += slots * GB) {
+        for (long long pb = p0 + slot; pb < p1; pb += slots * GB) {
             uint4 v[GB];
 #pragma unroll
             for (int j = 0; j < GB; ++j) {
-                const int p = pb + j * slots;
+                const long long p = pb + j * slots;
                 v[j] = make_uint4(0, 0, 0, 0);
                 if (p < p1) v[j] = __ldg(reinterpret_cast<const uint4 *>(x + ((long long)b * HW + p) * C + cv * 8));
             }
@@ -505,8 +507,8 @@ int sige_conv_in_nhwc_tiles(const void *x, const void *w, const void *bias, void
     if (n_tiles == 0) return 0;
     const size_t smem = sizeof(float) * ((size_t)(Cout / 8) * conv_in_pitch(Cin) + Cout);
     SIGE_REQUIRE(smem <= 48 * 1024, "sige_conv_in_nhwc_tiles: weights do not fit in shared memory");
-    const int NT = B * n_tiles;
-    const long long total = (long long)NT * R * S * (Cout / 8);
+    const long long NT = (long long)B * n_tiles;
+    const long long total = NT * R * S * (Cout / 8);
     SIGE_REQUIRE(total < 2147483647LL && (long long)B * H * W * Cout < 2147483647LL * 8, "sige_conv_in_nhwc_tiles: tensor too large");
     const long long want_blocks = (total + 255) / 256;
     const int grid = (int)(want_blocks < 4LL * sm_count() ? want_blocks : 4LL * sm_count());
@@ -519,8 +521,8 @@ int sige_conv_in_nhwc_tiles(const void *x, const void *w, const void *bias, void
         ia[i] = InAux{aux[i].ptr, aux[i].scale, aux[i].shift, aux[i].act};
     }
     switch (dtype) {
-        case SIGE_F16: (void)launch_ex(conv_in_tiles_kernel<__half>, dim3(grid), dim3(256), smem, st, true, dim3(1, 1, 1), (const __half *)x, (const __half *)w, (const __half *)bias, (__half *)out, H, W, Cin, Cout, idx, n_tiles, NT, R, S, idx_per_image, n_aux, ia[0], ia[1]); break;
-        case SIGE_BF16: (void)launch_ex(conv_in_tiles_kernel<__nv_bfloat16>, dim3(grid), dim3(256), smem, st, true, dim3(1, 1, 1), (const __nv_bfloat16 *)x, (const __nv_bfloat16 *)w, (const __nv_bfloat16 *)bias, (__nv_bfloat16 *)out, H, W, Cin, Cout, idx, n_tiles, NT, R, S, idx_per_image, n_aux, ia[0], ia[1]); break;
+        case SIGE_F16: (void)launch_ex(conv_in_tiles_kernel<__half>, dim3(grid), dim3(256), smem, st, true, dim3(1, 1, 1), (const __half *)x, (const __half *)w, (const __half *)bias, (__half *)out, H, W, Cin, Cout, idx, n_tiles, (int)NT, R, S, idx_per_image, n_aux, ia[0], ia[1]); break;
+        case SIGE_BF16: (void)launch_ex(conv_in_tiles_kernel<__nv_bfloat16>, dim3(grid), dim3(256), smem, st, true, dim3(1, 1, 1), (const __nv_bfloat16 *)x, (const __nv_bfloat16 *)w, (const __nv_bfloat16 *)bias, (__nv_bfloat16 *)out, H, W, Cin, Cout, idx, n_tiles, (int)NT, R, S, idx_per_image, n_aux, ia[0], ia[1]); break;
         default: set_error("sige_conv_in_nhwc_tiles: dtype must be f16/bf16"); return 1;
     }
     return check_launch("sige_conv_in_nhwc_tiles");
@@ -530,16 +532,24 @@ int sige_conv_in_nhwc_tiles(const void *x, const void *w, const void *bias, void
 // the same device)
 static int gn_partial_blocks() { return 2 * sm_count(); }
 
-int sige_group_norm_fold_workspace(int B, int C) { return B * gn_partial_blocks() * C * 2; }
+static long long gn_workspace_floats(int B, int nblk, int C) { return (long long)B * nblk * C * 2; }
+
+int sige_group_norm_fold_workspace(int B, int C) {
+    const long long n = gn_workspace_floats(B, gn_partial_blocks(), C);
+    if (n <= 2147483647LL) return (int)n;
+    set_error("sige_group_norm_fold_workspace: %lld floats exceed 2^31 - 1", n);
+    return -1;
+}
 
 int sige_group_norm_fold(const void *x, int dtype, int B, int H, int W, int C, int groups, float eps, const void *gamma, const void *beta,
                          float *scale, float *shift, float *workspace, int workspace_floats, sige_stream_t stream) {
     SIGE_REQUIRE(x && scale && shift && workspace, "sige_group_norm_fold: null pointer");
     SIGE_REQUIRE(B > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && C <= 1024 && groups > 0 && C % groups == 0, "sige_group_norm_fold: bad shape (C %% 8, C <= 1024)");
     SIGE_REQUIRE(((uintptr_t)x & 15) == 0, "sige_group_norm_fold: input not 16-byte aligned");
+    SIGE_REQUIRE((long long)H * W <= 2147483647LL, "sige_group_norm_fold: image too large (H * W = %lld, the limit is 2^31 - 1)", (long long)H * W);
     const int HW = H * W;
     int nblk = min(gn_partial_blocks(), max(1, HW / 64));
-    SIGE_REQUIRE(workspace_floats >= B * nblk * C * 2, "sige_group_norm_fold: workspace too small (%d floats, need %d)", workspace_floats, B * nblk * C * 2);
+    SIGE_REQUIRE(workspace_floats >= gn_workspace_floats(B, nblk, C), "sige_group_norm_fold: workspace too small (%d floats, need %lld)", workspace_floats, gn_workspace_floats(B, nblk, C));
     const int CV = C / 8;
     SIGE_REQUIRE(CV <= 256, "sige_group_norm_fold: too many channels");
     const int slots = 256 / CV;

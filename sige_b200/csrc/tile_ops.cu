@@ -180,15 +180,15 @@ __global__ void calibrate_kernel(long long total, TileGeom g, const T *__restric
 // ----------------------------------------------------------------------------
 // scatter map  (reference sige/cuda/scatter_gather_kernel.cu:69-98)
 // ----------------------------------------------------------------------------
-__global__ void scatter_map_kernel(int total, int H, int W, int Ro, int So, int offH, int offW, int strideH,
+__global__ void scatter_map_kernel(long long total, int H, int W, int Ro, int So, int offH, int offW, int strideH,
                                    int strideW, int32_t *__restrict__ map, const int32_t *__restrict__ idx) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
+    const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (i >= total) return;
-    int t = i;
+    long long t = i;
     const int s = t % So; t /= So;
     const int r = t % Ro; t /= Ro;
-    const int n = t;
-    const int hh = (offH + idx[2 * n]) / strideH + r, ww = (offW + idx[2 * n + 1]) / strideW + s;
+    const int n = (int)t;                       // < N
+    const int hh = (offH + idx[2LL * n]) / strideH + r, ww = (offW + idx[2LL * n + 1]) / strideW + s;
     if (hh < 0 || hh >= H || ww < 0 || ww >= W) return;
     int32_t *m = map + 3 * ((long long)hh * W + ww);
     m[0] = n; m[1] = r; m[2] = s;
@@ -289,12 +289,13 @@ __device__ int reduce_mask_cta(const uint8_t *__restrict__ mask, int H, int W, i
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
     if (threadIdx.x == 0) base_s = 0;
     __syncthreads();
-    const int total = nI * nJ;
-    for (int start = 0; start < total; start += blockDim.x) {
-        const int cand = start + threadIdx.x;
+    const int total = nI * nJ;                  // < 2^31 (checked on the host)
+    // unsigned: the step past the last chunk may reach 2^31
+    for (unsigned start = 0; start < (unsigned)total; start += blockDim.x) {
+        const unsigned cand = start + threadIdx.x;
         bool any = false;
         int i = 0, j = 0;
-        if (cand < total) {
+        if (cand < (unsigned)total) {
             i = cand / nJ; j = cand % nJ;
             const int h0 = max(i * strideH - padH, 0), h1 = min(i * strideH - padH + R, H);
             const int w0 = max(j * strideW - padW, 0), w1 = min(j * strideW - padW + S, W);
@@ -315,8 +316,8 @@ __device__ int reduce_mask_cta(const uint8_t *__restrict__ mask, int H, int W, i
         if (any) {
             const int pos = base + before + __popc(bal & ((1u << lane) - 1u));
             if (pos < capacity) {
-                out[2 * pos] = strideH * i - padH;
-                out[2 * pos + 1] = strideW * j - padW;
+                out[2LL * pos] = strideH * i - padH;
+                out[2LL * pos + 1] = strideW * j - padW;
             }
         }
         __syncthreads();
@@ -341,7 +342,7 @@ __global__ void reduce_mask_batched_kernel(const uint8_t *__restrict__ masks, in
     const int e = blockIdx.x;
     int32_t *seg = out + 2LL * e * cap;
     const int total = reduce_mask_cta(masks + (long long)e * H * W, H, W, R, S, strideH, strideW, padH, padW, nI, nJ, seg, cap);
-    for (int i = 2 * min(total, cap) + threadIdx.x; i < 2 * cap; i += blockDim.x) seg[i] = SIGE_TILE_NONE;
+    for (long long i = 2LL * min(total, cap) + threadIdx.x; i < 2LL * cap; i += blockDim.x) seg[i] = SIGE_TILE_NONE;
     if (threadIdx.x == 0) {
         counts[e] = total;
         if (total > cap) atomicOr(status, 1);
@@ -461,6 +462,16 @@ static size_t dtype_size(int dtype) { return dtype == SIGE_F32 ? 4 : 2; }
         default: ::sige::set_error("unsupported dtype %d", dtype); return 1; \
     }
 
+// Candidate tiles nI x nJ of the pooled grid: padded extent (H + pad + R), window R, floor mode -> (H + pad)/stride + 1
+// (reference sige/utils.py:27-28).  reduce_mask_cta counts them, and the tiles it finds, in an int, so 2^31 or more are refused:
+// -1 with the error set.
+static long long reduce_mask_candidates(const char *what, int H, int W, int strideH, int strideW, int padH, int padW) {
+    const long long n = (((long long)H + padH) / strideH + 1) * (((long long)W + padW) / strideW + 1);
+    if (n < 2147483648LL) return n;
+    set_error("%s: too many candidate tiles (%lld, the limit is 2^31 - 1)", what, n);
+    return -1;
+}
+
 }  // namespace sige
 
 using namespace sige;
@@ -470,8 +481,7 @@ extern "C" {
 int sige_reduce_mask_capacity(int H, int W, int R, int S, int strideH, int strideW, int padH, int padW) {
     (void)R; (void)S;
     if (H <= 0 || W <= 0 || strideH <= 0 || strideW <= 0) return 0;
-    // padded extent (H + pad + R), window R, floor mode -> (H + pad)/stride + 1   (reference sige/utils.py:27-28)
-    return ((H + padH) / strideH + 1) * ((W + padW) / strideW + 1);
+    return (int)reduce_mask_candidates("sige_reduce_mask_capacity", H, W, strideH, strideW, padH, padW);
 }
 
 int sige_reduce_mask(const uint8_t *mask, int H, int W, int R, int S, int strideH, int strideW, int padH, int padW,
@@ -480,8 +490,9 @@ int sige_reduce_mask(const uint8_t *mask, int H, int W, int R, int S, int stride
     SIGE_REQUIRE(H > 0 && W > 0 && R > 0 && S > 0 && strideH > 0 && strideW > 0 && padH >= 0 && padW >= 0,
                  "sige_reduce_mask: bad geometry H=%d W=%d R=%d S=%d stride=(%d,%d) pad=(%d,%d)", H, W, R, S,
                  strideH, strideW, padH, padW);
+    if (reduce_mask_candidates("sige_reduce_mask", H, W, strideH, strideW, padH, padW) < 0) return 1;
     SIGE_REQUIRE(capacity == 0 || idx_out, "sige_reduce_mask: idx_out is null with capacity %d", capacity);
-    const int nI = (H + padH) / strideH + 1, nJ = (W + padW) / strideW + 1;
+    const int nI = (int)(((long long)H + padH) / strideH + 1), nJ = (int)(((long long)W + padW) / strideW + 1);
     reduce_mask_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(mask, H, W, R, S, strideH, strideW, padH, padW, nI, nJ,
                                                              idx_out, capacity, count_out);
     return check_launch("sige_reduce_mask");
@@ -496,8 +507,9 @@ int sige_reduce_mask_batched(const uint8_t *masks, int E, int H, int W, int R, i
     SIGE_REQUIRE(H > 0 && W > 0 && R > 0 && S > 0 && strideH > 0 && strideW > 0 && padH >= 0 && padW >= 0,
                  "sige_reduce_mask_batched: bad geometry H=%d W=%d R=%d S=%d stride=(%d,%d) pad=(%d,%d)", H, W, R, S,
                  strideH, strideW, padH, padW);
+    if (reduce_mask_candidates("sige_reduce_mask_batched", H, W, strideH, strideW, padH, padW) < 0) return 1;
     SIGE_REQUIRE(cap == 0 || idx_out, "sige_reduce_mask_batched: idx_out is null with cap %d", cap);
-    const int nI = (H + padH) / strideH + 1, nJ = (W + padW) / strideW + 1;
+    const int nI = (int)(((long long)H + padH) / strideH + 1), nJ = (int)(((long long)W + padW) / strideW + 1);
     reduce_mask_batched_kernel<<<E, 1024, 0, (cudaStream_t)stream>>>(masks, H, W, R, S, strideH, strideW, padH, padW, nI,
                                                                      nJ, idx_out, cap, counts_out, status);
     return check_launch("sige_reduce_mask_batched");
@@ -575,12 +587,13 @@ int sige_get_scatter_map(int H, int W, int R, int S, int kH, int kW, int offH, i
     SIGE_REQUIRE(H > 0 && W > 0 && R >= kH && S >= kW && kH > 0 && kW > 0 && strideH > 0 && strideW > 0 && N >= 0,
                  "sige_get_scatter_map: bad geometry");
     SIGE_REQUIRE(map_out, "sige_get_scatter_map: null output");
+    const int Ro = (R - kH) / strideH + 1, So = (S - kW) / strideW + 1;
+    const long long total = (long long)N * Ro * So;
+    SIGE_REQUIRE(total <= 2147483647LL * kThreads, "sige_get_scatter_map: grid too large (%lld tile pixels)", total);
+    SIGE_REQUIRE(N == 0 || idx, "sige_get_scatter_map: null index list");
     cudaError_t e = cudaMemsetAsync(map_out, 0xFF, sizeof(int32_t) * 3 * (size_t)H * W, (cudaStream_t)stream);
     SIGE_REQUIRE(e == cudaSuccess, "sige_get_scatter_map: memset failed: %s", cudaGetErrorString(e));
     if (N == 0) return 0;
-    SIGE_REQUIRE(idx, "sige_get_scatter_map: null index list");
-    const int Ro = (R - kH) / strideH + 1, So = (S - kW) / strideW + 1;
-    const int total = N * Ro * So;
     scatter_map_kernel<<<ceil_div(total, kThreads), kThreads, 0, (cudaStream_t)stream>>>(
         total, H, W, Ro, So, offH, offW, strideH, strideW, map_out, idx);
     return check_launch("sige_get_scatter_map");

@@ -494,7 +494,7 @@ class CudaExecutor:
         b = None if bias is None else bias.detach().to(dt).contiguous()
         scale = torch.empty((B, C), dtype=torch.float32, device=x.device)
         shift = torch.empty((B, C), dtype=torch.float32, device=x.device)
-        ws = torch.empty((ops._cabi.lib().sige_group_norm_fold_workspace(B, C),), dtype=torch.float32, device=x.device)
+        ws = torch.empty((ops.group_norm_fold_workspace(B, C),), dtype=torch.float32, device=x.device)
 
         def run(_stream):
             ops.group_norm_fold(x, groups, eps, g, bt, scale=scale, shift=shift, workspace=ws)

@@ -132,9 +132,10 @@ def reduce_mask_cuda_launch(mask: torch.Tensor, block_size, stride, padding):
     """Enqueue the ordered-compaction kernel; returns (idx buffer [capacity, 2], device count [1]) WITHOUT synchronising."""
     _require_cuda(mask)
     H, W = mask.shape
+    cap = _cabi.lib().sige_reduce_mask_capacity(H, W, block_size[0], block_size[1], stride[0], stride[1], padding[0], padding[1])
+    _cabi.check(cap < 0, "sige_reduce_mask_capacity")
     m8 = mask.to(torch.uint8) if mask.dtype != torch.uint8 else mask
     m8 = m8.contiguous()
-    cap = _cabi.lib().sige_reduce_mask_capacity(H, W, block_size[0], block_size[1], stride[0], stride[1], padding[0], padding[1])
     out = torch.empty((cap, 2), dtype=torch.int32, device=mask.device)
     count = torch.empty((1,), dtype=torch.int32, device=mask.device)
     with torch.cuda.device(mask.device):
@@ -529,6 +530,13 @@ def conv_in_nhwc(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Ten
     return out
 
 
+def group_norm_fold_workspace(B: int, C: int) -> int:
+    """Floats of workspace sige_group_norm_fold needs for B images of C channels on the current device."""
+    need = _cabi.lib().sige_group_norm_fold_workspace(B, C)
+    _cabi.check(need < 0, "sige_group_norm_fold_workspace")
+    return need
+
+
 def group_norm_fold(x: torch.Tensor, groups: int, eps: float, gamma: Optional[torch.Tensor], beta: Optional[torch.Tensor],
                     scale: Optional[torch.Tensor] = None, shift: Optional[torch.Tensor] = None, workspace: Optional[torch.Tensor] = None):
     """(scale, shift) fp32 [B, C] with GroupNorm(x) == x*scale + shift (reference models/common.py:37-57)."""
@@ -541,7 +549,7 @@ def group_norm_fold(x: torch.Tensor, groups: int, eps: float, gamma: Optional[to
         scale = torch.empty((B, C), dtype=torch.float32, device=x.device)
     if shift is None:
         shift = torch.empty((B, C), dtype=torch.float32, device=x.device)
-    need = _cabi.lib().sige_group_norm_fold_workspace(B, C)
+    need = group_norm_fold_workspace(B, C)
     if workspace is None:
         workspace = torch.empty((need,), dtype=torch.float32, device=x.device)
     with torch.cuda.device(x.device):

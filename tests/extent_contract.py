@@ -6,7 +6,8 @@ index no longer fits 15 bits) and against the last row or column.  Each case is 
 is replaced by `edge_origins`; mma_tile_conv_contract.reference is the float64 restatement of the launch (it gathers only the
 tiles, so a tall image costs no more than its buffers).
 
-Imported by tests/test_gpu_extent_contracts.py.
+Imported by tests/test_gpu_extent_contracts.py and tests/test_gpu_extent_contracts_ops.py (and, for the host descriptor, by
+tests/test_extent_limits.py).
 """
 from __future__ import annotations
 
@@ -25,6 +26,16 @@ MID = 32768                     # first row / column whose index needs the 16th 
 NARROW = 16
 GiB = 1 << 30
 HOST_PTR = 0x10000              # a 16-byte aligned address that no host-side test dereferences
+
+
+def need(nbytes: int, device) -> None:
+    """Skip the calling test, with the amount it is short, when the device has less than `nbytes` free."""
+    import pytest
+
+    free, _ = torch.cuda.mem_get_info(device)
+    if free < nbytes:
+        pytest.skip("needs %.1f GiB of free device memory, %.1f GiB free (%.1f GiB short)"
+                    % (nbytes / GiB, free / GiB, (nbytes - free) / GiB))
 
 
 def host_tile_conv(cin=128, cout=256, k=3, N=16):
@@ -50,26 +61,30 @@ def _c_div(a: int, b: int) -> int:
     return q if a >= 0 else -q
 
 
-def edge_origins(spec: mc.Spec, tall: bool, targets: Sequence[int]) -> List[Tuple[int, int]]:
+def spread(targets: Sequence[int], R_long: int, R_short: int, off_long: int, off_short: int, stride: int, short_out: int, tall: bool,
+           name: str = "") -> List[Tuple[int, int]]:
     """Tile origins (h, w) at the given origins along the long axis, spread over the bands of the regular grid along the short
-    axis so that no two tiles write one output pixel.  Every target is placed (asserted)."""
-    Ro = spec.Ro if tall else spec.So
-    So = spec.So if tall else spec.Ro
-    off_long, off_short = (spec.offs[0], spec.offs[1]) if tall else (spec.offs[1], spec.offs[0])
-    short_out = spec.dW if tall else spec.dH
-    bands = [spec.stride * So * j - off_short for j in range(-(-short_out // So))]
+    axis so that no two R_long x R_short footprints, at (off + origin) / stride (C division), share an output pixel.  Every
+    target is placed (asserted)."""
+    bands = [stride * R_short * j - off_short for j in range(-(-short_out // R_short))]
     used = {b: [] for b in bands}
     out = []
     for t in targets:
-        o = _c_div(off_long + t, spec.stride)
+        o = _c_div(off_long + t, stride)
         for b in bands:
-            if all(o + Ro <= lo or lo + Ro <= o for lo in used[b]):
+            if all(o + R_long <= lo or lo + R_long <= o for lo in used[b]):
                 used[b].append(o)
                 out.append((t, b) if tall else (b, t))
                 break
         else:
-            raise AssertionError("%s: no band left for origin %d" % (spec.name, t))
+            raise AssertionError("%s: no band left for origin %d" % (name, t))
     return out
+
+
+def edge_origins(spec: mc.Spec, tall: bool, targets: Sequence[int]) -> List[Tuple[int, int]]:
+    """`spread` for the output tiles of a tile-conv spec."""
+    return spread(targets, spec.Ro if tall else spec.So, spec.So if tall else spec.Ro, spec.offs[0] if tall else spec.offs[1],
+                  spec.offs[1] if tall else spec.offs[0], spec.stride, spec.dW if tall else spec.dH, tall, spec.name)
 
 
 def targets(spec: mc.Spec, tall: bool) -> List[int]:
@@ -252,3 +267,100 @@ def big_check(label: str, bc: BigCase, idx: torch.Tensor, want: torch.Tensor, bo
                              % (label, i // BIG_C, i % BIG_C, float(bc.flat[i]), float(want[k]), float(err[k]), float(bound[k]),
                                 int((ratio > 1).sum())))
     return r
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# the tile ops, the stem, the GroupNorm fold and conv_out on 65535 x 16 and 16 x 65535 images
+# ----------------------------------------------------------------------------------------------------------------------
+def paste_targets(n: int, R: int, off: int, stride: int) -> List[int]:
+    """Origins along an axis of n output pixels whose R-pixel footprints at (off + origin) / stride (C division) hang out
+    before the first pixel, cross pixel 32768 or end on it, and reach the last pixel or hang out past it."""
+    first = -off - stride
+    mid = range(MID * stride - off - R * stride, MID * stride - off + 3)
+    end = range((n - R) * stride - off - 1, n * stride - off)
+    return [first] + list(mid) + list(end)
+
+
+def edge_extent(tall: bool, even: bool = False) -> Tuple[int, int]:
+    long = LIMIT - 1 if even else LIMIT
+    return (long, NARROW) if tall else (NARROW, long)
+
+
+def tile_op_origins(spec, tall: bool) -> dict:
+    """Tile lists for a step_kernel_contracts.TileSpec on an edge image: gather tiles at every target, cycling over the
+    columns (rows) of the short axis, one of them hanging out; pasted and calibration tiles `spread` so none overlap."""
+    n, short = (spec.H, spec.W) if tall else (spec.W, spec.H)
+    if spec.op == "gather":
+        ts = paste_targets(n, 6, 0, 1)
+        cols = [-5, 0, short - 6, short - 1, 5]
+        return {"idx": [(t, cols[i % len(cols)]) if tall else (cols[i % len(cols)], t) for i, t in enumerate(ts)]}
+    if spec.op == "scatter_gather":
+        Ro, off, stride = 4, 1, 1
+    else:
+        (Ro, off), stride = spec.geometry, spec.stride
+    out = {"idx": spread(paste_targets(n, Ro, off, stride), Ro, Ro, off, off, stride, short, tall, spec.name)}
+    if spec.op == "swbr":
+        out["idx1"] = spread(paste_targets(n, 4, 0, 1), 4, 4, 0, 0, 1, short, tall, spec.name)
+    return out
+
+
+def stem_tile_origins(H: int, W: int, R: int, tall: bool) -> List[Tuple[int, int]]:
+    """R x R stem tiles at every target along the long axis, cycling over the short axis (the stem allows overlaps)."""
+    n, short = (H, W) if tall else (W, H)
+    cols = [-(R - 1), 0, short - R, short - 1]
+    return [(t, cols[i % len(cols)]) if tall else (cols[i % len(cols)], t) for i, t in enumerate(paste_targets(n, R, 0, 1))]
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# pure moves (gather, scatter, write-back) on buffers of 2^31 elements or more, checked bitwise
+# ----------------------------------------------------------------------------------------------------------------------
+def tile_pixels(origins: Sequence[Tuple[int, int]], R: int, off: int, stride: int, H: int, W: int):
+    """Per tile n, the in-image pixels of its R x R footprint at (off + origin) / stride (C division): lists of
+    (n, row in tile, column in tile, image row, image column) as long tensors (on the CPU)."""
+    out = []
+    for n, (h, w) in enumerate(origins):
+        h0, w0 = _c_div(off + h, stride), _c_div(off + w, stride)
+        for r in range(R):
+            for s in range(R):
+                if 0 <= h0 + r < H and 0 <= w0 + s < W:
+                    out.append((n, r, s, h0 + r, w0 + s))
+    return torch.tensor(out, dtype=torch.long).unbind(1)
+
+
+def nchw_offsets(C: int, H: int, W: int, b, h, w) -> torch.Tensor:
+    """[K, C] element offsets of the pixels (b, h, w) [K] of an NCHW [B, C, H, W] tensor."""
+    c = torch.arange(C, device=h.device)
+    return ((b[:, None] * C + c) * H + h[:, None]) * W + w[:, None]
+
+
+def nhwc_offsets(C: int, H: int, W: int, b, h, w) -> torch.Tensor:
+    c = torch.arange(C, device=h.device)
+    return ((b[:, None] * H + h[:, None]) * W + w[:, None]) * C + c
+
+
+def moved_check(label: str, flat: torch.Tensor, seed: int, idx: torch.Tensor, want: torch.Tensor) -> None:
+    """Every element of `flat` outside `idx` bitwise as `fill` left it; the elements at `idx` bitwise equal to `want`."""
+    idx, want = idx.reshape(-1), want.reshape(-1).to(flat.dtype)
+    stray = changed(flat, seed)
+    stray = stray[~torch.isin(stray, idx)]
+    if stray.numel():
+        raise AssertionError("%s: %d elements changed outside the written set, the first at element %d"
+                             % (label, stray.numel(), int(stray[0])))
+    got = flat[idx]
+    bad = kc.bits(got) != kc.bits(want)
+    if bool(bad.any()):
+        k = int(bad.nonzero()[0])
+        raise AssertionError("%s: element %d: got %r, want %r; %d elements differ"
+                             % (label, int(idx[k]), float(got[k]), float(want[k]), int(bad.sum())))
+
+
+def unchanged_outside(label: str, flat: torch.Tensor, seed: int, allowed) -> None:
+    """Every element of `flat` for which `allowed(indices)` is False bitwise as `fill` left it, checked chunk by chunk (the
+    written set may be too large to list)."""
+    for k in range(-(-flat.numel() // CHUNK)):
+        part = flat[k * CHUNK:(k + 1) * CHUNK]
+        i = torch.arange(k * CHUNK, k * CHUNK + part.numel(), device=flat.device)
+        stray = (kc.bits(part) != kc.bits(_chunk(flat, k, seed))) & ~allowed(i)
+        if bool(stray.any()):
+            raise AssertionError("%s: %d elements changed outside the written set, the first at element %d"
+                                 % (label, int(stray.sum()), int(i[stray][0])))

@@ -590,8 +590,10 @@ def _phys(shape, layout):
     return (n, h, w, c) if layout == "nhwc" else (n, c, h, w)
 
 
-def make_tile(spec: TileSpec, dtype: torch.dtype, device, oracle_safe: bool = False) -> TileCase:
+def make_tile(spec: TileSpec, dtype: torch.dtype, device, oracle_safe: bool = False, origins: Optional[Dict[str, list]] = None) -> TileCase:
     """Inputs are drawn before the destination, so two specs that differ only in `misalign` hold the same values.
+
+    origins: the tile lists to use ("idx", and "idx1" for swbr) instead of the drawn ones (spec.N is then not used).
 
     oracle_safe: drop the tiles whose pasted output starts above or left of the image.  The C oracle, like the reference's CPU
     code it restates, has no lower bound check there (only the CUDA kernels skip negative rows and columns), so it can only
@@ -617,25 +619,26 @@ def make_tile(spec: TileSpec, dtype: torch.dtype, device, oracle_safe: bool = Fa
             bc[name] = randn(tuple(n if f else 1 for f, n in zip(shp, (B, C, H, W))), dt=aff_dt, scale=sc_, offset=off_)
     if spec.op == "gather":
         o = [(int(h), int(w)) for h, w in zip(rng.integers(-5, H, spec.N), rng.integers(-5, W, spec.N))]
-        idx["idx"] = torch.tensor([(-5, -5), (H - 1, W - 1)] + o, dtype=torch.int32, device=device)
+        o = [(-5, -5), (H - 1, W - 1)] + o if origins is None else origins["idx"]
+        idx["idx"] = torch.tensor(o, dtype=torch.int32, device=device)
         t["x"] = phys((B, C, H >> spec.up, W >> spec.up))
         N, R = idx["idx"].shape[0], 6
         out_shape = (B * N, C, R, R)
     elif spec.op in ("scatter", "swbr"):
         Ro, off = spec.geometry
         forced = [(-1, 3), (3, -2), (-2, -1), (-1, -1)] if spec.stride == 2 else [(-1, -1), (H - 2, W - 3)]
-        o = safe(_paste_origins(spec, rng, spec.N, Ro, off, spec.stride, forced), off, spec.stride)
+        o = safe(_paste_origins(spec, rng, spec.N, Ro, off, spec.stride, forced), off, spec.stride) if origins is None else origins["idx"]
         idx["idx"] = torch.tensor(o, dtype=torch.int32, device=device)
         t["x"] = phys((B * len(o), C, Ro, Ro))
         t["y"] = phys((B, C, H, W))
         if spec.op == "swbr":
-            o1 = safe(_paste_origins(spec, rng, spec.N, 4, 0, 1, [(-2, -1), (H - 2, W - 1)]), 0, 1)
+            o1 = safe(_paste_origins(spec, rng, spec.N, 4, 0, 1, [(-2, -1), (H - 2, W - 1)]), 0, 1) if origins is None else origins["idx1"]
             idx["idx1"] = torch.tensor(o1, dtype=torch.int32, device=device)
             t["x1"] = phys((B * len(o1), C, 4, 4))
             t["y1"] = phys((B, C, H, W))
         out_shape = (B, C, H, W)
     elif spec.op == "scatter_gather":
-        o = safe(_paste_origins(spec, rng, spec.N, 4, 1, 1, [(-1, -1), (H - 2, W - 3), (H - 4, -2)]), 1, 1)
+        o = safe(_paste_origins(spec, rng, spec.N, 4, 1, 1, [(-1, -1), (H - 2, W - 3), (H - 4, -2)]), 1, 1) if origins is None else origins["idx"]
         idx["idx"] = torch.tensor(o, dtype=torch.int32, device=device)
         idx["map"] = scatter_map(H, W, idx["idx"], 4, 4, 1, 1, 1, 1)
         t["x"] = phys((B * len(o), C, 4, 4))

@@ -34,13 +34,6 @@ BASES = [
 KERNELS = ("mma", "wgmma")
 
 
-def _need(nbytes):
-    free, _ = torch.cuda.mem_get_info(DEV)
-    if free < nbytes:
-        pytest.skip("needs %.1f GiB of free device memory, %.1f GiB free (%.1f GiB short)"
-                    % (nbytes / ec.GiB, free / ec.GiB, (nbytes - free) / ec.GiB))
-
-
 def _run(case, init, d):
     from sige_b200 import ops
 
@@ -58,7 +51,7 @@ def test_tile_conv_at_the_extent_limit(base, tall, kernel, dtype):
     spec = ec.spec_at_edge(base, tall)
     peak = ec.peak_bytes(spec, dtype)
     assert peak <= MAX_PEAK, "%s: %.1f GiB" % (spec.name, peak / ec.GiB)
-    _need(peak)
+    ec.need(peak, DEV)
     from sige_b200 import _cabi
 
     flags, path = (_cabi.CONV_TC5, 1) if kernel == "wgmma" else (0, 0)
@@ -87,7 +80,7 @@ def test_tile_conv_on_a_buffer_of_2_to_the_31_elements(bs, dtype):
     es = torch.empty((), dtype=dtype).element_size()
     peak = bs.elements * es + 2 * ec.CHUNK * 8
     assert peak <= MAX_PEAK
-    _need(peak)
+    ec.need(peak, DEV)
     from sige_b200 import ops
 
     bc = ec.make_big_case(bs, dtype, DEV)
