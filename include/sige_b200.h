@@ -259,22 +259,23 @@ typedef struct {
      * 0 (the reference's layout, sige/cuda/gather_kernel.cu:30): every image of the batch uses the same N tile origins.
      * 1: `idx` (and `sc_flags`) hold B*N entries, row b*N + i = tile i of image b — each edit has its own mask; lists shorter
      * than N are padded with SIGE_TILE_NONE origins (such a tile reads zeros and writes nothing).  Weights are read once for
-     * the whole batch.  Full-tensor source and destination only (no stacks). */
+     * the whole batch.  Full-tensor source and destination only (no stacks).  A window source (src_pixel_stride) or a modulated
+     * one (modulation) takes per-image lists only with SIGE_CONV_PER_IMAGE_OPERANDS in `flags`. */
     int idx_per_image;
     /* ---- single source read as a channel window of a wider NHWC buffer ----
      * 0: src[0] has src[0].C channels per pixel.  Otherwise src[0] is channels [c0, c0 + src[0].C) of a buffer with
      * src_pixel_stride channels per pixel, src[0].ptr pointing at channel c0 of pixel 0 — e.g. one torch.split part of a conv's
      * output (SPADE's actv_0 / actv_1 / actv_s, reference gaugan/models/spade_generators/sige_fused_spade_generator.py:160-167),
      * read in place.  The launch is the one of the compacted window (same kernel, plan and result); SIGE_CONV_TC5 is honoured.
-     * Needs n_src == 1, a full-tensor source, no fused shortcut, idx_per_image == 0, a stride that is a multiple of 8 and at
-     * least src[0].C, a 16-byte aligned source, and no modulation. */
+     * Needs n_src == 1, a full-tensor source, no fused shortcut, idx_per_image == 0 (or 1 with SIGE_CONV_PER_IMAGE_OPERANDS), a
+     * stride that is a multiple of 8 and at least src[0].C, a 16-byte aligned source, and no modulation. */
     int src_pixel_stride;
     /* ---- SPADE's modulation in the gather stage (sige_conv_modulation_t above), or NULL ----
      * The pre-op is followed by the modulation.  With SIGE_CONV_TC5, the stride-1 wgmma geometries (3x3 on 6x6 tiles, 1x1 on 4x4
      * tiles, Cin and Cout multiples of 64) run on the wgmma kernel with the plan of the unmodulated launch; everything else (narrow
      * Cin, other Cout, stride 2, no flag) runs on the mma.sync kernel.  Both stage the same operand.  Needs n_src == 1, a
-     * full-tensor source, act == SIGE_ACT_IDENTITY (negative_slope is the activation), no fused shortcut, idx_per_image == 0, a
-     * finite slope, non-null 16-byte aligned gamma / beta whose windows are multiples of 8 elements within their buffers, and
+     * full-tensor source, act == SIGE_ACT_IDENTITY (negative_slope is the activation), no fused shortcut, idx_per_image == 0 (or 1
+     * with SIGE_CONV_PER_IMAGE_OPERANDS), a finite slope, non-null 16-byte aligned gamma / beta whose windows are multiples of 8 elements within their buffers, and
      * src_pixel_stride == 0. */
     const sige_conv_modulation_t *modulation;
 } sige_tile_conv_t;
@@ -307,6 +308,13 @@ typedef struct {
 #define SIGE_CONV_EARLY_SRC0 16
 #define SIGE_CONV_EARLY_SRC1 32
 #define SIGE_CONV_EARLY_SHORTCUT 64
+/* A batch of INDEPENDENT EDITS (sige_tile_conv_t.flags and sige_separable_conv_t.flags): every operand of the launch holds B
+ * images — the source or its window, gamma and beta of the modulation, the destinations — image b of each at b * H * W * (its
+ * pixel stride), and the launch reads per-image tile lists: row b*N + i of `idx` is tile i of image b, a SIGE_TILE_NONE row reads
+ * zeros and writes nothing.  sige_tile_conv: needs idx_per_image == 1 (and so full-tensor source and destination); it is what lets
+ * a window or a modulated source take per-image lists.  sige_separable_conv: needs an NHWC buffer source and buffer destinations
+ * (no stacks).  Both refuse the flag otherwise, before any CUDA call; SIGE_CONV_PADDED behaves as for per-image lists. */
+#define SIGE_CONV_PER_IMAGE_OPERANDS 128
 /* Origin of a padding entry of a per-image tile list (both coordinates). */
 #define SIGE_TILE_NONE (-30000)
 
@@ -429,7 +437,9 @@ int sige_spade_modulate(const void *x, long long x_pixel_stride, const void *gam
  * SIGE_TILE_NONE entry writes nothing to either kind of destination: its stack row keeps its contents (whatever a stack source
  * holds in that row is read and discarded).  A stack-to-stack launch may pass idx = NULL: every row is then a tile.
  * Cin a multiple of 16 in [16, 256], Cout a multiple of 8 in [8, 1024], f16 / bf16 (sige_separable_conv_supported() tells, k = 3);
- * channel counts and offsets multiples of 8; buffers 16-byte aligned.  flags: SIGE_CONV_PDL. */
+ * channel counts and offsets multiples of 8; buffers 16-byte aligned.  flags: SIGE_CONV_PDL, SIGE_CONV_PER_IMAGE_OPERANDS (a batch of
+ * independent edits: `idx` holds B*N rows, row b*N + i = tile i of image b, for a buffer source and buffer destinations); other
+ * bits are ignored. */
 typedef struct {
     const float *dw_weight; /* fp32 [Cin][3][3], affine folded */
     const float *dw_bias;   /* fp32 [Cin] or NULL */

@@ -25,6 +25,7 @@ CONV_TC5 = 2
 CONV_PADDED = 4
 CONV_EARLY_RELEASE = 8
 CONV_EARLY_SRC0, CONV_EARLY_SRC1, CONV_EARLY_SHORTCUT = 16, 32, 64      # early source groups: (mask & 7) << 4
+CONV_PER_IMAGE_OPERANDS = 128       # a batch of independent edits: per-image tile lists over B-image operands
 TILE_NONE = -30000
 
 

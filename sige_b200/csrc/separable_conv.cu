@@ -52,6 +52,7 @@ struct Params {
     int dst_is_stack[2], dH[2], dW[2], dC[2], dc0[2];
     int offH, offW;
     int pdl;
+    int per_image;                     // SIGE_CONV_PER_IMAGE_OPERANDS: idx holds B * N rows (row b*N + i = tile i of image b)
 };
 
 __host__ __device__ constexpr int smem_bytes(int cin) {
@@ -105,7 +106,7 @@ __global__ void __launch_bounds__(NTHREADS) separable_conv_kernel(const Params p
             if (p.src_is_stack) {
                 off = ((long long)gt * HPIX + pix) * p.sC;
             } else {
-                const int b = gt / p.N, ti = gt - b * p.N;
+                const int b = gt / p.N, ti = p.per_image ? gt : gt - b * p.N;
                 const int oh = p.idx[2 * ti], ow = p.idx[2 * ti + 1];
                 const int h = oh + pix / 6, w = ow + pix % 6;
                 ok = oh != SIGE_TILE_NONE && h >= 0 && h < p.H && w >= 0 && w < p.W;
@@ -218,7 +219,7 @@ __global__ void __launch_bounds__(NTHREADS) separable_conv_kernel(const Params p
         const int n = n0 + v * 8, gt = t0 + (m >> 4);
         if (n >= p.Cout || gt >= p.total) continue;
         const int oy = (m >> 2) & 3, ox = m & 3;
-        const int b = gt / p.N, ti = gt - b * p.N;
+        const int b = gt / p.N, ti = p.per_image ? gt : gt - b * p.N;
         const int oh = p.idx ? p.idx[2 * ti] : 0;            // no list: a stack-to-stack launch, every row is a tile
         if (oh == SIGE_TILE_NONE) continue;                  // padding tiles write nothing, to a stack as to a buffer
         long long off;
@@ -288,6 +289,10 @@ extern "C" int sige_separable_conv(const sige_separable_conv_t *d, sige_stream_t
                      "pixel channels multiples of 8)", b, r.dst_c0, r.dst_c0 + d->Cout, r.dst_C);
         if (!r.dst_is_stack) SIGE_REQUIRE(r.dH > 0 && r.dW > 0, "sige_separable_conv: branch %d: destination extent %d x %d", b, r.dH, r.dW);
     }
+    const bool per_image = (d->flags & SIGE_CONV_PER_IMAGE_OPERANDS) != 0;
+    if (per_image)
+        SIGE_REQUIRE(!d->src_is_stack && !d->branch[0].dst_is_stack && (d->nbranch == 1 || !d->branch[1].dst_is_stack),
+                     "sige_separable_conv: SIGE_CONV_PER_IMAGE_OPERANDS (per-image tile lists) needs a buffer source and buffer destinations, not stacks");
     if (d->N == 0) return 0;
     SIGE_REQUIRE(d->src != nullptr, "sige_separable_conv: null source");
     SIGE_REQUIRE(d->idx != nullptr || (d->src_is_stack && d->branch[0].dst_is_stack && (d->nbranch == 1 || d->branch[1].dst_is_stack)),
@@ -328,6 +333,7 @@ extern "C" int sige_separable_conv(const sige_separable_conv_t *d, sige_stream_t
     p.offH = d->offH;
     p.offW = d->offW;
     p.pdl = (d->flags & SIGE_CONV_PDL) ? 1 : 0;
+    p.per_image = per_image ? 1 : 0;
     cudaStream_t st = (cudaStream_t)stream;
     return d->dtype == SIGE_F16 ? sep::launch<__half>(p, st) : sep::launch<__nv_bfloat16>(p, st);
 }

@@ -558,11 +558,16 @@ using namespace sige;
 extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) {
     SIGE_REQUIRE(a != nullptr, "sige_tile_conv: null descriptor");
     SIGE_REQUIRE(a->src_pixel_stride == 0 || a->modulation == nullptr, "sige_tile_conv: a source window cannot be modulated");
+    // a batch of independent edits: per-image lists over full tensors (every operand indexed by the tile's image, as for any B > 1)
+    const bool per_image_ops = (a->flags & SIGE_CONV_PER_IMAGE_OPERANDS) != 0;
+    if (per_image_ops)
+        SIGE_REQUIRE(a->idx_per_image && !a->src_is_stack && !a->dst_is_stack,
+                     "sige_tile_conv: SIGE_CONV_PER_IMAGE_OPERANDS needs per-image tile lists (idx_per_image = 1) and full-tensor source and destination");
     if (a->src_pixel_stride != 0) {
         SIGE_REQUIRE(a->n_src == 1, "sige_tile_conv (window): one source segment (got n_src %d)", a->n_src);
         SIGE_REQUIRE(!a->src_is_stack, "sige_tile_conv (window): the source must be a full tensor read through the tile list, not a stack");
         SIGE_REQUIRE(a->n_src2 == 0, "sige_tile_conv (window): no fused shortcut");
-        SIGE_REQUIRE(!a->idx_per_image, "sige_tile_conv (window): per-image tile lists are not supported");
+        SIGE_REQUIRE(!a->idx_per_image || per_image_ops, "sige_tile_conv (window): per-image tile lists need SIGE_CONV_PER_IMAGE_OPERANDS");
         SIGE_REQUIRE(a->src_pixel_stride >= a->src[0].C && a->src_pixel_stride % 8 == 0,
                      "sige_tile_conv (window): pixel stride %d must be a multiple of 8 and at least the source's %d channels", a->src_pixel_stride, a->src[0].C);
         SIGE_REQUIRE(((uintptr_t)a->src[0].ptr & 15) == 0, "sige_tile_conv (window): source is not 16-byte aligned");
@@ -573,7 +578,7 @@ extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) {
         SIGE_REQUIRE(!a->src_is_stack, "sige_tile_conv (modulation): the source must be a full tensor read through the tile list, not a stack");
         SIGE_REQUIRE(a->act == SIGE_ACT_IDENTITY, "sige_tile_conv (modulation): act must be identity (negative_slope is the activation)");
         SIGE_REQUIRE(a->n_src2 == 0, "sige_tile_conv (modulation): no fused shortcut");
-        SIGE_REQUIRE(!a->idx_per_image, "sige_tile_conv (modulation): per-image tile lists are not supported");
+        SIGE_REQUIRE(!a->idx_per_image || per_image_ops, "sige_tile_conv (modulation): per-image tile lists need SIGE_CONV_PER_IMAGE_OPERANDS");
         SIGE_REQUIRE(isfinite(m->negative_slope), "sige_tile_conv (modulation): negative_slope must be finite");
     }
     SIGE_REQUIRE(a->dtype == SIGE_F16 || a->dtype == SIGE_BF16,

@@ -375,7 +375,7 @@ class CudaExecutor:
 
     def prepare_conv(self, fc: FusedConv) -> None:
         ops = self.ops
-        from ._cabi import CONV_EARLY_RELEASE, CONV_PADDED, CONV_PDL, CONV_TC5
+        from ._cabi import CONV_EARLY_RELEASE, CONV_PADDED, CONV_PDL, CONV_PER_IMAGE_OPERANDS, CONV_TC5
 
         s = fc.spec
         w, b = s.weight, s.bias
@@ -448,6 +448,8 @@ class CudaExecutor:
             mod = ops.conv_modulation(gamma, beta, slope)
             d.modulation = ctypes.pointer(mod)
             keep.append(mod)
+        if s.tile_img is not None and (s.modulation is not None or d.src_pixel_stride):
+            d.flags |= CONV_PER_IMAGE_OPERANDS    # a batch's window / gamma / beta: image b of each at b * H * W * (pixel stride)
         d.n_src2 = 0
         if s.shortcut is not None:
             sc_tensors, sc_w, sc_b, sc_flags = s.shortcut
@@ -547,6 +549,11 @@ class CudaExecutor:
         the concatenated lists with a per-row image index, and a new batch recompiles."""
         return True
 
+    def per_image_operands_supported(self) -> bool:
+        """Can the modulated, windowed and separable launches of a batch of edits read per-edit lists over operands of E images
+        (SIGE_CONV_PER_IMAGE_OPERANDS)?  Then the GauGAN generators' SPADE layers lower for a batch as for one edit."""
+        return True
+
     def prepare_writeback(self, entries) -> Callable[[int], None]:
         """One `sige_tile_writeback` over (src buffer, module cache, tile list, off, stride, output tile) entries."""
         return self.ops.tile_writeback_launcher(entries)
@@ -614,11 +621,13 @@ class CudaExecutor:
 
     def prepare_separable(self, rec: "SepLaunch") -> Callable[[int], None]:
         """One sige_separable_conv launch of a SepLaunch record (gamma and beta of one SPADE layer)."""
-        from ._cabi import CONV_PDL
+        from ._cabi import CONV_PDL, CONV_PER_IMAGE_OPERANDS
 
         branches = [self._separable_weights(dw, pw_w, pw_b) + (dst.raw,) for (dw, pw_w, pw_b, dst) in rec.branches]
         src = rec.src[:, rec.c0:rec.c0 + rec.Cin]
         ops, idx, off, stack, batch, flags = self.ops, rec.idx, rec.off, rec.src_stack, rec.batch, (CONV_PDL if rec.pdl else 0)
+        if rec.tile_img is not None:
+            flags |= CONV_PER_IMAGE_OPERANDS      # a batch of edits: the slot's per-edit lists
 
         def run(_stream):
             ops.separable_conv(src, branches, idx, src_stack=stack, offset=off, batch=batch, flags=flags)
@@ -836,6 +845,7 @@ class SepLaunch:
     def __init__(self, name: str, src: torch.Tensor, src_stack: bool, c0: int, idx: torch.Tensor, off: int, batch: int, slot: int):
         self.name, self.src, self.src_stack, self.c0, self.idx, self.off, self.batch = name, src, src_stack, c0, idx, off, batch
         self.slot = slot                      # index of the launch in Lowering.steps
+        self.tile_img: Optional[torch.Tensor] = None       # a batch of edits: image of each row of idx (the IdxSlot's per-edit lists)
         self.pdl = False
         self.branches: List[Tuple[DWConv, torch.Tensor, Optional[torch.Tensor], Buf]] = []
 
@@ -943,6 +953,8 @@ class Lowering:
         self.headroom = float(headroom)
         ok = getattr(executor, "batch_slots_supported", None)
         self.batch_slots = ok is not None and ok()
+        ok = getattr(executor, "per_image_operands_supported", None)
+        self.per_image_ops = self.batch_slots and ok is not None and ok()
         self.module_names = module_names or {}
         self.pdl, self.tc5, self.producer_preop, self.fuse_shortcut = pdl, tc5, producer_preop, fuse_shortcut
         self.fused_attention, self.sparse_stem, self.ksplit = fused_attention, sparse_stem, ksplit
@@ -1799,7 +1811,7 @@ class Lowering:
         if not isinstance(sx, Stack) or isinstance(sx, (ModStack, WinStack)):
             return None
         g, f = sx.gather, sx.src
-        if (getattr(g, "tile_images", None) is not None or g.activation_name != "identity" or g.block_size[0] != g.block_size[1]
+        if (not self._batch_ok(g) or g.activation_name != "identity" or g.block_size[0] != g.block_size[1]
                 or int(g.active_indices.shape[0]) == 0 or not f.plain or len(f.segs) != 1):
             return None
         windows = getattr(self.ex, "strided_conv_supported", None) is not None
@@ -1850,7 +1862,7 @@ class Lowering:
         st, c0, C = win
         g = st.gather
         if (st.src.single is None or st.scale is not None or st.shift is not None or g.activation_name != "identity"
-                or g.block_size[0] != g.block_size[1] or getattr(g, "tile_images", None) is not None or c0 % 8 or C % 8):
+                or g.block_size[0] != g.block_size[1] or not self._batch_ok(g) or c0 % 8 or C % 8):
             return None
         k, s = _pair(weight.shape[2:]), _pair(stride)
         if k[0] != k[1] or s[0] != s[1] or not ok(C, int(weight.shape[0]), k[0], s[0]):
@@ -1899,7 +1911,7 @@ class Lowering:
         if isinstance(v, Stack):
             g = v.gather
             if (v.src.single is None or v.scale is not None or v.shift is not None or g.activation_name != "identity"
-                    or tuple(g.block_size) != (6, 6) or getattr(g, "tile_images", None) is not None or c0 % 8):
+                    or tuple(g.block_size) != (6, 6) or not self._batch_ok(g) or c0 % 8):
                 return None
             return v, c0
         if isinstance(v, ChanSlice):             # torch.split of a stack: the whole stack became one NHWC buffer
@@ -1948,21 +1960,25 @@ class Lowering:
 
     def _sep_fits(self, so: SepOut, g) -> bool:
         """Can the launch scatter through Gather `g`'s tile set?"""
-        if getattr(g, "tile_images", None) is not None or tuple(g.block_size) != (6, 6) or tuple(g.offset)[0] != tuple(g.offset)[1]:
+        if not self._batch_ok(g) or tuple(g.block_size) != (6, 6) or tuple(g.offset)[0] != tuple(g.offset)[1]:
             return False
         src = so.dw.src
         if isinstance(src, Stack):
             return self._same_gather(src.gather, g)
+        if getattr(g, "tile_images", None) is not None:      # a materialised stack has no per-edit lists
+            return False
         return int(src.tensor.shape[0]) % max(1, int(g.active_indices.shape[0])) == 0 and int(g.active_indices.shape[0]) > 0
 
     def _sep_emit(self, node: Node, so: SepOut, dst: Buf, g) -> None:
         """Add the branch to the previous launch if that one is the other branch of the same SPADE layer (same source window,
         same tile set, emitted just before), else open a new launch."""
         dw = so.dw
+        timg = None
         if isinstance(dw.src, Stack):
             f = dw.src.src
-            src, src_stack, idx = f.single.raw, False, self.slot(g).buf
-            f.single.readers.append((idx, 6, 0, None))
+            sl = self.slot(g)
+            src, src_stack, idx, timg = f.single.raw, False, sl.buf, sl.tile_img
+            f.single.readers.append((idx, 6, 0, timg))
         else:
             src, src_stack, idx = dw.src.tensor, True, g.active_indices.to(self.dev)
         last = self.separable[-1] if self.separable else None
@@ -1972,7 +1988,7 @@ class Lowering:
             last.name += "+" + self._module_name(node)
         else:
             rec = SepLaunch(self._module_name(node), src, src_stack, dw.c0, idx, int(g.offset[0]), dst.shape[0], len(self.steps))
-            rec.pdl = self.pdl
+            rec.pdl, rec.tile_img = self.pdl, timg
             rec.branches.append((dw, so.weight, so.bias, dst))
             self.separable.append(rec)
             self.steps.append(("separable", None))
@@ -1982,7 +1998,7 @@ class Lowering:
                 self.steps[rec.slot] = ("separable", ex.prepare_separable(rec))
 
             self._pending_prepare.append(prep)
-        slot = next((sl for sl in self.slots.values() if sl.buf is idx), None)
+        slot = next((sl for sl in self.slots.values() if sl.buf is idx and timg is None), None)
         self.cache_writers.append((dst, slot, int(g.offset[0]), 1, 4))
         _ = dst.raw               # written in place every step: the buffer must exist (initialised from the module's cache)
 
@@ -2013,6 +2029,11 @@ class Lowering:
 
     def _module_name(self, node: Node) -> str:
         return self.module_names.get(id(node.module), "n%d" % node.index)
+
+    def _batch_ok(self, g) -> bool:
+        """Can the SPADE launches (modulated, windowed, separable) read Gather `g`'s tile set?  One edit always; a batch of edits
+        when the executor runs them on per-edit lists over operands of E images."""
+        return getattr(g, "tile_images", None) is None or self.per_image_ops
 
     @staticmethod
     def _same_gather(a, g) -> bool:

@@ -719,8 +719,10 @@ def separable_conv(x: torch.Tensor, branches, idx: Optional[torch.Tensor] = None
     through ``idx`` (int32 [N, 2] halo-tile origins), or a tile stack [B*N, Cin, 6, 6] (``src_stack``).  ``branches``: one or two
     (dw_weight fp32 [Cin, 9], dw_bias fp32 [Cin], pw_weight [Cout, Cin] in x's dtype, pw_bias fp32 [Cout] or None, out) with the
     affine folded into the depthwise part (``separable_fold``); ``out`` is a channels-innermost NHWC buffer [B, Cout, dH, dW] whose
-    tiles at ``idx + offset`` are overwritten in place, or a stack [B*N, Cout, 4, 4] (``dst_stack``)."""
-    from ._cabi import SeparableConv
+    tiles at ``idx + offset`` are overwritten in place, or a stack [B*N, Cout, 4, 4] (``dst_stack``).  With
+    CONV_PER_IMAGE_OPERANDS in ``flags`` (a batch of independent edits; buffer source and destinations) ``idx`` holds B lists of
+    N rows, row b*N + i = tile i of image b."""
+    from ._cabi import CONV_PER_IMAGE_OPERANDS, SeparableConv
 
     _require_cuda(x, idx)
     if not 1 <= len(branches) <= 2:
@@ -740,6 +742,10 @@ def separable_conv(x: torch.Tensor, branches, idx: Optional[torch.Tensor] = None
         if idx is None:
             raise ValueError("separable_conv: a buffer source needs the tile list")
         d.B, d.H, d.W, d.N = int(x.shape[0]), int(x.shape[2]), int(x.shape[3]), int(idx.shape[0])
+        if flags & CONV_PER_IMAGE_OPERANDS:
+            if d.N % d.B:
+                raise ValueError("separable_conv: per-image lists hold B * N rows")
+            d.N //= d.B
     if idx is not None:
         idx = _idx(idx)
         if idx.dim() != 2 or idx.shape[1] != 2 or (src_stack and int(idx.shape[0]) != d.N):

@@ -342,6 +342,36 @@ def gaugan_gc_inputs(size: str = "mini") -> Tuple[torch.Tensor, torch.Tensor, to
     return onehot(lab0), onehot(lab1), mask
 
 
+def gaugan_gc_edits(size: str = "mini", E: int = 3) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """E independent label edits of the workload's scene: the original map [1, 36, H, W], the edited maps [E, 36, H, W] and their
+    masks [E, H, W] (the `set_masks` argument of a batch, after the usual pyramid per edit).  Edit 0 is the workload's edit, 1 a
+    smaller one elsewhere (`edit_b`), 2 a strip along the image's left border, later ones seeded rectangles of 1 to 3 % of the
+    image anywhere."""
+    s0, s1, mask = gaugan_gc_inputs(size)
+    H, W = int(s0.shape[2]), int(s0.shape[3])
+    lab0 = s0.argmax(1)[0]
+    maps = [s1[0]]
+    for e in range(1, E):
+        lab = lab0.clone()
+        if e == 1:
+            if size == "full":
+                lab[360:440, 700:800] = 3
+            else:
+                lab[40:48, 16:28] = 3
+        elif e == 2:
+            lab[H // 4:H // 4 + H // 3, 0:W // 12] = 11
+        else:
+            g = torch.Generator().manual_seed(1000 + e)
+            h, w = (int(v) for v in torch.randint(H // 10, H // 5, (2,), generator=g))
+            y, x = int(torch.randint(0, H - h + 1, (1,), generator=g)), int(torch.randint(0, W - w + 1, (1,), generator=g))
+            lab[y:y + h, x:x + w] = int(torch.randint(0, 35, (1,), generator=g))
+        t = torch.zeros(36, H, W)
+        t.scatter_(0, lab[None], 1.0)
+        maps.append(t)
+    s1s = torch.stack(maps, 0)
+    return s0, s1s, (s1s != s0).any(1)
+
+
 def run_gaugan_gc(net: nn.Module, downsample_mask, dilate_mask, device="cpu", fused=None, size: str = "mini"):
     """Dense pass on the original label map, set_masks (the dilated difference-mask pyramid of reference gaugan/runner.py), sparse
     pass on the edited one."""

@@ -2,7 +2,7 @@
 the default) or the full SPADE generator.
 
     python tools/bench_gaugan_gc.py [--generator gc|spade] [--steps 50] [--warmup 10] [--dtype fp16|bf16] [--size full|mini]
-                                    [--headroom 0.5] [--dump-outputs DIR] [--per-launch]
+                                    [--headroom 0.5] [--dump-outputs DIR] [--per-launch] [--edits E]
 
 Workload (--generator gc): sige_b200/workloads/gaugan_gc.py at full size — 512 x 1024 label map, config 32_32_32_48_32_24_24_32 (the
 published GAN Compression Cityscapes sub-network), 5 sparse blocks, the 2.98 % label edit of the full-size GauGAN workload.
@@ -16,7 +16,11 @@ the wall time from `set_masks_async` of a second, smaller label edit to the sync
 interactive user's next stroke), taken three times alternating with the first edit; `next_edit_in_place` says whether the
 compiled step took the edit without recompiling.  --per-launch adds the CUDA-event time of every tile-conv launch of the compiled
 step, each after an L2 flush (launch latency included), and the kernel it runs (from its launch plan: `wgmma bn=.. ksplit=..` or
-`mma.sync`).  Prints one JSON line.
+`mma.sync`).  --edits E (E > 1) adds a batch of E independent label edits of the scene (`gaugan_gc_edits`: the workload's edit,
+`edit_b`, then seeded edits elsewhere): one compiled step of the batch against the E single-edit steps, timed in the same run and
+alternated (each step replayed through its own CUDA graph, an L2 flush before each), and the install of the next batch of E edits
+into the batched step through `set_masks` and through `set_masks_async`, against a recompile (wall time to the synchronised end
+of the step that follows).  Prints one JSON line.
 """
 from __future__ import annotations
 
@@ -49,19 +53,10 @@ def gpu_info() -> dict:
 
 def edit_b(size: str):
     """A second label edit, smaller than the workload's and elsewhere in the image: (edited label map, its mask)."""
-    import torch
-
     from sige_b200.workloads import gaugan_gc as G
 
-    s0, _, _ = G.gaugan_gc_inputs(size)
-    lab = s0.argmax(1)[0].clone()
-    if size == "full":
-        lab[360:440, 700:800] = 3
-    else:
-        lab[40:48, 16:28] = 3
-    s1 = torch.zeros_like(s0)
-    s1.scatter_(1, lab[None, None], 1.0)
-    return s1, (s1 != s0).any(1)[0]
+    _, s1s, masks = G.gaugan_gc_edits(size, 2)
+    return s1s[1:2], masks[1]
 
 
 def next_edit(net, x_a, dilate_mask, downsample_mask, size: str, dev):
@@ -88,6 +83,92 @@ def next_edit(net, x_a, dilate_mask, downsample_mask, size: str, dev):
     return out, in_place
 
 
+def batch_of_edits(net, E: int, size: str, dtype, headroom: float, steps: int, warmup: int, flush, dev) -> dict:
+    """The --edits figures (see the module docstring); `net` has had its dense pass and is in sparse mode."""
+    import numpy as np
+    import torch
+
+    from sige.utils import dilate_mask, downsample_mask
+    from sige_b200.masks import stack_mask_pyramids
+    from sige_b200.workloads import gaugan_gc as G
+
+    _, s1s, masks = G.gaugan_gc_edits(size, 2 * E)
+    s1s, masks = s1s.to(dev), masks.to(dev)
+
+    def pyr(m):
+        return downsample_mask(dilate_mask(m, 1), min_res=(4, 8), dilation=0)
+
+    def batch(sel):
+        return stack_mask_pyramids([pyr(masks[e]) for e in sel])
+
+    A, B = list(range(E)), list(range(E, 2 * E))
+    singles = []
+    with torch.no_grad():
+        for e in A:
+            net.set_fused(True, dtype=dtype, headroom=headroom)
+            net.set_masks(pyr(masks[e]))
+            net(s1s[e:e + 1])
+            singles.append((net.fused_step, s1s[e:e + 1]))
+        net.set_fused(True, dtype=dtype, headroom=headroom)
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats(dev)
+        base = torch.cuda.memory_allocated(dev)
+        t0 = time.perf_counter()
+        net.set_masks(batch(A))
+        net(s1s[A])
+        torch.cuda.synchronize()
+        compile_s = time.perf_counter() - t0
+        peak = torch.cuda.max_memory_allocated(dev) - base
+        step, xa = net.fused_step, s1s[A]
+
+    def one(st, x):
+        if flush is not None:
+            flush.fill_(1)
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        st(x)
+        b.record()
+        return a, b
+
+    batched, separate = [], []
+    with torch.no_grad():
+        for i in range(warmup + steps):
+            ev_b = one(step, xa)
+            ev_s = [one(st, x) for st, x in singles]
+            torch.cuda.synchronize()
+            if i >= warmup:
+                batched.append(ev_b[0].elapsed_time(ev_b[1]))
+                separate.append(sum(a.elapsed_time(b) for a, b in ev_s))
+
+    def install(fn, pyramid, x):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        fn(pyramid)
+        net(x)
+        torch.cuda.synchronize()
+        return time.perf_counter() - t0
+
+    res = {"sync": [], "async": []}
+    in_place = True
+    with torch.no_grad():
+        pa, pb = batch(A), batch(B)
+        for _ in range(3):
+            for k, fn in (("sync", net.set_masks), ("async", net.set_masks_async)):
+                res[k].append(install(fn, pb, s1s[B]))
+                in_place = in_place and net.fused_step is step
+                install(net.set_masks, pa, xa)
+        in_place = in_place and net.masks_async_ok()
+        recompile = []
+        for _ in range(2):
+            net.set_fused(True, dtype=dtype, headroom=headroom)
+            recompile.append(install(net.set_masks, pb, s1s[B]))
+    return {"E": E, "mask_pixels": [int(m.sum()) for m in masks[A]], "batched_ms": float(np.median(batched)),
+            "single_edit_steps_ms": float(np.median(separate)), "batched_over_singles": float(np.median(batched) / np.median(separate)),
+            "rounds": len(batched), "batched_compile_seconds": compile_s, "batched_compile_peak_bytes": int(peak),
+            "next_batch_set_masks_seconds": res["sync"], "next_batch_set_masks_async_seconds": res["async"],
+            "next_batch_recompile_seconds": recompile, "next_batch_in_place": in_place}
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--generator", choices=["gc", "spade"], default="gc", help="sub-mobile (GAN Compression) or full SPADE generator")
@@ -99,6 +180,7 @@ def main():
     ap.add_argument("--headroom", type=float, default=0.5, help="extra tile-list capacity of the compiled step")
     ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     ap.add_argument("--per-launch", action="store_true", help="time every tile-conv launch of the compiled step on its own")
+    ap.add_argument("--edits", type=int, default=1, help="E > 1: also time a batch of E label edits against E single-edit steps")
     args = ap.parse_args()
 
     import numpy as np
@@ -186,6 +268,9 @@ def main():
     }
     if per_launch is not None:
         line["per_launch"] = per_launch
+    if args.edits > 1:
+        line["batch_of_edits"] = batch_of_edits(net, args.edits, args.size, dtype, args.headroom, max(1, args.steps), max(1, args.warmup), flush, dev)
+        line["batch_of_edits"]["gpu"] = gpu_info()
     print(json.dumps(line), flush=True)
 
 
