@@ -400,8 +400,9 @@ int sige_attention_tokens(const void *qkv, void *out, int B, int N, int C, int d
  *   out[b, h, i, :] = softmax_j(scale * q[b, h, i, :] . k[b, h, j, :]) v[b, h, j, :]
  * Element strides {batch, head, token} per operand, the head dim D contiguous — so both the reference's "(b h) n d" copies
  * (heads = 1, B = b*h) and the "b n (h d)" layout the Linear layers produce are addressable without a rearrange.
- * D in {32, 40, 64, 80, 128, 160}, f16 / bf16 (sige_sparse_attention_supported() tells); strides multiples of 8 elements, buffers
- * 16-byte aligned; scale > 0; Nq == 0 is a no-op. */
+ * D in {32, 40, 64, 80, 128, 160, 512}, f16 / bf16 (sige_sparse_attention_supported() tells); strides multiples of 8 elements,
+ * buffers 16-byte aligned; scale > 0; Nq == 0 is a no-op.  D = 512 (the single head of the Stable Diffusion VAE's mid-block
+ * attention) splits the key range over a thread-block cluster and merges the partial softmax statistics in the same launch. */
 typedef struct {
     const void *q;               /* Nq query tokens per (batch, head) */
     const void *k, *v;           /* Nk key / value tokens per (batch, head) */

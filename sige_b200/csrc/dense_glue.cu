@@ -468,6 +468,16 @@ __global__ void __launch_bounds__(CO_TH * 32) conv_out_kernel(const T *__restric
 
 using namespace sige;
 
+// Weights of more than 48 KB (Cout > ~320: the Stable Diffusion VAE decoder's 4 -> 512 stem) need the dynamic shared-memory opt-in.
+template <typename K> static bool conv_in_smem_ok(K kernel, size_t smem) {
+    if (smem <= 48 * 1024) return true;
+    if (smem > 227 * 1024 || cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+        (void)cudaGetLastError();
+        return false;
+    }
+    return true;
+}
+
 extern "C" {
 
 int sige_conv_in_nhwc(const void *x, const void *w, const void *bias, void *out, int dtype, int B, int H, int W, int Cin, int Cout,
@@ -476,7 +486,8 @@ int sige_conv_in_nhwc(const void *x, const void *w, const void *bias, void *out,
     SIGE_REQUIRE(B > 0 && H > 0 && W > 0 && W % 4 == 0 && Cin >= 1 && Cin <= 4 && Cout > 0 && Cout % 8 == 0, "sige_conv_in_nhwc: needs W %% 4 == 0, Cin <= 4 and Cout %% 8 == 0");
     SIGE_REQUIRE(((uintptr_t)out & 15) == 0, "sige_conv_in_nhwc: output not 16-byte aligned");
     const size_t smem = sizeof(float) * ((size_t)(Cout / 8) * conv_in_pitch(Cin) + Cout);
-    SIGE_REQUIRE(smem <= 48 * 1024, "sige_conv_in_nhwc: weights do not fit in shared memory");
+    SIGE_REQUIRE(dtype != SIGE_F16 || conv_in_smem_ok(conv_in_kernel<__half>, smem), "sige_conv_in_nhwc: weights do not fit in shared memory");
+    SIGE_REQUIRE(dtype != SIGE_BF16 || conv_in_smem_ok(conv_in_kernel<__nv_bfloat16>, smem), "sige_conv_in_nhwc: weights do not fit in shared memory");
     const long long total = (long long)B * H * (W / 4) * (Cout / 8);
     SIGE_REQUIRE(total * 4 < 2147483647LL, "sige_conv_in_nhwc: tensor too large");
     const long long want_blocks = (total + 255) / 256;
@@ -506,7 +517,8 @@ int sige_conv_in_nhwc_tiles(const void *x, const void *w, const void *bias, void
     SIGE_REQUIRE(((uintptr_t)out & 15) == 0, "sige_conv_in_nhwc_tiles: output not 16-byte aligned");
     if (n_tiles == 0) return 0;
     const size_t smem = sizeof(float) * ((size_t)(Cout / 8) * conv_in_pitch(Cin) + Cout);
-    SIGE_REQUIRE(smem <= 48 * 1024, "sige_conv_in_nhwc_tiles: weights do not fit in shared memory");
+    SIGE_REQUIRE(dtype != SIGE_F16 || conv_in_smem_ok(conv_in_tiles_kernel<__half>, smem), "sige_conv_in_nhwc_tiles: weights do not fit in shared memory");
+    SIGE_REQUIRE(dtype != SIGE_BF16 || conv_in_smem_ok(conv_in_tiles_kernel<__nv_bfloat16>, smem), "sige_conv_in_nhwc_tiles: weights do not fit in shared memory");
     const long long NT = (long long)B * n_tiles;
     const long long total = NT * R * S * (Cout / 8);
     SIGE_REQUIRE(total < 2147483647LL && (long long)B * H * W * Cout < 2147483647LL * 8, "sige_conv_in_nhwc_tiles: tensor too large");

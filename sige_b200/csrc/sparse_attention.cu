@@ -12,7 +12,11 @@
 // through a double-buffered cp.async ring; logits, running max / sum and the output accumulator never leave registers.
 // Tensor cores: mma.sync.m16n8k16 (fp32 accumulate).  Head dims that are not a multiple of 16 (40) are zero-padded in
 // shared memory only.
+#include <cooperative_groups.h>
+
 #include "common.cuh"
+
+namespace cg = cooperative_groups;
 
 namespace sige {
 namespace sattn {
@@ -221,6 +225,248 @@ template <typename T, int D> static int launch(const Params &p, int BH, cudaStre
     return check_launch("sige_sparse_attention");
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// D = 512: the single head of the Stable Diffusion VAE's mid-block attention (SIGEAttnBlock, 512 channels, 4096 keys).
+// One warp cannot hold 16 query rows x 512 fp32 accumulators (256 registers), so a CTA of 8 warps shares its 64 queries:
+// warp w owns query rows 16 (w & 3) .. +15, computes their logits against keys 16 (w >> 2) .. +15 of each 32-key block and
+// accumulates output channels 256 (w >> 2) .. +255 (128 fp32 registers).  Row maxima cross the two key halves through shared
+// memory, P goes through shared memory as 16 bits.  Q (64 KB) stays resident; K / V blocks of 32 keys stream through a
+// double-buffered cp.async ring (4 x 32 KB).
+//
+// A 15 % edit of a 64 x 64 latent has only ~600-800 queries, 10-13 CTAs: the key range is split over the CS CTAs of a
+// cluster (grid (query blocks, CS, B * heads)), each runs its own online softmax over whole key blocks, and the partial
+// (max, sum, O) are merged through distributed shared memory in the same launch — CTA r of the cluster reduces output
+// channels [r 512 / CS, (r + 1) 512 / CS) of all 64 rows, summing the peers in rank order (deterministic).
+namespace wide {
+constexpr int D = 512;
+constexpr int BM = 64;                        // queries per CTA
+constexpr int BNK = 32;                       // keys per ring stage
+constexpr int NTHREADS = 256;
+constexpr int MAX_CS = 8;                     // portable cluster size
+constexpr int PITCH = D * 2 + 16;             // bytes per Q / K / V row
+constexpr int P_PITCH = BNK * 2 + 16;         // bytes per P row
+constexpr int O_PITCH = D + 8;                // floats per row of the fp32 partial O (merge)
+constexpr int OFF_Q = 0;
+constexpr int OFF_K = OFF_Q + BM * PITCH;     // [2][BNK] rows
+constexpr int OFF_V = OFF_K + 2 * BNK * PITCH;
+constexpr int OFF_P = OFF_V + 2 * BNK * PITCH;
+constexpr int OFF_MAX = OFF_P + BM * P_PITCH;            // [2][BM] float: row maxima of the two key halves
+constexpr int OFF_L = OFF_MAX + 2 * BM * 4;              // [2][BM] float: row sums of the two key halves
+constexpr int OFF_ML = OFF_L + 2 * BM * 4;               // [BM] float2: (max, sum) of this CTA's key range, read by the peers
+constexpr int OFF_W = OFF_ML + BM * 8;                   // [MAX_CS][BM] float: merge weight of each peer
+constexpr int TOTAL = OFF_W + MAX_CS * BM * 4;
+constexpr int OFF_O = OFF_K;                             // [BM][O_PITCH] float, over the K / V ring once the loop is done
+static_assert(BM * O_PITCH * 4 <= OFF_P - OFF_K, "partial O must fit over the K / V ring");
+static_assert(TOTAL <= 232448, "shared memory");
+
+template <typename T>
+__global__ void __launch_bounds__(NTHREADS, 1) kernel(const Params p, const int cs) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    cg::cluster_group cluster = cg::this_cluster();
+    const uint32_t sb = smem_u32(smem);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int rg = warp & 3, kh = warp >> 2;
+    const int g = lane >> 2, tq = lane & 3;
+    const int rank = cs > 1 ? (int)cluster.block_rank() : 0;
+    const int q0 = blockIdx.x * BM;
+    const int bh = blockIdx.z, b = bh / p.heads, h = bh - b * p.heads;
+    const T *qp = reinterpret_cast<const T *>(p.q) + b * p.q_sb + h * p.q_sh;
+    const T *kp = reinterpret_cast<const T *>(p.k) + b * p.k_sb + h * p.k_sh;
+    const T *vp = reinterpret_cast<const T *>(p.v) + b * p.v_sb + h * p.v_sh;
+    constexpr int CH = D / 8;
+    // this CTA's key blocks: [t0, t1), never empty (the host keeps cs <= blocks)
+    const int nblk = (p.Nk + BNK - 1) / BNK;
+    const int t0 = (int)((long long)nblk * rank / cs), t1 = (int)((long long)nblk * (rank + 1) / cs);
+
+    for (int i = tid; i < BM * CH; i += NTHREADS) {
+        const int r = i / CH, c = i - r * CH;
+        const bool ok = q0 + r < p.Nq;
+        cp_async16_zfill(sb + OFF_Q + r * PITCH + c * 16, qp + (ok ? (long long)(q0 + r) * p.q_sn + c * 8 : 0), ok);
+    }
+    auto load_kv = [&](int t, int stage) {
+        const int k0 = t * BNK;
+        for (int i = tid; i < BNK * CH; i += NTHREADS) {
+            const int r = i / CH, c = i - r * CH;
+            const bool ok = k0 + r < p.Nk;
+            const long long tok = ok ? (long long)(k0 + r) : 0;
+            cp_async16_zfill(sb + OFF_K + (stage * BNK + r) * PITCH + c * 16, kp + tok * p.k_sn + c * 8, ok);
+            cp_async16_zfill(sb + OFF_V + (stage * BNK + r) * PITCH + c * 16, vp + tok * p.v_sn + c * 8, ok);
+        }
+    };
+    load_kv(t0, 0);
+    cp_async_commit();
+
+    float o[32][4];
+#pragma unroll
+    for (int i = 0; i < 32; ++i)
+#pragma unroll
+        for (int z = 0; z < 4; ++z) o[i][z] = 0.f;
+    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+    float *smax = reinterpret_cast<float *>(smem + OFF_MAX);
+    const uint32_t a_base = sb + OFF_Q + (rg * 16 + (lane & 15)) * PITCH + (lane >> 4) * 16;
+    const int brow = ((lane >> 4) << 3) + (lane & 7), bhalf = (lane >> 3) & 1;
+    const int vkey = ((lane >> 3) & 1) * 8 + (lane & 7), vsel = lane >> 4;
+    const uint32_t p_base = sb + OFF_P + (rg * 16 + (lane & 15)) * P_PITCH + (lane >> 4) * 16;
+
+    for (int t = t0; t < t1; ++t) {
+        const int stage = (t - t0) & 1;
+        if (t + 1 < t1) load_kv(t + 1, stage ^ 1);
+        cp_async_commit();
+        cp_async_wait<1>();
+        __syncthreads();
+        // ---- S = Q K^T: rows 16 rg .. +15 x keys 16 kh .. +15 of the block, over all 512 channels
+        float s[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
+        {
+            const uint32_t b_base = sb + OFF_K + (stage * BNK + kh * 16 + brow) * PITCH + bhalf * 16;
+#pragma unroll 8
+            for (int kk = 0; kk < D / 16; ++kk) {
+                uint32_t a[4], b0, b1, b2, b3;
+                ldmatrix_x4(a_base + kk * 32, a[0], a[1], a[2], a[3]);
+                ldmatrix_x4(b_base + kk * 32, b0, b1, b2, b3);
+                mma_m16n8k16<T>(s[0], a, b0, b1);
+                mma_m16n8k16<T>(s[1], a, b2, b3);
+            }
+        }
+        const int k0 = t * BNK + kh * 16;
+        if (k0 + 16 > p.Nk) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int key = k0 + i * 8 + 2 * tq;
+                if (key >= p.Nk) { s[i][0] = -INFINITY; s[i][2] = -INFINITY; }
+                if (key + 1 >= p.Nk) { s[i][1] = -INFINITY; s[i][3] = -INFINITY; }
+            }
+        }
+#pragma unroll
+        for (int h2 = 0; h2 < 2; ++h2) {
+            float mx = fmaxf(fmaxf(s[0][2 * h2], s[0][2 * h2 + 1]), fmaxf(s[1][2 * h2], s[1][2 * h2 + 1]));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+            if (tq == 0) smax[kh * BM + rg * 16 + g + 8 * h2] = mx;
+        }
+        __syncthreads();
+        // ---- online softmax over the whole block (both key halves): both warps of a row group see the same maximum
+#pragma unroll
+        for (int h2 = 0; h2 < 2; ++h2) {
+            const int row = rg * 16 + g + 8 * h2;
+            const float m_new = fmaxf(m[h2], fmaxf(smax[row], smax[BM + row]));     // finite: key t * BNK is real
+            const float corr = fast_exp2((m[h2] - m_new) * p.scale_log2e);
+            const float mb = m_new * p.scale_log2e;
+            m[h2] = m_new;
+            float sum = 0.f;
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const float e0 = fast_exp2(fmaf(s[i][2 * h2], p.scale_log2e, -mb)), e1 = fast_exp2(fmaf(s[i][2 * h2 + 1], p.scale_log2e, -mb));
+                sum += e0 + e1;
+                *reinterpret_cast<uint32_t *>(smem + OFF_P + row * P_PITCH + (kh * 16 + i * 8 + 2 * tq) * 2) = pack2<T>(e0, e1);
+            }
+            l[h2] = fmaf(l[h2], corr, sum);
+#pragma unroll
+            for (int i = 0; i < 32; ++i) { o[i][2 * h2] *= corr; o[i][2 * h2 + 1] *= corr; }
+        }
+        __syncthreads();
+        // ---- O += P V: rows 16 rg .. +15 x channels 256 kh .. +255, all 32 keys of the block
+        {
+            const uint32_t v_base = sb + OFF_V + (stage * BNK + vkey) * PITCH + vsel * 16 + kh * 512;
+#pragma unroll
+            for (int kk = 0; kk < BNK / 16; ++kk) {
+                uint32_t a[4];
+                ldmatrix_x4(p_base + kk * 32, a[0], a[1], a[2], a[3]);
+#pragma unroll
+                for (int n2 = 0; n2 < 16; ++n2) {
+                    uint32_t b0, b1, b2, b3;
+                    ldmatrix_x4_trans(v_base + kk * 16 * PITCH + n2 * 32, b0, b1, b2, b3);
+                    mma_m16n8k16<T>(o[2 * n2], a, b0, b1);
+                    mma_m16n8k16<T>(o[2 * n2 + 1], a, b2, b3);
+                }
+            }
+        }
+        __syncthreads();                  // the stage, P and the maxima are rewritten by the next block
+    }
+    cp_async_wait<0>();
+
+    // ---- this CTA's partial: unnormalised O (fp32) over the ring, (max, sum) per row
+    float *so = reinterpret_cast<float *>(smem + OFF_O);
+    float *sl = reinterpret_cast<float *>(smem + OFF_L);
+#pragma unroll
+    for (int h2 = 0; h2 < 2; ++h2) {
+        const int row = rg * 16 + g + 8 * h2;
+        float sum = l[h2];
+        sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+        sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+        if (tq == 0) sl[kh * BM + row] = sum;
+#pragma unroll
+        for (int i = 0; i < 32; ++i)
+            *reinterpret_cast<float2 *>(so + row * O_PITCH + kh * 256 + i * 8 + 2 * tq) = make_float2(o[i][2 * h2], o[i][2 * h2 + 1]);
+        if (kh == 0 && tq == 0) smax[row] = m[h2];
+    }
+    __syncthreads();
+    float2 *sml = reinterpret_cast<float2 *>(smem + OFF_ML);
+    if (tid < BM) sml[tid] = make_float2(smax[tid], sl[tid] + sl[BM + tid]);
+    if (cs > 1) cluster.sync(); else __syncthreads();   // every peer's partial has landed
+
+    // ---- merge: out = sum_c 2^((m_c - M) c) O_c / sum_c 2^((m_c - M) c) l_c, peers in rank order
+    float *sw = reinterpret_cast<float *>(smem + OFF_W);
+    if (tid < BM) {
+        auto peer = [&](int c) { return *(c == rank ? sml + tid : cluster.map_shared_rank(sml + tid, c)); };
+        float M = -INFINITY;
+        for (int c = 0; c < cs; ++c) M = fmaxf(M, peer(c).x);
+        float L = 0.f;
+        for (int c = 0; c < cs; ++c) {
+            const float2 ml = peer(c);
+            const float e = fast_exp2((ml.x - M) * p.scale_log2e);
+            sw[c * BM + tid] = e;
+            L = fmaf(e, ml.y, L);
+        }
+        const float inv = 1.f / L;
+        for (int c = 0; c < cs; ++c) sw[c * BM + tid] *= inv;
+    }
+    __syncthreads();
+    const int cw = D / cs;                            // output channels this CTA reduces
+    T *op = reinterpret_cast<T *>(p.out) + b * p.o_sb + h * p.o_sh;
+    for (int i = tid; i < BM * (cw / 4); i += NTHREADS) {
+        const int row = i / (cw / 4), col = rank * cw + (i - row * (cw / 4)) * 4;
+        if (q0 + row >= p.Nq) continue;
+        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int c = 0; c < cs; ++c) {
+            const float *src = so + row * O_PITCH + col;
+            const float4 x = *reinterpret_cast<const float4 *>(c == rank ? src : cluster.map_shared_rank(src, c));
+            const float w = sw[c * BM + row];
+            acc.x = fmaf(w, x.x, acc.x); acc.y = fmaf(w, x.y, acc.y); acc.z = fmaf(w, x.z, acc.z); acc.w = fmaf(w, x.w, acc.w);
+        }
+        uint2 pk;
+        pk.x = pack2<T>(acc.x, acc.y);
+        pk.y = pack2<T>(acc.z, acc.w);
+        *reinterpret_cast<uint2 *>(op + (long long)(q0 + row) * p.o_sn + col) = pk;
+    }
+    if (cs > 1) cluster.sync();                       // the peers' shared memory is read up to here
+}
+
+// Cluster size: the smallest power of two that puts about one CTA on every SM, at most one key block per CTA and 8.
+template <typename T> static int launch(const Params &p, int BH, cudaStream_t stream) {
+    static int attr_dev = -1;
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (attr_dev != dev) {
+        if (cudaFuncSetAttribute(kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, TOTAL) != cudaSuccess) {
+            set_error("sige_sparse_attention: cannot reserve %d bytes of shared memory", TOTAL);
+            (void)cudaGetLastError();
+            return 2;
+        }
+        attr_dev = dev;
+    }
+    const long long ctas = (long long)ceil_div(p.Nq, BM) * BH;
+    const int nblk = ceil_div(p.Nk, BNK);
+    int cs = 1;
+    while (cs < MAX_CS && 2 * cs <= nblk && ctas * cs < sm_count()) cs *= 2;
+    const dim3 grid(ceil_div(p.Nq, BM), cs, BH);
+    if (launch_ex(kernel<T>, grid, dim3(NTHREADS), TOTAL, stream, false, dim3(1, cs, 1), p, cs) != cudaSuccess) {
+        set_error("sige_sparse_attention: launch of the D = 512 kernel (cluster %d) failed: %s", cs, cudaGetErrorString(cudaGetLastError()));
+        return 2;
+    }
+    return check_launch("sige_sparse_attention");
+}
+}  // namespace wide
+
 template <typename T> static int dispatch(const Params &p, int BH, int D, cudaStream_t stream) {
     switch (D) {
         case 32: return launch<T, 32>(p, BH, stream);
@@ -229,8 +475,9 @@ template <typename T> static int dispatch(const Params &p, int BH, int D, cudaSt
         case 80: return launch<T, 80>(p, BH, stream);
         case 128: return launch<T, 128>(p, BH, stream);
         case 160: return launch<T, 160>(p, BH, stream);
+        case 512: return wide::launch<T>(p, BH, stream);
     }
-    set_error("sige_sparse_attention: head dim %d is not one of 32, 40, 64, 80, 128, 160", D);
+    set_error("sige_sparse_attention: head dim %d is not one of 32, 40, 64, 80, 128, 160, 512", D);
     return 1;
 }
 
@@ -238,7 +485,7 @@ template <typename T> static int dispatch(const Params &p, int BH, int D, cudaSt
 }  // namespace sige
 
 extern "C" int sige_sparse_attention_supported(int D, int dtype) {
-    return ((D == 32 || D == 40 || D == 64 || D == 80 || D == 128 || D == 160) && (dtype == SIGE_F16 || dtype == SIGE_BF16)) ? 1 : 0;
+    return ((D == 32 || D == 40 || D == 64 || D == 80 || D == 128 || D == 160 || D == 512) && (dtype == SIGE_F16 || dtype == SIGE_BF16)) ? 1 : 0;
 }
 
 extern "C" int sige_sparse_attention(const sige_sparse_attention_t *a, sige_stream_t stream_) {
@@ -247,7 +494,7 @@ extern "C" int sige_sparse_attention(const sige_sparse_attention_t *a, sige_stre
     SIGE_REQUIRE(a, "sige_sparse_attention: null descriptor");
     SIGE_REQUIRE(a->B >= 0 && a->heads >= 1 && a->Nq >= 0 && a->Nk >= 1, "sige_sparse_attention: B = %d, heads = %d, Nq = %d, Nk = %d", a->B, a->heads,
                  a->Nq, a->Nk);
-    SIGE_REQUIRE(sige_sparse_attention_supported(a->D, a->dtype), "sige_sparse_attention: unsupported head dim %d (32, 40, 64, 80, 128, 160) / dtype %d (f16, bf16)",
+    SIGE_REQUIRE(sige_sparse_attention_supported(a->D, a->dtype), "sige_sparse_attention: unsupported head dim %d (32, 40, 64, 80, 128, 160, 512) / dtype %d (f16, bf16)",
                  a->D, a->dtype);
     // scale = 0 makes the last-block mask -inf * 0 = NaN; scale < 0 takes the running maximum at the wrong end
     SIGE_REQUIRE(a->scale > 0.f && isfinite(a->scale), "sige_sparse_attention: scale = %g must be positive and finite", (double)a->scale);

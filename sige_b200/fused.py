@@ -725,10 +725,11 @@ class WinStack(Stack):
 
 
 class RealStack:
-    """A materialised tile stack (B*N, C, R, S) produced by an eager node."""
+    """A materialised tile stack (B*N, C, R, S) produced by an eager node, or one row per entry of a fixed-capacity tile list
+    (`slot`: the sparse-attention core's output) — scattered through that list."""
 
-    def __init__(self, tensor: torch.Tensor):
-        self.tensor = tensor
+    def __init__(self, tensor: torch.Tensor, slot: Optional["IdxSlot"] = None):
+        self.tensor, self.slot = tensor, slot
 
 
 class ConvOut:
@@ -959,6 +960,7 @@ class Lowering:
         self.pdl, self.tc5, self.producer_preop, self.fuse_shortcut = pdl, tc5, producer_preop, fuse_shortcut
         self.fused_attention, self.sparse_stem, self.ksplit = fused_attention, sparse_stem, ksplit
         self.sparse_attention_calls = 0
+        self._consumers: Optional[Dict[int, Node]] = None       # LazyTensor id -> first node that reads it (_sole_consumer)
         self.spade_calls = 0
         self.separable: List[SepLaunch] = []
         self._nhwc_stacks: Dict[int, torch.Tensor] = {}
@@ -2019,7 +2021,7 @@ class Lowering:
     def _tile_emit(self, node: Node, co: ConvOut, dst: Buf, residual: Optional[Buf] = None, shortcut=None, name: str = "", gather=None) -> None:
         segs, pre, hw, idx, block, off, stack_src, timg = self.tile_conv_args(co)
         if stack_src is not None and gather is not None:      # a materialised stack scattered through `gather`'s tile set
-            idx, off = gather.active_indices.to(self.dev), int(gather.offset[0])
+            idx, off = co.src.slot.buf if co.src.slot is not None else gather.active_indices.to(self.dev), int(gather.offset[0])
         self.emit_conv(name or ("n%d" % node.index), segs, pre, hw, idx, block, co.weight, co.bias, co.stride, off, dst, residual=residual,
                        shortcut=shortcut, stack_src=stack_src, tile_img=timg, cin_pad=co.cin_pad, epilogue=co.act, window=self._window_of(co))
 
@@ -2060,7 +2062,8 @@ class Lowering:
         g = m.gather.module
         if isinstance(co.src, Stack) and not self._same_gather(co.src.gather, g):
             return False
-        if isinstance(co.src, RealStack) and (int(co.src.tensor.shape[2]) != int(g.block_size[0]) or g.block_size[0] != g.block_size[1]):
+        if isinstance(co.src, RealStack) and (int(co.src.tensor.shape[2]) != int(g.block_size[0]) or g.block_size[0] != g.block_size[1]
+                                              or (co.src.slot is not None and co.src.slot is not self.slots.get(id(g.active_indices)))):
             return False
         res_buf = None
         if residual is not None:
@@ -2503,6 +2506,8 @@ class Lowering:
         return False
 
     def _h_bmm(self, node: Node):
+        if self._tile_attention(node):
+            return True
         a, b = self.sym(node.args[0]), self.sym(node.args[1])
         if isinstance(a, Tok) and isinstance(b, Tok) and a.layout == "bnc" and b.layout == "bcn":
             self.env[id(node.outs[0])] = Scores(a.sl, b.sl)
@@ -2526,6 +2531,100 @@ class Lowering:
         if isinstance(a, GScores) and a.probs and self.n_uses(node.args[0]) == 1 and node.args[1].dim() == 3:
             return self._emit_sdpa(node, a, node.args[1])
         return False
+
+    def _sole_consumer(self, lt: LazyTensor, name: Tuple[str, ...]) -> Optional[Node]:
+        """The one node that reads `lt`, if it is one of `name`."""
+        if self._consumers is None:
+            self._consumers = {}
+
+            def note(o, n):
+                if isinstance(o, LazyTensor):
+                    self._consumers.setdefault(id(o), n)
+                return o
+
+            for n in self.tape.nodes:
+                lazy._tree_map(lambda o, n=n: note(o, n), n.args)
+                lazy._tree_map(lambda o, n=n: note(o, n), n.kwargs)
+        n = self._consumers.get(id(lt)) if self.n_uses(lt) == 1 else None
+        return n if n is not None and n.name in name else None
+
+    def _tile_attention(self, node: Node) -> bool:
+        """SIGEAttnBlock's core in sparse mode (reference stable-diffusion/ldm/modules/diffusionmodules/model.py:180-252, the VAE's
+        mid block): the queries are the q conv's tile stack as tokens (reshape -> permute -> reshape: tile-major, then pixel order),
+        the keys and values the full k / v maps that k_scatter / v_scatter paste together:
+            bmm(q, k.reshape(b, c, hw)) * c^-0.5 -> softmax(2) -> bmm(v.reshape(b, c, hw), . .permute(0, 2, 1))
+            -> reshape(b, c, tiles, bs, bs) -> permute(0, 2, 1, 3, 4) -> reshape(-1, c, bs, bs) -> proj_out -> out_scatter.
+        Recognised at the first bmm, with every later node of the chain checked on the tape; then ONE `sige_sparse_attention`
+        launch reads the q stack (written by the q conv's launch over the fixed-capacity tile list) and the k / v buffers in place
+        (token stride C) and writes the NHWC tile stack that proj_out reads — padding tiles' rows are computed and never scattered.
+        Anything else keeps the recorded calls."""
+        qa, kb = node.args[0], node.args[1]
+        if not (isinstance(qa, LazyTensor) and isinstance(kb, LazyTensor) and qa.dim() == 3 and kb.dim() == 3 and qa.shape[0] == 1):
+            return False
+        # queries: reshape(1, tiles * bs * bs, c) <- permute(0, 1, 3, 2) <- reshape(1, tiles, c, bs * bs) <- 1x1 conv on the tiles
+        q3 = qa
+        p3 = q3.node.args[0] if q3.node is not None and q3.node.name in ("reshape", "view") else None
+        r4 = p3.node.args[0] if isinstance(p3, LazyTensor) and p3.node is not None and p3.node.name == "permute" else None
+        qc = r4.node.args[0] if isinstance(r4, LazyTensor) and r4.node is not None and r4.node.name in ("reshape", "view") else None
+        co = self.sym(qc) if isinstance(qc, LazyTensor) else None
+        if not (isinstance(co, ConvOut) and isinstance(co.src, Stack) and not isinstance(co.src, (ModStack, WinStack)) and co.k == 1
+                and co.stride == 1 and co.act is None and co.cin_pad == 0 and all(self.n_uses(t) == 1 for t in (q3, p3, r4, qc))):
+            return False
+        g = co.src.gather
+        bs = int(g.block_size[0])
+        nt, C = int(qc.shape[0]), int(qc.shape[1])
+        if (tuple(g.block_size) != (bs, bs) or tuple(qc.shape[2:]) != (bs, bs) or tuple(r4.shape) != (1, nt, C, bs * bs)
+                or tuple(int(d) for d in p3.node.args[1:]) != (0, 1, 3, 2) or tuple(q3.shape) != (1, nt * bs * bs, C)
+                or getattr(g, "tile_images", None) is not None or int(g.active_indices.shape[0]) != nt or nt == 0):
+            return False
+
+        def full_tokens(t):          # reshape(1, c, h * w) of a plain single-buffer map
+            if not (t.node is not None and t.node.name in ("reshape", "view") and self.n_uses(t) == 1):
+                return None
+            f = self.sym(t.node.args[0])
+            buf = f.single if isinstance(f, Full) else None
+            if buf is None or tuple(buf.shape[:2]) != (1, C) or tuple(t.shape) != (1, C, buf.shape[2] * buf.shape[3]):
+                return None
+            return buf
+
+        kbuf = full_tokens(kb)
+        # the rest of the chain
+        mul = self._sole_consumer(node.outs[0], ("mul",))
+        scale = mul.args[1] if mul is not None and len(mul.args) == 2 and mul.args[0] is node.outs[0] and not mul.kwargs else None
+        sm = self._sole_consumer(mul.outs[0], ("softmax",)) if isinstance(scale, (int, float)) else None
+        if sm is None:
+            return False
+        a = self._bind(sm, ("input", "dim"), {"dim": None})
+        pt = self._sole_consumer(sm.outs[0], ("permute",)) if a["dim"] in (2, -1) and a.get("dtype") is None else None
+        bmm2 = self._sole_consumer(pt.outs[0], ("bmm",)) if pt is not None and tuple(int(d) for d in pt.args[1:]) == (0, 2, 1) else None
+        vbuf = full_tokens(bmm2.args[0]) if bmm2 is not None and bmm2.args[1] is pt.outs[0] else None
+        o5 = self._sole_consumer(bmm2.outs[0], ("reshape", "view")) if vbuf is not None else None
+        o5p = self._sole_consumer(o5.outs[0], ("permute",)) if o5 is not None and tuple(o5.outs[0].shape) == (1, C, nt, bs, bs) else None
+        o4 = (self._sole_consumer(o5p.outs[0], ("reshape", "view"))
+              if o5p is not None and tuple(int(d) for d in o5p.args[1:]) == (0, 2, 1, 3, 4) else None)
+        if (o4 is None or tuple(o4.outs[0].shape) != (nt, C, bs, bs) or kbuf is None or tuple(vbuf.shape) != tuple(kbuf.shape)
+                or not (float(scale) > 0 and self.ex.sparse_attention_supported(C))):
+            return False
+        # q: the conv's launch over the fixed-capacity list writes a capacity-row NHWC stack
+        segs, pre, hw, idx, block, off, stack_src, timg = self.tile_conv_args(co)
+        sl = self.slots.get(id(g.active_indices))
+        if stack_src is not None or timg is not None or sl is None or idx is not sl.buf or segs[0][0].shape[0] != 1:
+            return False
+        cap = int(idx.shape[0])
+        q_st = torch.empty((cap, C, bs, bs), dtype=self.dtype, device=self.dev, memory_format=torch.channels_last)
+        self.emit_conv("n%d.q_stack" % co.node.index, segs, pre, hw, idx, block, co.weight, co.bias, co.stride, off, None, dst_stack=q_st)
+        o_st = torch.empty_like(q_st)
+
+        def tokens(t):               # [1, 1, tokens, C] view of an NHWC map or stack
+            return t.permute(0, 2, 3, 1).reshape(1, -1, C).unsqueeze(1)
+
+        for buf in (kbuf, vbuf):
+            buf.readers.append(None)
+        self.steps.append(("sparse_attention", self.ex.prepare_sparse_attention(tokens(q_st), tokens(kbuf.raw), tokens(vbuf.raw), float(scale),
+                                                                                 tokens(o_st))))
+        self.sparse_attention_calls += 1
+        self.env[id(o4.outs[0])] = RealStack(o_st, slot=sl)
+        return True
 
     def _emit_sdpa(self, node: Node, g: GScores, v: LazyTensor) -> bool:
         def rt(t):
