@@ -376,6 +376,8 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
             hh += (p.offH + __ldg(p.idx + 2 * nn)) / p.stride;
             ww += (p.offW + __ldg(p.idx + 2 * nn + 1)) / p.stride;
             img = t / p.N;
+        } else if (p.idx && __ldg(p.idx + 2 * (t % p.N)) <= SIGE_TILE_NONE) {
+            continue;                                  // a padding entry of the list writes nothing to its stack row
         }
         if (hh < 0 || hh >= p.dH || ww < 0 || ww >= p.dW) continue;
         float v[8];

@@ -523,6 +523,8 @@ tile_conv_tc5_kernel(const __grid_constant__ Params p, const __grid_constant__ C
                 hh += p.offH + s_idx[2 * tl];
                 ww += p.offW + s_idx[2 * tl + 1];
             }
+        } else if (p.idx && s_idx[2 * tl] <= SIGE_TILE_NONE) {
+            return -1;                                 // a padding entry of the list writes nothing to its stack row
         }
         if (hh < 0 || hh >= p.dH || ww < 0 || ww >= p.dW) return -1;
         return ((long long)img * p.dH + hh) * p.dW + ww;

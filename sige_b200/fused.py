@@ -1029,9 +1029,8 @@ class Lowering:
         """Does the executor's one-launch cache load (`sige_cache_load`) fill this cached buffer?"""
         return self.cache_load is not None and self.cache_load(buf.cached_init)
 
-    def load_caches(self, stream: int) -> None:
-        """Every cached buffer (raw copy and transformed views) from its cache, as the step starts a new edit: one
-        `sige_cache_load` for the caches the executor takes, the torch chain (`Buf.restore`) for the others."""
+    def prepared_loader(self):
+        """(the prepared `sige_cache_load` or None, the cached buffers it does not take), prepared once per set of caches."""
         if self.loader is None:
             entries, rest = [], []
             for b in self.cached_bufs:
@@ -1040,7 +1039,12 @@ class Lowering:
                 elif b.has_raw or b.view_inits:
                     entries.append((b.cached_init, b._raw, [(v, sc, sh, act) for (v, sc, sh, act) in b.view_inits]))
             self.loader = (self.ex.prepare_cache_load(entries) if entries else None, rest)
-        run, rest = self.loader
+        return self.loader
+
+    def load_caches(self, stream: int) -> None:
+        """Every cached buffer (raw copy and transformed views) from its cache, as the step starts a new edit: one
+        `sige_cache_load` for the caches the executor takes, the torch chain (`Buf.restore`) for the others."""
+        run, rest = self.prepared_loader()
         if run is not None:
             run(stream)
         for b in rest:

@@ -11,7 +11,10 @@ and what the launches leave for each other:
     outputs, attention and tail buffers, tile lists, shortcut flags and the module caches, deduplicated by storage.
   * `walk(step, program)` runs the program one entry at a time: the expectation of the entry's record in float64 from the live
     tensors, a snapshot of the whole state, the launch, a synchronise; every element the record writes within its bound and
-    every other byte of the whole state bitwise unchanged.  Recorded torch calls and copies (`eager`) run unchecked.
+    every other byte of the whole state bitwise unchanged.  Recorded torch calls and copies (`eager`) run unchecked.  Before
+    it, every padding row of a fixed-capacity stack (`poison_padding`) is NaN: a launch that reads one shows NaN in a live
+    element, one that writes one a stray byte.
+  * `walk_loads(step)` checks the cache load of a new edit (`sige_cache_load`) the same way.
 
 The restatements read the records (ConvSpec, ConvInRec, the tail / attention / SPADE arguments, write-back entries), never the C
 descriptors, so a translation error of the executor shows as a wrong element or a stray write of the launch that made it.
@@ -79,6 +82,9 @@ class RecordingMixin:
 
     def prepare_writeback(self, entries):
         return self._keep("writeback", super().prepare_writeback(entries), list(entries))
+
+    def prepare_cache_load(self, entries):
+        return self._keep("cache_load", super().prepare_cache_load(entries), [(src, raw, list(views)) for (src, raw, views) in entries])
 
     def record_of(self, kind: str, fn):
         if kind == "conv":
@@ -163,7 +169,7 @@ class State:
             _buf_tensors(rec.out, ts)
             add("conv_in", ts)
         for rec in low.separable:
-            ts = [rec.src, rec.idx]
+            ts = [rec.src, rec.idx, rec.tile_img]
             for br in rec.branches:
                 _buf_tensors(br[3], ts)
             add(rec.name, ts)
@@ -172,7 +178,7 @@ class State:
         outs: List[torch.Tensor] = []
         _tensors(step.outputs, outs)
         add("output", outs)
-        add("tile list", [sl.buf for sl in low.slots.values()])
+        add("tile list", [sl.buf for sl in low.slots.values()] + [sl.tile_img for sl in low.slots.values()])
         add("shortcut flags", [r[0] for r in low.flag_recipes])
         for kind, rec, _fn in getattr(step.ex, "records", {}).values():
             ts = []
@@ -193,6 +199,22 @@ class State:
                 continue
             b = torch.empty(0, dtype=torch.uint8, device=t.device).set_(st, 0, (st.nbytes(),), (1,))
             self.storages[key] = Storage(name, b)
+
+    def holds(self, t: torch.Tensor) -> bool:
+        return _key(t) in self.storages
+
+    def assert_complete(self, step) -> None:
+        """Every per-edit tensor a launch could wrongly write is part of the state: the tile lists and their image indices, the
+        separable launches' image indices, the stacks of the attention chain (the q and o stacks of a sparse attention)."""
+        low = step.low
+        want = [("tile list", sl.buf) for sl in low.slots.values()]
+        want += [("tile_img of a tile list", sl.tile_img) for sl in low.slots.values() if sl.tile_img is not None]
+        want += [("tile_img of %s" % r.name, r.tile_img) for r in low.separable if r.tile_img is not None]
+        for kind, rec, _fn in getattr(step.ex, "records", {}).values():
+            if kind == "sparse_attention":
+                want += [("sparse attention q", rec["q"]), ("sparse attention out", rec["out"])]
+        for what, t in want:
+            assert self.holds(t), "the step's state misses the %s" % what
 
     @property
     def nbytes(self) -> int:
@@ -216,6 +238,43 @@ def _key(t: torch.Tensor):
     return (t.device.type, t.untyped_storage().data_ptr())
 
 
+def padded_stacks(step) -> Dict[Tuple[str, int], Tuple[torch.Tensor, torch.Tensor]]:
+    """Per storage: (stack [cap, C, h, w], its fixed-capacity list [cap, 2]) of every stack a launch writes or reads row for row
+    through a one-edit list (row r is the tile of list entry r): the rows of SIGE_TILE_NONE entries belong to no tile."""
+    out = {}
+    for fc in list(step.low.fused) + list(step.low.epilogue_fused):
+        s = fc.spec
+        if s.idx is None or s.tile_img is not None or s.B != 1:
+            continue
+        for t in ([s.dst_stack] if s.dst_stack is not None else []) + ([s.srcs[0][0]] if s.src_is_stack else []):
+            if t.shape[0] == s.idx.shape[0]:
+                out[_key(t)] = (t, s.idx)
+    return out
+
+
+def poison_padding(step) -> int:
+    """NaN into every row of a padded stack whose list entry is SIGE_TILE_NONE, so that a launch that reads one shows as NaN in a
+    live element, or writes one as a stray byte.  Returns the number of rows poisoned."""
+    n = 0
+    with torch.no_grad():
+        for t, idx in padded_stacks(step).values():
+            pad = (idx[:, 0] <= NONE_BELOW).to(t.device)
+            t[pad] = float("nan")
+            n += int(pad.sum())
+    return n
+
+
+def live_tokens(step, t: torch.Tensor) -> Optional[torch.Tensor]:
+    """bool [tokens] of a token view of a padded stack (row r: tokens r*h*w ..): the tokens of real tiles; None for another tensor."""
+    hit = padded_stacks(step).get(_key(t))
+    if hit is None:
+        return None
+    stack, idx = hit
+    per = int(stack.shape[2] * stack.shape[3])
+    assert t.data_ptr() == stack.data_ptr() and t.shape[-2] == stack.shape[0] * per
+    return (idx[:, 0] > NONE_BELOW).to(t.device).repeat_interleave(per)
+
+
 # ----------------------------------------------------------------------------------------------------------------------
 # expectations
 # ----------------------------------------------------------------------------------------------------------------------
@@ -229,6 +288,8 @@ class Want:
     written: torch.Tensor
     bound: torch.Tensor
     rounding: torch.Tensor
+    free: Optional[torch.Tensor] = None      # elements the launch may leave with any value (rows of no tile)
+    exact: Optional[torch.Tensor] = None     # the written tensor's exact contents in its dtype: compared bit for bit
 
 
 def _from_expects(expects: List[kc.Expect]) -> List[Want]:
@@ -460,14 +521,22 @@ def attention_expect(r, dtype) -> List[Want]:
     return _from_expects(kc.attn_reference(case))
 
 
-def sparse_attention_expect(r, dtype) -> List[Want]:
+def sparse_attention_expect(r, dtype, live: Optional[torch.Tensor] = None) -> List[Want]:
+    """live: bool [Nq], the queries of real tiles (None: all).  Every live query within its bound; the others (rows of padding
+    tiles) may be left with any value."""
     q, k, v, out = r["q"], r["k"], r["v"], r["out"]
     if q.dim() == 3:
         q, k, v, out = q.unsqueeze(1), k.unsqueeze(1), v.unsqueeze(1), out.unsqueeze(1)
     B, Hh, Nq, D = q.shape
     spec = skc.SAttnSpec("sparse_attention", B, Hh, Nq, int(k.shape[2]), D, scale=float(r["scale"]))
     case = skc.SAttnCase(spec, dtype, q, k, v, {}, _live(out, "bhnd"), out)
-    return _from_expects(skc.sattn_reference(case))
+    sms = torch.cuda.get_device_properties(q.device).multi_processor_count if q.device.type == "cuda" else kc.H100_SMS
+    (w,) = _from_expects(skc.wide_sattn_reference(case, sms=sms) if D == skc.WIDE_D else skc.sattn_reference(case))
+    if live is not None:
+        dead = (~live.to(q.device)).view(1, 1, Nq, 1).expand(B, Hh, Nq, D).reshape(-1)
+        w.free = dead & w.written
+        w.written = w.written & ~dead
+    return [w]
 
 
 class _LiveSpade(skc.SpadeCase):
@@ -508,10 +577,12 @@ def spade_expect(r, dtype) -> List[Want]:
 
 def separable_expect(rec, dtype) -> List[Want]:
     """A SepLaunch as a kernel_contracts separable case on the live tensors: the depthwise weight and bias with the record's
-    per-channel affine folded in fp32 (scale * w, scale * b + shift), the 1x1 weight in `dtype`, its fp32 bias."""
+    per-channel affine folded in fp32 (scale * w, scale * b + shift), the 1x1 weight in `dtype`, its fp32 bias.  A batch of
+    edits (`tile_img`): row m of the list is a tile of image tile_img[m] only, the per-image form of the restatement."""
     src = _nhwc(rec.src)
     idx = rec.idx
-    n = int(idx.shape[0])
+    per_image = rec.tile_img is not None
+    n = int(idx.shape[0]) // (rec.batch if per_image else 1)
     Cin, Cout = rec.Cin, rec.Cout
     dw_w, dw_b, pw_w, pw_b, dst = [], [], [], [], []
     for (dwc, w1, b1, buf) in rec.branches:
@@ -532,8 +603,8 @@ def separable_expect(rec, dtype) -> List[Want]:
     dH, dW = int(rec.branches[0][3].shape[2]), int(rec.branches[0][3].shape[3])
     spec = kc.SepSpec(rec.name, B=rec.batch, Cin=Cin, Cout=Cout, H=6 if rec.src_stack else int(src.shape[1]), W=6 if rec.src_stack else int(src.shape[2]),
                       real=n, lead=n, pre=rec.c0, post=int(src.shape[3]) - rec.c0 - Cin, src_stack=rec.src_stack, offH=rec.off, offW=rec.off,
-                      dH=dH, dW=dW, dsts=tuple(("buf", int(b_.shape[1]) - Cout, 0) for (_, _, _, b_) in rec.branches))
-    case = kc.SepCase(spec, dtype, src, idx, dw_w, dw_b, pw_w, pw_b, dst)
+                      dH=dH, dW=dW, dsts=tuple(("buf", int(b_.shape[1]) - Cout, 0) for (_, _, _, b_) in rec.branches), per_image=per_image)
+    case = kc.SepCase(spec, dtype, src, idx, dw_w, dw_b, pw_w, pw_b, dst, rec.tile_img)
     return _from_expects(kc.sep_reference(case))
 
 
@@ -562,8 +633,38 @@ def writeback_expect(entries, dtype) -> List[Want]:
     return out
 
 
+def cached_view(c: torch.Tensor, sc, sh, act: str, dtype) -> Tuple[torch.Tensor, torch.Tensor]:
+    """float64 act(cache * scale + shift) of a producer-written view of a cached buffer, and its bound: the fp32 affine and
+    activation (4 fp32 roundings of |cache * scale| + |shift| through the activation), the rounding to `dtype`."""
+    z = c.double()
+    if sc is not None:
+        z = z * sc.double().view(1, -1, 1, 1)
+    if sh is not None:
+        z = z + sh.double().view(1, -1, 1, 1)
+    want = _act(z, act)
+    lin = c.double().abs() * (1 if sc is None else sc.double().abs().view(1, -1, 1, 1)) + (0 if sh is None else sh.double().abs().view(1, -1, 1, 1))
+    return want, _u(dtype) * want.abs() + SWISH_LIP * 4 * 2.0 ** -24 * lin + ABS
+
+
+def cache_load_expect(entries, dtype) -> List[Want]:
+    """sige_cache_load: each raw buffer the cache in `dtype` broadcast over the buffer's images, bitwise; each view
+    act(cache * scale + shift) within cached_view's bound."""
+    out = []
+    for i, (src, raw, views) in enumerate(entries):
+        if raw is not None:
+            exact = src.to(raw.device).to(dtype).expand(raw.shape)
+            z = torch.zeros(raw.shape, dtype=torch.float64, device=raw.device)
+            out.append(Want("raw%d" % i, raw, exact.double(), torch.ones(raw.shape, dtype=torch.bool, device=raw.device), z, z, exact=exact))
+        for j, (v, sc, sh, act) in enumerate(views):
+            want, bound = cached_view(src.to(v.device), sc, sh, act, dtype)
+            want, bound = want.expand(v.shape), bound.expand(v.shape)
+            out.append(Want("view%d.%d" % (i, j), v, want, torch.ones(v.shape, dtype=torch.bool, device=v.device), bound, _u(dtype) * want.abs()))
+    return out
+
+
 EXPECT = {"conv": conv_expect, "conv_in": conv_in_expect, "tail": tail_expect, "attention": attention_expect,
-          "sparse_attention": sparse_attention_expect, "spade": spade_expect, "separable": separable_expect, "writeback": writeback_expect}
+          "sparse_attention": sparse_attention_expect, "spade": spade_expect, "separable": separable_expect, "writeback": writeback_expect,
+          "cache_load": cache_load_expect}
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -579,7 +680,7 @@ def _allowed(state: State, wants: List[Want]) -> Dict[Tuple[str, int], torch.Ten
         nb = state.storages[key].bytes.numel()
         es = t.element_size()
         elem = torch.zeros(nb // es, dtype=torch.bool, device=t.device)
-        elem.as_strided(t.shape, t.stride(), t.storage_offset())[w.written] = True
+        elem.as_strided(t.shape, t.stride(), t.storage_offset())[w.written if w.free is None else (w.written | w.free)] = True
         byte = elem.view(-1, 1).expand(-1, es).reshape(-1)
         out[key] = byte if key not in out else (out[key] | byte)
     return out
@@ -597,6 +698,12 @@ class KindStats:
 def _check_values(label: str, wants: List[Want]) -> Tuple[float, float]:
     worst = excess = 0.0
     for w in wants:
+        if w.exact is not None:
+            same = kc.bits(w.tensor.contiguous()) == kc.bits(w.exact.contiguous())
+            if not bool(same.all()):
+                pos = tuple(int(z) for z in (~same).nonzero()[0])
+                raise AssertionError("%s: %s at %s of %s: got %r, want %r bit for bit; %d elements differ"
+                                     % (label, w.name, pos, tuple(w.tensor.shape), float(w.tensor[pos]), float(w.exact[pos]), int((~same).sum())))
         m = w.written
         if not bool(m.any()):
             continue
@@ -622,12 +729,38 @@ def _sync(dev) -> None:
         torch.cuda.synchronize(dev)
 
 
+def _check_launch(state: State, kinds: Dict[str, KindStats], kind: str, label: str, wants: List[Want], fn, stream, dev) -> None:
+    """Snapshot the whole state, launch, synchronise: nothing outside the wanted elements changed, every wanted one in bound."""
+    allowed = _allowed(state, wants)
+    snap = state.snapshot()
+    fn(stream)
+    _sync(dev)
+    for key, s in state.storages.items():
+        changed = s.bytes != snap[key]
+        if key in allowed:
+            changed &= ~allowed[key]
+        if bool(changed.any()):
+            i = int(changed.nonzero()[0])
+            raise AssertionError("%s: wrote outside its record into %s at byte %d of %d (%d stray bytes)"
+                                 % (label, s.name, i, s.bytes.numel(), int(changed.sum())))
+    r, x = _check_values(label, wants)
+    ks = kinds.setdefault(kind, KindStats())
+    ks.launches += 1
+    if r >= ks.worst:
+        ks.worst, ks.worst_at = r, label
+    if x >= ks.excess:
+        ks.excess, ks.excess_at = x, label
+
+
 def walk(step, program=None, model=None, state: Optional[State] = None) -> Dict[str, object]:
-    """Run `program` (default: the step's main program) entry by entry, checking each against its record.  Returns
-    {"kinds": {kind: KindStats}, "eager": count, "seconds": wall time, "state_bytes": size of the whole state}."""
+    """Run `program` (default: the step's main program) entry by entry, checking each against its record, after poisoning the
+    padding rows of the step's stacks (poison_padding).  Returns {"kinds": {kind: KindStats}, "eager": count, "seconds": wall
+    time, "state_bytes": size of the whole state, "poisoned": padding rows poisoned}."""
     program = step.steps if program is None else program
     ex = step.ex
     state = state or State(step, model)
+    state.assert_complete(step)
+    poisoned = poison_padding(step)
     dev = step.dev
     stream = torch.cuda.current_stream(dev).cuda_stream if dev.type == "cuda" else 0
     kinds: Dict[str, KindStats] = {}
@@ -644,33 +777,40 @@ def walk(step, program=None, model=None, state: Optional[State] = None) -> Dict[
                 raise AssertionError("step %d: no restatement for launch kind %r" % (pos, kind))
             rec = ex.record_of(kind, fn)
             label = "%s launch %d (%s)" % (kind, pos, rec.name if kind in ("conv", "separable") else kind)
-            wants = conv_expect(rec, step.dtype, ex.writes_raw(fn.__self__)) if kind == "conv" else EXPECT[kind](rec, step.dtype)
-            allowed = _allowed(state, wants)
-            snap = state.snapshot()
-            fn(stream)
-            _sync(dev)
-            for key, s in state.storages.items():
-                changed = s.bytes != snap[key]
-                if key in allowed:
-                    changed &= ~allowed[key]
-                if bool(changed.any()):
-                    i = int(changed.nonzero()[0])
-                    raise AssertionError("%s: wrote outside its record into %s at byte %d of %d (%d stray bytes)"
-                                         % (label, s.name, i, s.bytes.numel(), int(changed.sum())))
-            r, x = _check_values(label, wants)
-            ks = kinds.setdefault(kind, KindStats())
-            ks.launches += 1
-            if r >= ks.worst:
-                ks.worst, ks.worst_at = r, label
-            if x >= ks.excess:
-                ks.excess, ks.excess_at = x, label
-    return {"kinds": kinds, "eager": eager, "seconds": time.perf_counter() - t0, "state_bytes": state.nbytes}
+            if kind == "conv":
+                wants = conv_expect(rec, step.dtype, ex.writes_raw(fn.__self__))
+            elif kind == "sparse_attention":
+                wants = sparse_attention_expect(rec, step.dtype, live_tokens(step, rec["q"]))
+            else:
+                wants = EXPECT[kind](rec, step.dtype)
+            _check_launch(state, kinds, kind, label, wants, fn, stream, dev)
+    return {"kinds": kinds, "eager": eager, "seconds": time.perf_counter() - t0, "state_bytes": state.nbytes, "poisoned": poisoned}
+
+
+def walk_loads(step, model=None, state: Optional[State] = None) -> Dict[str, object]:
+    """The cache load of a new edit (`Lowering.load_caches`) as a program of its own: the prepared `sige_cache_load`, checked as
+    `walk` checks a launch, then the torch restores of the cached buffers it does not take, unchecked and counted as `eager`."""
+    run, rest = step.low.prepared_loader()
+    state = state or State(step, model)
+    dev = step.dev
+    stream = torch.cuda.current_stream(dev).cuda_stream if dev.type == "cuda" else 0
+    kinds: Dict[str, KindStats] = {}
+    t0 = time.perf_counter()
+    with torch.no_grad():
+        if run is not None:
+            rec = step.ex.record_of("cache_load", run)
+            _check_launch(state, kinds, "cache_load", "cache_load launch 0 (cache_load)", cache_load_expect(rec, step.dtype), run, stream, dev)
+        for b in rest:
+            b.restore()
+        _sync(dev)
+    return {"kinds": kinds, "eager": len(rest), "seconds": time.perf_counter() - t0, "state_bytes": state.nbytes,
+            "entries": 0 if run is None else len(step.ex.record_of("cache_load", run))}
 
 
 def summary(tag: str, res) -> str:
     parts = ["%s x%d worst %.3f (%s) excess %.3f" % (k, s.launches, s.worst, s.worst_at, s.excess) for k, s in sorted(res["kinds"].items())]
-    return "[fused step contract] %s: %s; eager %d; %.2f s; state %.1f MB" % (tag, "; ".join(parts), res["eager"], res["seconds"],
-                                                                             res["state_bytes"] / 2 ** 20)
+    return "[fused step contract] %s: %s; eager %d; %d padding rows poisoned; %.2f s; state %.1f MB" % (
+        tag, "; ".join(parts), res["eager"], res.get("poisoned", 0), res["seconds"], res["state_bytes"] / 2 ** 20)
 
 
 def checked_all(step, res, program=None) -> None:
@@ -689,7 +829,6 @@ def cached_state_after_rebind(step) -> float:
     """After `rebind()`: every cached buffer's raw equals its cache in the step dtype, bitwise, and every producer-written view
     of it is within the aux bound of act(cache*scale + shift).  Returns the worst view error / bound ratio."""
     dt = step.dtype
-    u = _u(dt)
     worst = 0.0
     for b in step.low.cached_bufs:
         c = b.cached_init.to(b.raw.device if b.has_raw else step.dev)
@@ -697,16 +836,8 @@ def cached_state_after_rebind(step) -> float:
             want = c.to(dt).expand(b.shape)
             assert torch.equal(kc.bits(b.raw.contiguous()), kc.bits(want.contiguous())), "cached buffer %s differs from its cache" % (b.shape,)
         for (v, sc, sh, act) in b.view_inits:
-            z = c.double()
-            if sc is not None:
-                z = z * sc.double().view(1, -1, 1, 1)
-            if sh is not None:
-                z = z + sh.double().view(1, -1, 1, 1)
-            want = _act(z, act).expand(v.shape)
-            lin = (c.double().abs() * (1 if sc is None else sc.double().abs().view(1, -1, 1, 1))
-                   + (0 if sh is None else sh.double().abs().view(1, -1, 1, 1))).expand(v.shape)
-            bound = u * want.abs() + SWISH_LIP * 4 * 2.0 ** -24 * lin + ABS
-            r = float(((v.double() - want).abs() / bound).max())
+            want, bound = cached_view(c, sc, sh, act, dt)
+            r = float(((v.double() - want.expand(v.shape)).abs() / bound.expand(v.shape)).max())
             assert r <= 1.0, "view of cached buffer %s: error / bound %.3g" % (b.shape, r)
             worst = max(worst, r)
     return worst

@@ -253,6 +253,7 @@ class SepSpec:
     dsts: Tuple[Tuple[str, int, int], ...] = (("buf", 0, 0), ("buf", 0, 0))
     dw_bias: bool = True
     pw_bias: bool = True
+    per_image: bool = False         # B lists of N rows (SIGE_CONV_PER_IMAGE_OPERANDS): row b*N + i is tile i of image b
     seed: int = 0
 
     @property
@@ -315,6 +316,7 @@ class SepCase:
     pw_w: List[torch.Tensor]        # [Cout, Cin], launch dtype
     pw_b: List[Optional[torch.Tensor]]
     dst: List[Guarded]
+    tile_img: Optional[torch.Tensor] = None     # per-image lists: the image of each row (default row // N)
 
     def buffers(self) -> Dict[str, Guarded]:
         return {"dst%d" % i: g for i, g in enumerate(self.dst)}
@@ -391,14 +393,27 @@ def sep_descriptor(case: SepCase, flags: int = 0):
     return d
 
 
+def sep_images(case: SepCase) -> torch.Tensor:
+    """The image of each of the launch's B*N tile rows: row t // N of B shared lists, or `tile_img` of per-image lists."""
+    s = case.spec
+    t = torch.arange(s.B * s.N, device=case.src.device)
+    if s.per_image and case.tile_img is not None:
+        assert case.tile_img.numel() == s.B * s.N, s.name
+        return case.tile_img.long().to(t.device)
+    return t // s.N
+
+
 def sep_halo(case: SepCase):
     """float64 halo tiles [B*N, 6, 6, Cin] the launch reads (zero outside the source image and on padding tiles of a buffer
-    source), the tile origins [B*N, 2] (None without a list) and the padding mask [B*N]."""
+    source), the tile origins [B*N, 2] (None without a list) and the padding mask [B*N].  A shared list is read by every
+    image; per-image lists hold B*N rows, row t a tile of image sep_images(case)[t]."""
     s = case.spec
     dev = case.src.device
     NT = s.B * s.N
     t = torch.arange(NT, device=dev)
-    img, row = t // s.N, t % s.N
+    img, row = sep_images(case), (t if s.per_image else t % s.N)
+    if s.per_image:
+        assert not s.src_stack and case.idx is not None and case.idx.shape[0] == NT, s.name
     org = None if case.idx is None else case.idx.long()[row]
     none = torch.zeros(NT, dtype=torch.bool, device=dev) if org is None else org[:, 0] == TILE_NONE
     win = slice(s.pre, s.pre + s.Cin)
@@ -417,7 +432,7 @@ def sep_reference(case: SepCase) -> List[Expect]:
     u = ROUNDOFF[case.dtype]
     x, org, none = sep_halo(case)
     NT = s.B * s.N
-    img = torch.arange(NT, device=dev) // s.N
+    img = sep_images(case)
     d4 = torch.arange(4, device=dev)
     out = []
     for i, (kind, extra, c0) in enumerate(s.dsts):
@@ -483,6 +498,17 @@ CONV_IN_CASES = [
     ConvInSpec("tiles_per_image_two_aux", B=3, H=38, W=41, Cin=3, Cout=128, aux=((True, 1, False), (True, 1, True)),
                tiles=(True, (31, 12, 4), 6, 9), seed=8),
     ConvInSpec("tiles_per_image_cin1_cout256", B=2, H=22, W=19, Cin=1, Cout=256, aux=((False, 1, False),), tiles=(True, (9, 14), 4, 3), seed=9),
+    # weights above 48 KB take the dynamic shared-memory opt-in (dense_glue.cu conv_in_smem_ok): Cin 4 from Cout 328, Cin 3 from
+    # Cout 432; Cin 4, Cout 1544 is the largest stem that fits (231,600 B)
+    ConvInSpec("dense_cin4_cout320_below_optin", B=1, H=14, W=20, Cin=4, Cout=320, seed=10),
+    ConvInSpec("dense_cin4_cout328_optin", B=2, H=13, W=16, Cin=4, Cout=328, aux=((True, 1, False),), seed=11),
+    ConvInSpec("tiles_shared_cin4_cout328_optin", B=1, H=20, W=22, Cin=4, Cout=328, tiles=(False, (11,), 6, 5), seed=12),
+    ConvInSpec("dense_cin3_cout432_optin_aux", B=1, H=12, W=16, Cin=3, Cout=432, aux=((True, 1, True),), seed=13),
+    ConvInSpec("tiles_shared_cin3_cout512_aux", B=2, H=18, W=21, Cin=3, Cout=512, aux=((True, 0, False),), tiles=(False, (9,), 6, 3), seed=14),
+    ConvInSpec("tiles_per_image_cin4_cout512_sd_stem", B=2, H=24, W=20, Cin=4, Cout=512, aux=((True, 1, False),), tiles=(True, (7, 12), 6, 4),
+               seed=15),
+    ConvInSpec("dense_cin4_cout1544_largest", B=1, H=9, W=12, Cin=4, Cout=1544, seed=16),
+    ConvInSpec("tiles_shared_cin4_cout1544_largest", B=1, H=16, W=16, Cin=4, Cout=1544, aux=((True, 1, False),), tiles=(False, (5,), 6, 2), seed=17),
 ]
 
 

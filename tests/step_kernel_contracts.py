@@ -344,6 +344,179 @@ def sattn_reference(case: SAttnCase, chunk: int = 16) -> List[Expect]:
 
 
 # ----------------------------------------------------------------------------------------------------------------------
+# sige_sparse_attention at D = 512 (sparse_attention.cu, namespace wide)
+# ----------------------------------------------------------------------------------------------------------------------
+WIDE_D = 512
+WIDE_BNK = 32                   # keys per ring stage of the wide kernel
+WIDE_MAX_CS = 8                 # portable cluster size
+
+
+def wide_cluster(Nq: int, Nk: int, BH: int, sms: int) -> int:
+    """The launcher's cluster size: the smallest power of two that puts about one CTA on every SM, at most one key block per
+    CTA and 8 (wide::launch)."""
+    ctas = -(-Nq // BM) * BH
+    nblk = -(-Nk // WIDE_BNK)
+    cs = 1
+    while cs < WIDE_MAX_CS and 2 * cs <= nblk and ctas * cs < sms:
+        cs *= 2
+    return cs
+
+
+def wide_ranges(Nk: int, cs: int) -> List[Tuple[int, int]]:
+    """Key blocks [t0, t1) of each CTA of the cluster, in rank order."""
+    nblk = -(-Nk // WIDE_BNK)
+    return [(nblk * r // cs, nblk * (r + 1) // cs) for r in range(cs)]
+
+
+P = SAttnSpec
+WIDE_CASES = [
+    # cluster sizes at 132 SMs in the comments
+    P("q1_k1", 1, 1, 1, 1, 512, seed=1),                                                  # cs 1, one block
+    P("q63_k65_bnhd", 1, 1, 63, 65, 512, layout="bnhd", seed=2),                          # cs 2, a key tail of 1 after 2 blocks
+    P("q64_k4096", 1, 1, 64, 4096, 512, seed=3),                                          # cs 8
+    P("q65_k9216_bnhd", 1, 1, 65, 9216, 512, layout="bnhd", seed=4),                      # cs 8
+    P("q800_k4096", 1, 1, 800, 4096, 512, seed=5),                                        # cs 8, 13 query blocks
+    P("q800_k9216_bnhd", 1, 1, 800, 9216, 512, layout="bnhd", seed=6),
+    P("q64_k1_bnhd", 1, 1, 64, 1, 512, layout="bnhd", seed=7),
+    P("q65_k65", 1, 1, 65, 65, 512, seed=8),                                              # cs 2
+    P("q1_k4096_bnhd", 1, 1, 1, 4096, 512, layout="bnhd", seed=9),
+    P("q63_k9216_falling", 1, 1, 63, 9216, 512, mode="falling", seed=10),                 # 8 ranges across the falling blocks
+    P("q65_k4096_dominant_last_bnhd", 1, 1, 65, 4096, 512, mode="dominant", dom="last", layout="bnhd", seed=11),
+    P("q800_k65_dominant_first", 1, 1, 800, 65, 512, mode="dominant", seed=12),
+    P("q64_k4096_constant_v", 1, 1, 64, 4096, 512, mode="constant_v", seed=13),
+    P("b2_q65_k130_bnhd", 2, 1, 65, 130, 512, layout="bnhd", seed=14),                    # cs 4, B * heads 2
+    P("q8449_k96_cs1", 1, 1, 8449, 96, 512, seed=15),                                     # cs 1 over 3 blocks: 133 query blocks
+    P("q200_k96_falling_cs2", 1, 1, 200, 96, 512, mode="falling", seed=16),              # cs 2: ranges [0, 32) and [32, 96)
+    P("q64_k160_dominant_cs4", 1, 1, 64, 160, 512, mode="dominant", seed=17),             # cs 4: the dominant key in range 0 of 4
+    P("b2h2_q64_k1000_cs8", 2, 2, 64, 1000, 512, seed=18),                                # cs 8, B * heads 4, a key tail of 8
+    P("q64_k96_constant_v_cs2", 1, 1, 64, 96, 512, mode="constant_v", seed=19),
+]
+del P
+
+
+def wide_sattn_reference(case: SAttnCase, sms: int, chunk: int = 16) -> List[Expect]:
+    """out_i = softmax_j(scale q_i . k_j) v_j in float64, with the bound of the wide kernel's own algorithm.
+
+    How it computes (sparse_attention.cu, wide::kernel): the key range is split over a cluster of cs CTAs (wide_cluster), CTA r
+    taking the 32-key blocks [t0, t1) of wide_ranges; each runs its own online softmax from t0: fp32 logits l_j, the running
+    maximum m_t of its blocks t0 .. t, p_j = ex2.approx(fmaf(l_j, c, -fl(m_t c))), corr = ex2(fl(fl(m_{t-1} - m_t) c)) on o
+    and on l = fmaf(l, corr, sum); P rounded to 16 bits for P V.  The merge takes M = max_r m_r (m_r: CTA r's last maximum),
+    e_r = ex2(fl(fl(m_r - M) c)), L = sum_r fmaf(e_r, l_r), inv = fl(1 / L), w_r = fl(e_r inv) and out = sum_r fmaf(w_r, O_r),
+    peers in rank order, rounded once.  Per key j of block t in CTA r, the relative error of its weight that reaches numerator
+    and denominator alike (centred, as in sattn_reference):
+        e_j <= EX2_REL (t1 - t + 1)                   ex2 of p_j, of the t1 - 1 - t later corrs and of the merge weight
+             + U32 c (|m_t| + |l_j - m_t|)            the rounding of fl(m_t c) and of the fmaf argument
+             + 2 U32 c (m_r - m_t)                    the later corr arguments of the CTA (their differences telescope)
+             + 2 U32 c (M - m_r)                      the merge weight's argument: the difference and the product, rounded
+             + 2 U32 scale |l_j - M|                  c against scale * log2 e
+             + 2 scale dl                             the fp32 logit's error
+    Uncentred: the P rounding u sum_j s_j |v_j|, the f16 subnormal numerators ETA_P sum_j 2^(c (m_t - M)) |v_j| / L, the
+    per-CTA fp32 rest (2 T + 24) U32 mag with T the most blocks of a CTA, and the merge's (2 cs + 2) U32 mag: the cs fmaf of
+    L, the reciprocal, the product e_r inv and the cs fmaf of the output.  The output is rounded once: u |want|."""
+    s = case.spec
+    assert s.D == WIDE_D, s.name
+    u = ROUNDOFF[case.dtype]
+    sc = s.s32
+    c = sc * LOG2E
+    B, H, Nq, Nk, D = s.B, s.heads, s.Nq, s.Nk, s.D
+    cs = wide_cluster(Nq, Nk, B * H, sms)
+    ranges = wide_ranges(Nk, cs)
+    T = max(t1 - t0 for t0, t1 in ranges)
+    nblk = -(-Nk // WIDE_BNK)
+    dev = case.q.device
+    tj = torch.arange(Nk, device=dev) // WIDE_BNK                                          # block of each key
+    rank = torch.zeros(nblk, dtype=torch.long, device=dev)
+    t1_of = torch.zeros(nblk, dtype=torch.long, device=dev)
+    for r, (t0, t1) in enumerate(ranges):
+        rank[t0:t1], t1_of[t0:t1] = r, t1
+    rj, t1j = rank[tj], t1_of[tj]
+    q, k, v = case.q.double(), case.k.double(), case.v.double()
+    want = torch.empty(B, H, Nq, D, dtype=torch.float64, device=dev)
+    bound = torch.empty_like(want)
+    for b in range(B):
+        for h in range(H):
+            kk, vv = k[b, h], v[b, h]
+            for i0 in range(0, Nq, chunk):
+                qq = q[b, h, i0:i0 + chunk]
+                S = qq @ kk.t()
+                n = S.shape[0]
+                dl = ACC * (qq.abs() @ kk.abs().t()).amax(dim=1, keepdim=True)
+                padded = torch.full((n, nblk * WIDE_BNK), -math.inf, dtype=torch.float64, device=dev)
+                padded[:, :Nk] = S
+                bm = padded.view(n, nblk, WIDE_BNK).amax(dim=2)                           # block maxima
+                run = torch.empty_like(bm)
+                mr = torch.empty(n, cs, dtype=torch.float64, device=dev)
+                for r, (t0, t1) in enumerate(ranges):
+                    run[:, t0:t1] = bm[:, t0:t1].cummax(dim=1).values                    # each CTA's running maximum from t0
+                    mr[:, r] = run[:, t1 - 1]
+                M = mr.amax(dim=1, keepdim=True)
+                mt, mrj = run[:, tj], mr[:, rj]                                           # [n, Nk]
+                e = torch.exp(sc * (S - M))
+                L = e.sum(dim=1, keepdim=True)
+                sm = e / L
+                w = sm @ vv
+                ce = (EX2_REL * (t1j - tj + 1) + U32 * c * (mt.abs() + (S - mt).abs()) + 2 * U32 * c * (mrj - mt)
+                      + 2 * U32 * c * (M - mrj) + 2 * U32 * sc * (S - M).abs() + 2 * sc * dl)
+                cen = torch.einsum("qk,qkd->qd", ce * sm, (vv[None] - w[:, None]).abs())
+                mag = sm @ vv.abs()
+                eta = ETA_P[case.dtype] * (torch.exp(sc * (mt - M)) / L) @ vv.abs()
+                want[b, h, i0:i0 + n] = w
+                bound[b, h, i0:i0 + n] = (u * w.abs() + u * mag + cen + (ACC + (2 * T + 24 + 2 * cs + 2) * U32) * mag + eta + ABS)
+    ex, (wv, wr, bd, rnd) = expect_for("out", case.out, u)
+    view = (lambda t: t) if case.out.layout == "bhnd" else (lambda t: t[..., :D].permute(0, 2, 1, 3))      # noqa: E731
+    view(wv)[:], view(wr)[:], view(bd)[:], view(rnd)[:] = want, True, bound, u * want.abs()
+    return [ex]
+
+
+def wide_sattn_emulate(case: SAttnCase, sms: int) -> torch.Tensor:
+    """The wide kernel's arithmetic in float32, in its order (blocks of 32 keys, the cluster's key ranges, each range's online
+    softmax, the merge in rank order), on the case's 16-bit operands: [B, heads, Nq, D] float64 of the rounded output.  The fp32
+    logits are the exact dot products rounded once, ex2.approx is exp2 in float32, each fmaf one rounding of the float64 value."""
+    s = case.spec
+    f32 = torch.float32
+    c = float(np.float32(s.s32 * LOG2E))
+    cs = wide_cluster(s.Nq, s.Nk, s.B * s.heads, sms)
+    out = torch.empty(s.B, s.heads, s.Nq, s.D, dtype=torch.float64, device=case.q.device)
+
+    def fma(a, b, z):
+        return (a.double() * b.double() + z.double()).float()
+
+    for b in range(s.B):
+        for h in range(s.heads):
+            S = (case.q[b, h].double() @ case.k[b, h].double().t()).float()
+            v = case.v[b, h].float()
+            parts = []
+            for t0, t1 in wide_ranges(s.Nk, cs):
+                m = torch.full((s.Nq,), -math.inf, dtype=f32)
+                l = torch.zeros(s.Nq, dtype=f32)
+                o = torch.zeros(s.Nq, s.D, dtype=f32)
+                for t in range(t0, t1):
+                    j0, j1 = t * WIDE_BNK, min((t + 1) * WIDE_BNK, s.Nk)
+                    sb = S[:, j0:j1]
+                    m_new = torch.maximum(m, sb.amax(dim=1))
+                    corr = torch.exp2((m - m_new) * c)
+                    mb = m_new * c
+                    p = torch.exp2(fma(sb, torch.tensor(c, dtype=f32), -mb[:, None]))
+                    l = fma(l, corr, p.sum(dim=1))
+                    o = o * corr[:, None] + p.to(case.dtype).float() @ v[j0:j1]
+                    m = m_new
+                parts.append((m, l, o))
+            M = torch.stack([pm for pm, _, _ in parts]).amax(dim=0)
+            L = torch.zeros(s.Nq, dtype=f32)
+            es = []
+            for pm, pl, _ in parts:
+                e = torch.exp2((pm - M) * c)
+                es.append(e)
+                L = fma(e, pl, L)
+            inv = 1.0 / L
+            acc = torch.zeros(s.Nq, s.D, dtype=f32)
+            for e, (_, _, po) in zip(es, parts):
+                acc = fma((e * inv)[:, None], po, acc)
+            out[b, h] = acc.to(case.dtype).double()
+    return out
+
+
+# ----------------------------------------------------------------------------------------------------------------------
 # sige_spade_modulate
 # ----------------------------------------------------------------------------------------------------------------------
 SPADE_VEC = {torch.float32: 4, torch.float16: 8, torch.bfloat16: 8}

@@ -140,6 +140,21 @@ def test_conv_in_nhwc_tiles_size_guards(cabi_lib):
     assert _conv_in_tiles(1, 1, 2 ** 31 - 2, 1, 3) != 0 and "n_aux must be 0..2" in _err(), _err()
 
 
+@pytest.mark.parametrize("dtype", ["F16", "BF16"])
+@pytest.mark.parametrize("cin,cout", [(4, 1552), (2, 2984), (1, 5536)])
+def test_conv_in_refuses_weights_beyond_shared_memory(cabi_lib, cin, cout, dtype):
+    """The first stem per Cin whose staged weights, 4 ((Cout / 8) pitch(Cin) + Cout) bytes, pass 227 KB (Cin 4: 232,800 B) is
+    refused by both entry points before any CUDA call; the accepting side (Cout 1544 at Cin 4) is a GPU contract case, since it
+    calls cudaFuncSetAttribute."""
+    from sige_b200 import _cabi
+
+    lib, dt = _cabi.lib(), getattr(_cabi, dtype)
+    assert lib.sige_conv_in_nhwc(P, P, None, P, dt, 1, 8, 8, cin, cout, 0, None, None) != 0
+    assert "sige_conv_in_nhwc: weights do not fit in shared memory" in _err(), _err()
+    assert lib.sige_conv_in_nhwc_tiles(P, P, None, P, dt, 1, 8, 8, cin, cout, P, 1, 6, 6, 0, 0, None, None) != 0
+    assert "sige_conv_in_nhwc_tiles: weights do not fit in shared memory" in _err(), _err()
+
+
 def _entry(N, B=1, src_dtype=None):
     from sige_b200 import _cabi
 

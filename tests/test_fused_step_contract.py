@@ -2,6 +2,7 @@
 (tests/fused_step_contract.py), and mutants of the simulator that each break one launch, which the walk must name."""
 import copy
 import os
+import re
 import sys
 import types
 import warnings
@@ -400,3 +401,259 @@ def test_a_writeback_into_the_wrong_cache_is_rejected_by_name():
     fsc.walk(step, model=model)
     with pytest.raises(AssertionError, match=r"writeback launch \d+ \(writeback\)"):
         fsc.walk(step, step.low.epilogue, model=model)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the Stable Diffusion decoder (a q stack of fixed capacity, the D = 512 sparse attention), batches of label edits (per-image
+# separable and modulated launches) and the cache load of a new edit
+# ---------------------------------------------------------------------------------------------------------------------
+def _sd_step(executor_cls):
+    import test_sd_decoder as TSD
+
+    return TSD._steps(executor_cls())
+
+
+def _sd_rebind(net, step):
+    from oracle.cpu_runtime import reference_cpu_runtime
+    from sige.utils import downsample_mask
+    from sige_b200.workloads import sd_decoder as SD
+
+    _, z1, mask = SD.sd_decoder_inputs("mini")
+    mask2 = torch.zeros_like(mask)
+    mask2[12:20, 6:15] = True                    # the second mask of test_sd_decoder.py: fewer tiles than the first
+    with reference_cpu_runtime(), torch.no_grad():
+        net.set_masks(downsample_mask(mask2, min_res=(4, 4), dilation=0))
+        assert step.rebind()
+    step.static_inputs[0].copy_(z1)
+
+
+def _sd_checks(step, res):
+    assert res["kinds"]["sparse_attention"].launches == 1 and res["poisoned"] > 0
+    stems = [r for r in step.low.conv_ins if int(r.weight.shape[0]) == 512]
+    assert len(stems) == 1 and res["kinds"]["conv_in"].launches >= 1
+
+
+def test_sd_decoder_step_meets_its_records_before_and_after_a_rebind():
+    import test_sd_decoder as TSD
+
+    _, net, step = _sd_step(fsc.recording(TSD.TileListSim))
+    _sd_checks(step, _walk(step, "sd_decoder mini"))
+    live = {sl.n for sl in step.low.slots.values()}
+    _sd_rebind(net, step)
+    assert {sl.n for sl in step.low.slots.values()} != live
+    _sd_checks(step, _walk(step, "sd_decoder mini after rebind"))
+
+
+def _no_tiles_batch(pyramid_of, masks):
+    """The set_masks argument of a batch whose last edit has no tiles: its pyramid all False.  (A mask without a set pixel is
+    not that: downsample_mask thresholds at min(0.3, max - eps), so an all-zero mask selects the whole image, as in the
+    reference.)"""
+    from sige_b200.masks import stack_mask_pyramids
+
+    pyrs = [pyramid_of(m) for m in masks]
+    pyrs[-1] = {k: torch.zeros_like(v) for k, v in pyrs[-1].items()}
+    return stack_mask_pyramids(pyrs)
+
+
+def _batched_gaugan(which, executor_cls):
+    import test_batched_gaugan as TBG
+    from oracle.cpu_runtime import reference_cpu_runtime
+    from sige_b200.workloads import gaugan_gc as G
+
+    net = TBG._generator(which)
+    s0, s1s, masks = G.gaugan_gc_edits("mini", TBG.E + 2)
+    with reference_cpu_runtime(), torch.no_grad():
+        net.set_mode("full")
+        net(s0)
+        net.set_mode("sparse")
+        net.set_masks(_no_tiles_batch(TBG._pyramid, masks[:TBG.E]))       # the third edit has no tiles
+        step = _step(net, s1s[:TBG.E], executor=executor_cls(), headroom=0.5)
+    return net, step, s1s, masks
+
+
+def _batched_class():
+    import test_batched_gaugan as TBG
+
+    return TBG._sims()[0]
+
+
+@pytest.mark.parametrize("which", ["gc", "spade"])
+def test_batched_gaugan_step_meets_its_records_and_the_next_batch_too(which):
+    import test_batched_gaugan as TBG
+    from oracle.cpu_runtime import reference_cpu_runtime
+
+    net, step, s1s, masks = _batched_gaugan(which, fsc.recording(_batched_class()))
+    res = _walk(step, "gaugan_%s mini batch of %d, the third edit without tiles" % (which, TBG.E))
+    assert any(f.spec.tile_img is not None for f in step.fused)
+    assert all(bool((sl.buf.view(TBG.E, sl.cap, 2)[2, :, 0] <= fsc.NONE_BELOW).all()) for sl in step.low.slots.values())
+    if which == "gc":
+        assert res["kinds"]["separable"].launches > 0 and all(r.tile_img is not None for r in step.low.separable)
+    order = [1, 3, 4]
+    with reference_cpu_runtime(), torch.no_grad():
+        net.set_masks(TBG._batch_masks(masks[order]))
+        assert step.rebind()
+    step.static_inputs[0].copy_(s1s[order])
+    _walk(step, "gaugan_%s mini next batch" % which)
+
+
+def _load_sim(base=None):
+    import test_cache_refresh as TCR
+
+    return fsc.recording(type(TCR._sim(base)))
+
+
+def _spade_base():
+    import test_spade_generator as TSG
+
+    return TSG._sims()[0]
+
+
+def _walk_loads(step, tag, model):
+    res = fsc.walk_loads(step, model=model)
+    print(fsc.summary(tag, res) + "; %d entries" % res["entries"])
+    assert res["kinds"]["cache_load"].launches == 1 and res["entries"] > 0
+    return res
+
+
+def test_cache_loads_meet_their_records_at_build_after_a_rebind_and_after_a_refresh():
+    from sige.utils import downsample_mask
+    from sige_b200.workloads.ddpm import DDPMConfig, synthetic_inputs
+
+    model, x1, t = _prepared()
+    step = _step(model, x1, t, executor=_load_sim()(), headroom=0.6)
+    _walk_loads(step, "ddpm_small loads at build", model)
+    _second_edit(model)
+    with torch.no_grad():
+        assert step.rebind()
+    _walk_loads(step, "ddpm_small loads after rebind", model)
+    x0, _, _, _ = synthetic_inputs(DDPMConfig.small(), 0.05, seed=0)
+    with torch.no_grad():
+        model.set_mode("full")
+        model(x0 * 0.7, t)
+        model.set_mode("sparse")
+        assert step.refresh()
+    _walk_loads(step, "ddpm_small loads after refresh", model)
+    assert fsc.cached_state_after_rebind(step) <= 1.0
+
+
+def test_spade_generator_cache_loads_meet_their_records():
+    import consumers
+    import test_spade_generator as TS
+    from oracle.cpu_runtime import reference_cpu_runtime
+    from sige_b200.workloads import gaugan_spade as GS
+
+    net = GS.build_gaugan_spade("mini")
+    s0, s1, mask = consumers.gaugan_inputs("mini")
+    with reference_cpu_runtime(), torch.no_grad():
+        net.set_mode("full")
+        net(s0)
+        net.set_masks(TS._pyramid(mask))
+        net.set_mode("sparse")
+        step = _step(net, s1, executor=_load_sim(_spade_base())())
+    _walk_loads(step, "gaugan_spade mini loads at build", net)
+    with reference_cpu_runtime(), torch.no_grad():
+        net.set_mode("full")
+        net(s1)
+        net.set_mode("sparse")
+        assert step.refresh()
+    _walk_loads(step, "gaugan_spade mini loads after refresh", net)
+    with reference_cpu_runtime(), torch.no_grad():
+        assert step.rebind()
+    _walk_loads(step, "gaugan_spade mini loads after rebind", net)
+
+
+# mutants of the new launch kinds: each must be rejected with the kind and the position of its launch
+def test_a_separable_launch_that_reads_image_0s_list_for_every_image_is_rejected_by_name():
+    import test_batched_gaugan as TBG
+
+    class OneList(fsc.recording(_batched_class())):
+        victim = None
+
+        def prepare_separable(self, rec):
+            if self.victim is not None or rec.tile_img is None:
+                return super().prepare_separable(rec)
+            self.victim = rec.name
+            n = rec.idx.shape[0] // rec.batch
+            m = copy.copy(rec)
+            m.idx = rec.idx.clone()
+            fn = super().prepare_separable(rec)
+            inner = _batched_class().prepare_separable(self, m)
+
+            def run(stream):
+                m.idx.copy_(rec.idx[:n].repeat(rec.batch, 1))       # image 0's list, read at launch time
+                inner(stream)
+            self.records[id(run)] = ("separable", rec, run)
+            del self.records[id(fn)]
+            return run
+
+    _, step, _, _ = _batched_gaugan("gc", OneList)
+    assert step.ex.victim is not None and TBG.E > 1
+    with pytest.raises(AssertionError, match=r"separable launch \d+ \(%s\)" % re.escape(step.ex.victim)):
+        fsc.walk(step)
+
+
+def test_a_sparse_attention_with_a_wrong_scale_is_rejected_by_name():
+    import test_sd_decoder as TSD
+
+    class WrongScale(fsc.recording(TSD.TileListSim)):
+        def prepare_sparse_attention(self, q, k, v, scale, out):
+            fn = TSD.TileListSim.prepare_sparse_attention(self, q, k, v, scale * 1.01, out)
+            return self._keep("sparse_attention", fn, dict(q=q, k=k, v=v, scale=scale, out=out))
+
+    _, _, step = _sd_step(WrongScale)
+    with pytest.raises(AssertionError, match=r"sparse_attention launch \d+ \(sparse_attention\)"):
+        fsc.walk(step)
+
+
+def test_a_q_stack_conv_that_writes_its_padding_rows_is_rejected_by_name():
+    import test_sd_decoder as TSD
+
+    class WritesPadding(fsc.recording(TSD.TileListSim)):
+        victim = None
+
+        def prepare_conv(self, fc):
+            s = fc.spec
+            if s.dst_stack is None or s.src_is_stack:
+                return super().prepare_conv(fc)
+            self.victim = fc.name
+            SimExecutor = TSD.SimExecutor
+            SimExecutor.prepare_conv(self, fc)                        # the plain simulator writes every row of its stack
+            self._records()[id(fc)] = ("conv", False, fc)
+
+    _, _, step = _sd_step(WritesPadding)
+    assert step.ex.victim is not None and any(sl.cap > sl.n for sl in step.low.slots.values())
+    with pytest.raises(AssertionError, match=r"conv launch \d+ \(%s\): wrote outside its record" % re.escape(step.ex.victim)):
+        fsc.walk(step)
+
+
+def _load_mutant(change):
+    Base = _load_sim()
+
+    class Mutant(Base):
+        def prepare_cache_load(self, entries):
+            entries = [(src, raw, list(views)) for (src, raw, views) in entries]
+            fn = super(fsc.RecordingMixin, self).prepare_cache_load(change(entries))
+            return self._keep("cache_load", fn, entries)
+
+    return Mutant
+
+
+def _drop_a_shift(entries):
+    out = [(src, raw, list(views)) for (src, raw, views) in entries]
+    i, j = next((i, j) for i, (_, _, vs) in enumerate(out) for j, v in enumerate(vs) if v[2] is not None and float(v[2].abs().max()) > 0)
+    v, sc, _, act = out[i][2][j]
+    out[i][2][j] = (v, sc, None, act)
+    return out
+
+
+def _also_writes_its_source(entries):
+    src = entries[0][0]
+    return entries + [(src, None, [(src, None, torch.ones(src.shape[1]), "identity")])]      # cache + 1 into the cache itself
+
+
+@pytest.mark.parametrize("change", [_drop_a_shift, _also_writes_its_source], ids=["drops_a_views_shift", "writes_its_source_cache"])
+def test_a_broken_cache_load_is_rejected_by_name(change):
+    model, x1, t = _prepared()
+    step = _step(model, x1, t, executor=_load_mutant(change)())
+    with pytest.raises(AssertionError, match=r"cache_load launch 0 \(cache_load\)"):
+        fsc.walk_loads(step, model=model)

@@ -15,7 +15,6 @@ import sys
 import numpy as np
 import pytest
 import torch
-from torch.nn import functional as F
 
 from conftest import REPO
 
@@ -167,10 +166,10 @@ def test_flag_clear_keeps_the_parent_results():
 # ---------------------------------------------------------------------------------------------------------------- separable
 SEP_CASES = [
     # B = 3 edits, N rows per edit (real tiles at the front, SIGE_TILE_NONE behind), one edit without tiles
-    (kc.SepSpec("pi_sep48_96", B=3, Cin=48, Cout=96, H=22, W=30, real=20, lead=20, tail=12, pre=96, seed=931), (20, 7, 0)),
+    (kc.SepSpec("pi_sep48_96", B=3, Cin=48, Cout=96, H=22, W=30, real=20, lead=20, tail=12, pre=96, per_image=True, seed=931), (20, 7, 0)),
     (kc.SepSpec("pi_sep64_256_one_branch", B=3, Cin=64, Cout=256, H=20, W=24, real=14, lead=14, tail=2, post=64,
-                dsts=(("buf", 64, 64),), seed=932), (0, 14, 5)),
-    (kc.SepSpec("pi_sep16_40", B=3, Cin=16, Cout=40, H=18, W=26, real=15, lead=15, tail=9, seed=933), (15, 0, 9)),
+                dsts=(("buf", 64, 64),), per_image=True, seed=932), (0, 14, 5)),
+    (kc.SepSpec("pi_sep16_40", B=3, Cin=16, Cout=40, H=18, W=26, real=15, lead=15, tail=9, per_image=True, seed=933), (15, 0, 9)),
 ]
 
 
@@ -185,51 +184,13 @@ def _per_image_sep(spec, counts, dtype):
     return case
 
 
-def _sep_reference(case):
-    """kc.sep_reference restated for per-image lists: row t of idx is a tile of image t // N."""
-    s = case.spec
-    u = kc.ROUNDOFF[case.dtype]
-    NT = s.B * s.N
-    t = torch.arange(NT, device=DEV)
-    img = t // s.N
-    org = case.idx.long()
-    none = org[:, 0] == kc.TILE_NONE
-    win = slice(s.pre, s.pre + s.Cin)
-    d6, d4 = torch.arange(6, device=DEV), torch.arange(4, device=DEV)
-    hh, ww = org[:, :1] + d6, org[:, 1:] + d6
-    valid = ((hh >= 0) & (hh < s.H))[:, :, None] & ((ww >= 0) & (ww < s.W))[:, None, :] & ~none[:, None, None]
-    x = case.src[img[:, None, None], hh.clamp(0, s.H - 1)[:, :, None], ww.clamp(0, s.W - 1)[:, None, :]][..., win].double()
-    x = torch.where(valid[..., None], x, torch.zeros((), dtype=x.dtype, device=DEV))
-    out = []
-    for i, (kind, extra, c0) in enumerate(s.dsts):
-        assert kind == "buf"
-        w9 = case.dw_w[i].double().view(s.Cin, 1, 3, 3)
-        a64 = F.conv2d(x.permute(0, 3, 1, 2), w9, None if case.dw_b[i] is None else case.dw_b[i].double(), groups=s.Cin).permute(0, 2, 3, 1)
-        a = a64.to(case.dtype).double()
-        pw = case.pw_w[i].double()
-        v, mag = a @ pw.t(), a.abs() @ pw.abs().t()
-        if case.pw_b[i] is not None:
-            v, mag = v + case.pw_b[i].double(), mag + case.pw_b[i].double().abs()
-        bound = u * v.abs() + kc.ACC * mag + kc.PRE_ULPS * u * (a64.abs() @ pw.abs().t()) + kc.ABS
-        e, (want, written, bd, rnd) = kc.expect_for("dst%d" % i, case.dst[i], u)
-        sl = slice(c0, c0 + s.Cout)
-        oh, ow = org[:, :1] + s.offH + d4, org[:, 1:] + s.offW + d4
-        ok = ((oh >= 0) & (oh < s.dh))[:, :, None] & ((ow >= 0) & (ow < s.dw))[:, None, :] & ~none[:, None, None]
-        OB = img[:, None, None].expand(NT, 4, 4)[ok]
-        OH, OW = oh[:, :, None].expand(NT, 4, 4)[ok], ow[:, None, :].expand(NT, 4, 4)[ok]
-        want[OB, OH, OW, sl], written[OB, OH, OW, sl] = v[ok], True
-        bd[OB, OH, OW, sl], rnd[OB, OH, OW, sl] = bound[ok], (u * v.abs())[ok]
-        out.append(e)
-    return out
-
-
 @DTYPES
 @pytest.mark.parametrize("spec,counts", SEP_CASES, ids=lambda c: getattr(c, "name", ""))
 def test_per_image_separable_launch_meets_the_float64_contract(spec, counts, dtype):
     from sige_b200 import _cabi
 
     case = _per_image_sep(spec, counts, dtype)
-    expects = _sep_reference(case)
+    expects = kc.sep_reference(case)
     d = kc.sep_descriptor(case)
     lib = _cabi.lib()
 

@@ -8,6 +8,8 @@ against the existing float64 restatements (tests/step_kernel_contracts.py, tests
     and a second launch bitwise identical.
   * Counts: get_scatter_map with N * Ro * So = 2^32 tile pixels, reduce_mask at the largest candidate grid it accepts
     (46340 x 46340 = 2^31 - 88048), and the tiled stem at 2^31 - 4096 outputs, whose grid-stride loop index used to wrap.
+  * Offsets past 2^31: the D = 512 sparse attention reading keys / values and writing output rows as column slices of one
+    [2^15 + 1, 2^16] buffer (clusters of 8 and of 1), and sige_cache_load into a destination of 2^31 + 2^20 elements.
 
 Not measured: a reduce_mask call that lists more than 2^30 active tiles (its 64-bit list offsets) would need a 16 GiB list.
 """
@@ -715,3 +717,152 @@ def test_separable_conv_destination_past_2_to_the_31_elements(dtype):
         assert first is None or torch.equal(kc.bits(got), kc.bits(first)), "%s: a second launch differs" % label
         first = got
     print("[extent contract] %-56s worst |err| / bound %.3f" % (label, float(ratio.max())))
+
+
+# ---------------------------------------------------------------------------------------------------------------- D = 512 attention
+def _sms():
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+@DTYPES2
+def test_wide_sparse_attention_keys_past_2_to_the_31_elements(dtype):
+    """D = 512: keys and values are the first and last 512 columns of the rows of one [2^15 + 1, 2^16] buffer, so k_sn * Nk =
+    2^31 + 2^16 and the last value ends on the buffer's last element; 64 queries split the 1025 key blocks over a cluster of 8.
+    Checked against step_kernel_contracts.wide_sattn_reference (four queries at a time: [4, Nk, D] float64 is 0.5 GiB)."""
+    Nk, kn, D, Nq = 2 ** 15 + 1, 2 ** 16, 512, 64
+    es = torch.empty((), dtype=dtype).element_size()
+    _check_peak("wide sparse attention keys 2^31", Nk * kn * es + 2 * ec.CHUNK * 8 + 2 * Nk * D * 8 + 4 * 4 * Nk * D * 8)
+    flat = torch.empty(Nk * kn, dtype=dtype, device=DEV)
+    ec.fill(flat, 781)
+    rows = flat.view(Nk, kn)
+    k, v = rows[:, :D][None, None], rows[:, kn - D:][None, None]
+    g = torch.Generator(device=DEV)
+    g.manual_seed(781)
+    spec = sk.SAttnSpec("wide_keys_past_2_31", 1, 1, Nq, Nk, D, seed=781)
+    assert sk.wide_cluster(Nq, Nk, 1, _sms()) == 8
+    q = (torch.randn(1, 1, Nq, D, generator=g, device=DEV) * 2 / (spec.s32 * D ** 0.5)).to(dtype)
+    out = kc.guarded((1, 1, Nq, D), dtype, DEV, g, "bhnd")
+    case = sk.SAttnCase(spec, dtype, q, k, v, {"q": q}, out, out.view)
+    expects = sk.wide_sattn_reference(case, _sms(), chunk=4)
+    lib = _lib()
+    label = "sparse_attention d512 %s (k_sn %d x Nk %d, cluster 8)" % (NAME[dtype], kn, Nk)
+    _run_and_check("sattn", label, case, expects, lambda flags: sk.sattn_call(case, lib))
+    ec.unchanged_outside(label, flat, 781, lambda i: torch.zeros_like(i, dtype=torch.bool))
+
+
+@DTYPES2
+def test_wide_sparse_attention_output_rows_past_2_to_the_31_elements(dtype):
+    """D = 512: the output rows are the last 512 columns of the rows of one [2^15 + 1, 2^16] buffer, so o_sn * Nq = 2^31 + 2^16;
+    64 keys and 513 query blocks give a cluster of 1.  The float64 restatement (wide_sattn_reference, 64 queries at a time: with 64
+    keys [queries, Nk, D] is small) is written into a [Nq, D] stand-in; every element of the big buffer outside those columns
+    stays bitwise as it was filled."""
+    Nq, on, D, Nk = 2 ** 15 + 1, 2 ** 16, 512, 64
+    es = torch.empty((), dtype=dtype).element_size()
+    _check_peak("wide sparse attention output 2^31", Nq * on * es + 2 * ec.CHUNK * 8 + 6 * Nq * D * 8 + Nq * D * es)
+    flat = torch.empty(Nq * on, dtype=dtype, device=DEV)
+    ec.fill(flat, 782)
+    o4 = flat.view(Nq, on)[:, on - D:][None, None]
+    spec = sk.SAttnSpec("wide_out_past_2_31", 1, 1, Nq, Nk, D, seed=782)
+    assert sk.wide_cluster(Nq, Nk, 1, _sms()) == 1
+    qv, kv_, vv = sk.sattn_values(spec, DEV)
+    q, k, v = (t.to(dtype).contiguous() for t in (qv, kv_, vv))
+    del qv, kv_, vv
+    g = torch.Generator(device=DEV)
+    g.manual_seed(782)
+    stand_in = kc.guarded((1, 1, Nq, D), dtype, DEV, g, "bhnd")
+    case = sk.SAttnCase(spec, dtype, q, k, v, {"q": q, "k": k, "v": v}, stand_in, o4)
+    (e,) = sk.wide_sattn_reference(case, _sms(), chunk=64)
+    n = Nq * D
+    want, bound = e.want[stand_in.off:stand_in.off + n].view(Nq, D), e.bound[stand_in.off:stand_in.off + n].view(Nq, D)
+    del e
+    inputs0 = [t.clone() for t in (q, k, v)]
+    lib = _lib()
+    label = "sparse_attention d512 %s (o_sn %d x Nq %d, cluster 1)" % (NAME[dtype], on, Nq)
+    first, worst = None, 0.0
+    for launch in range(2):
+        assert sk.sattn_call(case, lib) == 0, lib.sige_last_error()
+        torch.cuda.synchronize()
+        ec.unchanged_outside(label, flat, 782, lambda i: i % on >= on - D)
+        assert all(torch.equal(kc.bits(a), kc.bits(b)) for a, b in zip((q, k, v), inputs0)), "%s: an input changed" % label
+        got = o4[0, 0]
+        if launch == 0:
+            first = got.clone()
+            for r0 in range(0, Nq, 4096):
+                err = (got[r0:r0 + 4096].double() - want[r0:r0 + 4096]).abs()
+                ratio = torch.nan_to_num(torch.where(err == 0, torch.zeros_like(err), err / bound[r0:r0 + 4096]), nan=float("inf"))
+                r = float(ratio.max())
+                if r > 1:
+                    i, c = (int(z) for z in (ratio == ratio.max()).nonzero()[0])
+                    raise AssertionError("%s: query %d channel %d: got %r, want %r, bound %.3g"
+                                         % (label, r0 + i, c, float(got[r0 + i, c]), float(want[r0 + i, c]), float(bound[r0 + i, c])))
+                worst = max(worst, r)
+        else:
+            assert torch.equal(kc.bits(got), kc.bits(first)), "%s: a second launch differs" % label
+    print("[extent contract] %-56s worst |err| / bound %.3f" % (label, worst))
+
+
+# ---------------------------------------------------------------------------------------------------------------- cache load
+@DTYPES2
+@pytest.mark.parametrize("what", ["raw", "swish_view"])
+def test_cache_load_destination_past_2_to_the_31_elements(what, dtype):
+    """sige_cache_load of one image's f32 cache (C = 256, 2048 x 2049 pixels) into a channels-last destination of E = 2 images:
+    2^31 + 2^20 elements, followed by a guard band of 2^16 in one buffer.  raw: the cache in `dtype`, bitwise, in both images;
+    swish_view: swish(cache * scale + shift) within fused_step_contract.cached_view's bound.  Every other element of the buffer
+    bitwise as it was filled; a second launch bitwise identical."""
+    import fused_step_contract as fsc
+    from sige_b200 import ops
+
+    E, C, H, W, guard = 2, 256, 2048, 2049, 2 ** 16
+    n = E * C * H * W
+    assert n == 2 ** 31 + 2 ** 20
+    es = torch.empty((), dtype=dtype).element_size()
+    rows = 32                                                               # image rows per check chunk
+    _check_peak("cache_load 2^31", (n + guard) * es + C * H * W * 4 + max(2 * ec.CHUNK * 8, 6 * rows * W * C * 8, 3 * (1 << 24) * 8))
+    flat = torch.empty(n + guard, dtype=dtype, device=DEV)
+    ec.fill(flat, 791)
+    dst = flat[:n].view(E, H, W, C).permute(0, 3, 1, 2)                    # channels-last [E, C, H, W]
+    g = torch.Generator(device=DEV)
+    g.manual_seed(791)
+    src = torch.randn(1, C, H, W, generator=g, device=DEV)
+    sc = (1 + 0.3 * torch.randn(C, generator=g, device=DEV)).float()
+    sh = (0.4 * torch.randn(C, generator=g, device=DEV)).float()
+    entry = (src, dst, []) if what == "raw" else (src, None, [(dst, sc, sh, "swish")])
+    run = ops.cache_load_launcher([entry], dtype)
+    label = "cache_load %s %s (E 2 x %d elements)" % (what, NAME[dtype], C * H * W)
+
+    def digest():                    # per chunk of the destination: a position-weighted sum of its bits (a second launch's check)
+        out = []
+        for k in range(0, n, 1 << 24):
+            b = kc.bits(flat[k:min(k + (1 << 24), n)]).long()
+            out.append(int((b * (torch.arange(b.numel(), device=DEV) % 65521 + 1)).sum()))
+        return out
+
+    worst = 0.0
+    run(_stream())
+    torch.cuda.synchronize()
+    ec.unchanged_outside(label, flat, 791, lambda i: i < n)
+    for e in range(E):
+        for h0 in range(0, H, rows):
+            c = src[:, :, h0:h0 + rows]
+            got = dst[e:e + 1, :, h0:h0 + rows]
+            if what == "raw":
+                same = kc.bits(got.contiguous()) == kc.bits(c.to(dtype).contiguous())
+                if not bool(same.all()):
+                    _, ch, hh, ww = (int(z) for z in (~same).nonzero()[0])
+                    raise AssertionError("%s: image %d (c, h, w) = (%d, %d, %d) is not the cache bit for bit" % (label, e, ch, h0 + hh, ww))
+                continue
+            want, bound = fsc.cached_view(c, sc, sh, "swish", dtype)
+            ratio = torch.nan_to_num((got.double() - want).abs() / bound, nan=float("inf"))
+            r = float(ratio.max())
+            if r > 1:
+                _, ch, hh, ww = (int(z) for z in (ratio == ratio.max()).nonzero()[0])
+                raise AssertionError("%s: image %d (c, h, w) = (%d, %d, %d): got %r, want %r"
+                                     % (label, e, ch, h0 + hh, ww, float(got[0, ch, hh, ww]), float(want[0, ch, hh, ww])))
+            worst = max(worst, r)
+            del want, bound, ratio
+    first = digest()
+    run(_stream())
+    torch.cuda.synchronize()
+    assert digest() == first, "%s: a second launch differs" % label
+    ec.unchanged_outside(label, flat, 791, lambda i: i < n)
+    print("[extent contract] %-56s worst |err| / bound %.3f" % (label, worst))

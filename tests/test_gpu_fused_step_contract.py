@@ -5,6 +5,7 @@ bitwise where the synchronised walk left it.  Two mutants of the executor, each 
 rejected by name."""
 import copy
 import os
+import re
 import sys
 import time
 import warnings
@@ -71,6 +72,7 @@ def _step(model, *args, step_dtype, executor_cls=None, **opts):
 def _walk_and_replay(step, tag, program=None, model=None, replays=True):
     """(a) the walk, (c) every non-eager entry checked, (b) graph replay and eager run bitwise equal to the walk."""
     t0 = time.perf_counter()
+    fsc.poison_padding(step)                 # (the walk poisons them too: replays start from the same padding rows)
     state = fsc.State(step, model)
     start = state.snapshot()
     res = fsc.walk(step, program, model=model, state=state)
@@ -287,3 +289,167 @@ def test_a_mistranslated_launch_is_rejected_by_name(mutate):
     with pytest.raises(AssertionError, match=r"conv launch \d+ \(%s\)" % step.ex.victim.replace(".", r"\.")) as err:
         fsc.walk(step, model=model)
     print("[fused step contract] mutant %s rejected: %s" % (mutate.__name__, str(err.value).splitlines()[0][:200]))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the Stable Diffusion decoder (its fixed-capacity q stack, the D = 512 sparse attention, the 4 -> 512 stem), batches of label
+# edits and the cache load of a new edit
+# ---------------------------------------------------------------------------------------------------------------------
+def _sd(size="mini"):
+    from sige.utils import downsample_mask
+    from sige_b200.workloads import sd_decoder as SD
+
+    net = SD.build_sd_decoder(size).to(DEV)
+    z0, z1, mask = (t.to(DEV) for t in SD.sd_decoder_inputs(size))
+    with torch.no_grad():
+        net.set_mode("full")
+        net(z0)
+        net.set_mode("sparse")
+        net.set_masks(downsample_mask(mask, min_res=(4, 4), dilation=0))
+    return net, z1, mask
+
+
+def _sd_launches(step, res):
+    assert res["kinds"]["sparse_attention"].launches == 1 and res["poisoned"] > 0
+    assert sum(1 for r in step.low.conv_ins if int(r.weight.shape[0]) == 512) == 1 and res["kinds"]["conv_in"].launches >= 1
+
+
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16], ids=["f16", "bf16"])
+def test_sd_decoder_step_meets_its_records_before_and_after_a_rebind(dtype):
+    from sige.utils import downsample_mask
+
+    net, z1, mask = _sd()
+    step = _step(net, z1, step_dtype=dtype)
+    _sd_launches(step, _walk_and_replay(step, "sd_decoder mini %s" % dtype, model=net))
+    mask2 = torch.zeros_like(mask)
+    mask2[12:20, 6:15] = True
+    net.set_masks(downsample_mask(mask2, min_res=(4, 4), dilation=0))
+    with torch.no_grad():
+        assert step.rebind()
+    res = fsc.walk_loads(step, model=net)
+    print(fsc.summary("sd_decoder mini %s loads after rebind" % dtype, res))
+    _sd_launches(step, _walk_and_replay(step, "sd_decoder mini %s after rebind" % dtype, model=net))
+
+
+def test_full_sd_decoder_step_meets_its_records():
+    """The in-tree "full" decoder: 4096 keys, so the D = 512 attention splits its key range over a cluster."""
+    import step_kernel_contracts as skc
+
+    net, z1, _ = _sd("full")
+    torch.cuda.reset_peak_memory_stats()
+    step = _step(net, z1, step_dtype=torch.float16)
+    (rec,) = [r for k, r, _ in step.ex.records.values() if k == "sparse_attention"]
+    nq, nk = int(rec["q"].shape[-2]), int(rec["k"].shape[-2])
+    cs = skc.wide_cluster(nq, nk, 1, torch.cuda.get_device_properties(0).multi_processor_count)
+    res = _walk_and_replay(step, "sd_decoder full fp16 (Nq %d, Nk %d, cluster %d)" % (nq, nk, cs), model=net)
+    print("[fused step contract] sd_decoder full: peak %.2f GB" % (torch.cuda.max_memory_allocated() / 2 ** 30))
+    _sd_launches(step, res)
+    assert nk == 4096 and cs > 1
+
+
+def _batched(which):
+    import test_fused_step_contract as TF
+    import test_gpu_batched_gaugan as TG
+    from sige_b200.workloads import gaugan_gc as G
+
+    net = TG._net(which)
+    s0, s1s, masks = (t.to(DEV) for t in G.gaugan_gc_edits("mini", 5))
+    with torch.no_grad():
+        net.set_mode("full")
+        net(s0)
+        net.set_mode("sparse")
+        net.set_masks(TF._no_tiles_batch(TG._pyr, masks[[0, 1, 2]]))       # the third edit has no tiles
+    return TG, net, s1s, masks
+
+
+@pytest.mark.parametrize("which", ["gc", "spade"])
+def test_batched_gaugan_step_meets_its_records(which):
+    TG, net, s1s, masks = _batched(which)
+    step = _step(net, s1s[[0, 1, 2]], step_dtype=torch.float16, headroom=0.5)
+    res = _walk_and_replay(step, "gaugan_%s mini fp16 batch of 3, the third edit without tiles" % which, model=net)
+    assert any(f.spec.tile_img is not None for f in step.fused)
+    assert all(bool((sl.buf.view(3, sl.cap, 2)[2, :, 0] <= fsc.NONE_BELOW).all()) for sl in step.low.slots.values())
+    assert (res["kinds"].get("separable", fsc.KindStats()).launches > 0) == (which == "gc")
+    net.set_masks(TG._batch(masks[[1, 3, 4]]))
+    with torch.no_grad():
+        assert step.rebind()
+    step.static_inputs[0].copy_(s1s[[1, 3, 4]])
+    _walk_and_replay(step, "gaugan_%s mini fp16 next batch" % which, model=net)
+
+
+def test_cache_loads_meet_their_records_after_a_refresh_and_after_a_rebind():
+    from sige_b200.workloads.ddpm import DDPMConfig, synthetic_inputs
+
+    model, x1, t = _prepared(DDPMConfig.small(), torch.float16)
+    step = _step(model, x1, t, step_dtype=torch.float16)
+    x0, _, _, _ = synthetic_inputs(DDPMConfig.small(), 0.05, seed=0)
+    with torch.no_grad():
+        model.set_mode("full")
+        model((x0 * 0.7).to(DEV).half(), t)
+        model.set_mode("sparse")
+        assert step.refresh()
+    res = fsc.walk_loads(step, model=model)
+    print(fsc.summary("ddpm_small fp16 loads after refresh", res))
+    assert res["kinds"]["cache_load"].launches == 1
+
+    import consumers
+    from sige.utils import dilate_mask, downsample_mask
+    from sige_b200.workloads import gaugan_spade as GS
+
+    net = GS.build_gaugan_spade("mini").to(DEV)
+    consumers.run_gaugan(net, downsample_mask, dilate_mask, device=DEV, size="mini", fused=lambda n: n.set_fused(False))
+    step = _step(net, consumers.gaugan_inputs("mini")[1].to(DEV), step_dtype=torch.float16)
+    with torch.no_grad():
+        assert step.rebind()
+    res = fsc.walk_loads(step, model=net)
+    print(fsc.summary("gaugan_spade mini fp16 loads after rebind", res))
+    assert res["kinds"]["cache_load"].launches == 1
+
+
+# mutants of the separable and sparse-attention translations; every access stays inside its allocation
+def test_a_separable_launch_without_per_image_operands_is_rejected_by_name():
+    """The batch's separable launch without SIGE_CONV_PER_IMAGE_OPERANDS: its E lists read as one shared list of E * cap rows, so
+    every image takes the tiles of every edit (all of them inside each image, which share one extent)."""
+    from sige_b200._cabi import CONV_PER_IMAGE_OPERANDS
+
+    class NoPerImage(_recording()):
+        victim = None
+
+        def prepare_separable(self, rec):
+            if self.victim is not None or rec.tile_img is None:
+                return super().prepare_separable(rec)
+            self.victim = rec.name
+            fn = super().prepare_separable(rec)
+            ops, branches = self.ops, [self._separable_weights(dw, w, b) + (d.raw,) for (dw, w, b, d) in rec.branches]
+            src = rec.src[:, rec.c0:rec.c0 + rec.Cin]
+
+            def run(_stream):
+                ops.separable_conv(src, branches, rec.idx, src_stack=False, offset=rec.off, batch=rec.batch, flags=0)
+            del self.records[id(fn)]
+            return self._keep("separable", run, rec)
+
+    assert CONV_PER_IMAGE_OPERANDS == 128
+    TG, net, s1s, _ = _batched("gc")
+    step = _step(net, s1s[[0, 1, 2]], step_dtype=torch.float16, executor_cls=NoPerImage)
+    assert step.ex.victim is not None
+    (rec,) = [r for r in step.low.separable if r.name == step.ex.victim]
+    with torch.no_grad():
+        for br in rec.branches:      # the stray tiles rewrite what the build's run left there: move it off first
+            br[3].raw.add_(0.5)
+    with pytest.raises(AssertionError, match=r"separable launch \d+ \(%s\)" % re.escape(step.ex.victim)) as err:
+        fsc.walk(step, model=net)
+    print("[fused step contract] mutant separable without per-image operands rejected: %s" % str(err.value).splitlines()[0][:200])
+
+
+def test_a_sparse_attention_over_one_key_fewer_is_rejected_by_name():
+    class OneKeyShort(_recording()):
+        def prepare_sparse_attention(self, q, k, v, scale, out):
+            fn = super().prepare_sparse_attention(q, k[..., :-1, :], v[..., :-1, :], scale, out)
+            del self.records[id(fn)]
+            return self._keep("sparse_attention", fn, dict(q=q, k=k, v=v, scale=scale, out=out))
+
+    net, z1, _ = _sd()
+    step = _step(net, z1, step_dtype=torch.float16, executor_cls=OneKeyShort)
+    with pytest.raises(AssertionError, match=r"sparse_attention launch \d+ \(sparse_attention\)") as err:
+        fsc.walk(step, model=net)
+    print("[fused step contract] mutant sparse attention over Nk - 1 keys rejected: %s" % str(err.value).splitlines()[0][:200])

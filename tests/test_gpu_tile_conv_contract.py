@@ -139,3 +139,51 @@ def test_stem_per_image_tiles_match_the_dense_stem(dtype):
     for got, want, before in ((out, dense, out0), (aux, dense_aux, aux0)):
         assert torch.equal(nhwc(got)[inside], nhwc(want)[inside])
         assert torch.equal(nhwc(got)[~inside].view(torch.int16), nhwc(before)[~inside].view(torch.int16))
+
+
+# ---------------------------------------------------------------------------------------------------------------- stack destination
+STACK_CASES = [
+    # a fixed-capacity list (real tiles, then SIGE_TILE_NONE padding) read from an image, written as a stack of tile rows:
+    # the q conv of the SD decoder's attention (1x1 on 4x4 tiles, 512 -> 512) and a 3x3 conv on 6x6 tiles of two images
+    tcc.Spec("stack_k1_c512", B=1, H=20, W=24, k=1, srcs=((512, 0),), Cout=512, counts=(13,), pad_to=24, seed=951),
+    tcc.Spec("stack_k3_c64_128_b2", B=2, H=22, W=26, srcs=((64, 0),), Cout=128, counts=(11,), pad_to=16, seed=952),
+]
+
+
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16], ids=["f16", "bf16"])
+@pytest.mark.parametrize("kernel", ["wgmma", "mma.sync"])
+@pytest.mark.parametrize("spec", STACK_CASES, ids=lambda s: s.name)
+def test_stack_destination_rows_of_padding_keep_their_contents(spec, kernel, dtype):
+    """dst_is_stack with a padded list: the row of each real tile within the float64 bound of its conv, the row of each
+    SIGE_TILE_NONE entry still holding its NaN sentinel bitwise (include/sige_b200.h: such a tile writes nothing)."""
+    import torch.nn.functional as F
+
+    from sige_b200 import ops
+
+    case = tcc.make_case(spec, dtype, DEV)
+    B, N, Ro, Cout = spec.B, spec.N, spec.Ro, spec.Cout
+    stack = torch.full((B * N, Ro, Ro, Cout), float("nan"), dtype=dtype, device=DEV)
+    d = tcc.descriptor(case, flags=tcc.TC5 if kernel == "wgmma" else 0)
+    d.dst, d.dst_is_stack, d.dH, d.dW, d.dC, d.dst_c0 = stack.data_ptr(), 1, Ro, Ro, Cout, 0
+    assert (tcc.plan_of(d).path == 1) == (kernel == "wgmma"), kernel
+    ops.launch_tile_conv(d, torch.cuda.current_stream().cuda_stream)
+    torch.cuda.synchronize()
+
+    t = torch.arange(B * N, device=DEV)
+    org = case.idx.long()[t % N]
+    none = org[:, 0] == tcc.TILE_NONE
+    assert bool(none.any()) and not bool(none.all())
+    a, valid = tcc._gather([(case.srcs[0], 0)], torch.where(none[:, None], torch.zeros_like(org), org), t // N, spec.R, spec.H, spec.W)
+    a = torch.where(valid[..., None], a, torch.zeros((), dtype=a.dtype, device=DEV)).permute(0, 3, 1, 2)
+    w, b = case.w.double(), case.bias.double()
+    v = F.conv2d(a, w, b).permute(0, 2, 3, 1)
+    mag = F.conv2d(a.abs(), w.abs(), b.abs()).permute(0, 2, 3, 1)
+    bound = tcc.UNIT_ROUNDOFF[dtype] * v.abs() + tcc.ACC * mag + tcc.ABS
+    got = stack.double()
+    ratio = ((got[~none] - v[~none]).abs() / bound[~none]).nan_to_num(nan=float("inf"))
+    assert float(ratio.max()) <= 1.0, "%s %s: a real tile's row off by %.3g of its bound" % (spec.name, kernel, float(ratio.max()))
+    pad = stack[none].view(torch.int16)
+    assert torch.equal(pad, torch.full_like(stack[none], float("nan")).view(torch.int16)), "%s %s: a padding row was written" % (spec.name, kernel)
+    print("[tile conv contract] stack destination %s %s %s: %d real rows worst |err| / bound %.3f, %d padding rows untouched"
+          % (spec.name, kernel, tcc.DTYPE_NAME[dtype], int((~none).sum()), float(ratio.max()),
+             int(none.sum())))

@@ -104,6 +104,32 @@ def test_separable_restatement_matches_conv2d(name):
         assert torch.allclose(got, ref[m], rtol=1e-12, atol=1e-12), "%s dst%d: %.3g" % (name, i, float((got - ref[m]).abs().max()))
 
 
+def test_per_image_separable_restatement_is_each_image_on_its_own_list():
+    """Per-image lists (row b*N + i a tile of image b): image b's part of the restatement is the shared-list restatement of a
+    one-image case whose list is rows [b*N, (b+1)*N); an image whose list is all SIGE_TILE_NONE is left as it was."""
+    import dataclasses
+
+    spec = kc.SepSpec("pi_cpu", B=3, Cin=16, Cout=24, H=18, W=22, real=9, lead=9, tail=5, pre=16, per_image=True, seed=7)
+    case = kc.make_sep(spec, F64, "cpu")
+    rows = []
+    for b, n in enumerate((9, 0, 4)):
+        tiles = [t for t in kc.sep_tile_list(spec, np.random.default_rng(40 + b)) if t[0] != kc.TILE_NONE]
+        rows += tiles[:n] + [(kc.TILE_NONE, kc.TILE_NONE)] * (spec.N - n)
+    case.idx = torch.tensor(rows, dtype=torch.int32)
+    s1 = dataclasses.replace(spec, B=1, per_image=False)
+    for i, e in enumerate(kc.sep_reference(case)):
+        want, written, bound = (_window(e, t) for t in (e.want, e.written, e.bound))
+        for b in range(spec.B):
+            flats = [g.view[b:b + 1].clone() for g in case.dst]
+            c1 = kc.SepCase(s1, F64, case.src[b:b + 1], case.idx[b * spec.N:(b + 1) * spec.N], case.dw_w, case.dw_b, case.pw_w,
+                            case.pw_b, [kc.Guarded(f.reshape(-1), f, 0, "nhwc") for f in flats])
+            e1 = kc.sep_reference(c1)[i]
+            w1, m1, b1 = (t.view(flats[i].shape)[0] for t in (e1.want, e1.written, e1.bound))
+            assert torch.equal(written[b], m1) and torch.equal(bound[b], b1), (i, b)
+            assert torch.equal(want[b][m1], w1[m1]), (i, b)
+            assert bool(m1.any()) == (b != 1), "the image without tiles is not written"
+
+
 def test_separable_restatement_matches_the_descriptor_simulator():
     """The restatement against SeparableSim (tests/test_separable_conv.py), the simulator the lowering tests run on, in fp32."""
     from test_separable_conv import _sim_executors
@@ -212,6 +238,13 @@ def test_conv_in_case_table_covers_the_launch_paths():
     assert any(s.tiles[0] for s in tiles) and any(not s.tiles[0] for s in tiles)
     assert all(s.tiles[3] > 0 for s in tiles if s.tiles[0]), "per-image lists carry SIGE_TILE_NONE entries"
     assert all(s.W % 4 == 0 for s in dense) and any(s.W % 4 for s in tiles)
+    # the shared-memory opt-in of weights above 48 KB (4 ((Cout / 8) 292 + Cout) bytes at Cin 4), on both sides and at its limit
+    assert 4 * (1544 // 8 * 292 + 1544) == 231600 <= 227 * 1024 < 4 * (1552 // 8 * 292 + 1552)
+    for paths in (dense, tiles):
+        assert any(s.Cin == 4 and s.Cout == 1544 for s in paths) and any(s.Cin == 4 and s.Cout >= 328 for s in paths)
+        assert any(s.Cin == 3 and s.Cout >= 432 and s.aux for s in paths)
+    assert any(s.Cin == 4 and 256 < s.Cout < 328 for s in dense)
+    assert any(s.Cin == 4 and s.Cout == 512 and s.tiles[0] for s in tiles), "the SD decoder's stem: per-image tiles, Cout 512"
 
 
 # ---------------------------------------------------------------------------------------------------------------- GroupNorm fold

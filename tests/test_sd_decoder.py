@@ -20,12 +20,27 @@ from sige_b200._cabi import TILE_NONE  # noqa: E402
 
 
 class TileListSim(SimExecutor):
-    """The simulator, plus the kernel's rule for a stack source read through a fixed-capacity tile list: the SIGE_TILE_NONE rows
-    that pad the list are computed and write nothing (include/sige_b200.h, sige_tile_conv_t)."""
+    """The simulator, plus the kernel's rule for a stack source or destination with a fixed-capacity tile list: the SIGE_TILE_NONE
+    rows that pad the list are computed and write nothing (include/sige_b200.h, sige_tile_conv_t)."""
 
     def prepare_conv(self, fc):
         super().prepare_conv(fc)
         s = fc.spec
+        if s.dst_stack is not None and not s.src_is_stack and s.idx is not None and s.tile_img is None and s.B == 1:
+            inner = fc.launch_fn
+
+            def gathered(stream):                              # a padding row of the list writes nothing to its stack row
+                keep = s.dst_stack
+                s.dst_stack = keep.clone()
+                try:
+                    inner(stream)
+                finally:
+                    real = s.idx[:, 0] != TILE_NONE
+                    keep[real] = s.dst_stack[real]
+                    s.dst_stack = keep
+
+            fc.launch_fn = gathered
+            return
         if not s.src_is_stack or s.idx is None:
             return
         inner = fc.launch_fn

@@ -131,6 +131,71 @@ def test_sparse_attention_case_table_covers_every_instantiation():
     assert all(s.B * s.heads <= 2 for s in cases if s.Nk >= 4000), "B * heads stays small where Nk is large"
 
 
+WIDE_SMS = kc.H100_SMS
+
+
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16], ids=["f16", "bf16"])
+@pytest.mark.parametrize("spec", sk.WIDE_CASES, ids=lambda s: s.name)
+def test_wide_kernel_emulation_stays_within_the_wide_bound(spec, dtype):
+    """The wide kernel's arithmetic emulated in float32 (sk.wide_sattn_emulate: 32-key blocks, the cluster's key ranges, the
+    merge) is within sk.wide_sattn_reference's bound everywhere, and its values are softmax(scale q k^T) v."""
+    case = sk.make_sattn(spec, dtype, "cpu")
+    (e,) = sk.wide_sattn_reference(case, WIDE_SMS, chunk=4)
+    (old,) = sk.sattn_reference(case, chunk=4)
+    got = sk.wide_sattn_emulate(case, WIDE_SMS)
+    view = (lambda t: _window(e, t)) if spec.layout == "bhnd" else (lambda t: _window(e, t)[..., :spec.D].permute(0, 2, 1, 3))  # noqa: E731
+    want, bound, old_bound = view(e.want), view(e.bound), view(old.bound)
+    err = (got - want).abs()
+    r, r_old = float((err / bound).max()), float((err / old_bound).max())
+    print("[wide restatement] %s %s cs=%d: emulation |err| / bound %.3f, / the 64-key bound %.3f"
+          % (spec.name, str(dtype)[6:], sk.wide_cluster(spec.Nq, spec.Nk, spec.B * spec.heads, WIDE_SMS),
+             r, r_old))
+    assert r <= 1.0, (spec.name, r)
+    sm = torch.softmax(spec.s32 * case.q.double() @ case.k.double().transpose(2, 3), -1) @ case.v.double()
+    torch.testing.assert_close(want, sm, rtol=1e-12, atol=1e-12)
+
+
+def test_wide_bound_is_honest_and_tight():
+    """As test_sparse_attention_bound_is_honest_and_tight, for the wide kernel's bound: at least the output's and P's rounding,
+    and within a small multiple of u (|want| + sum_j s_j |v_j|) where the softmax is not peaked."""
+    for name in ("q63_k65_bnhd", "q64_k4096_constant_v", "b2_q65_k130_bnhd", "b2h2_q64_k1000_cs8"):
+        spec = next(s for s in sk.WIDE_CASES if s.name == name)
+        for dt in (torch.float16, torch.bfloat16):
+            case = sk.make_sattn(spec, dt, "cpu")
+            (e,) = sk.wide_sattn_reference(case, WIDE_SMS, chunk=4)
+            u = kc.ROUNDOFF[dt]
+            want, bound = _window(e, e.want), _window(e, e.bound)
+            if spec.layout != "bhnd":
+                want, bound = want[..., :spec.D].permute(0, 2, 1, 3), bound[..., :spec.D].permute(0, 2, 1, 3)
+            p = torch.softmax(spec.s32 * case.q.double() @ case.k.double().transpose(2, 3), -1)
+            mag = p @ case.v.double().abs()
+            ratio = bound / (u * (want.abs() + mag))
+            assert float(ratio.min()) >= 1 and float(ratio.max()) < 8, (name, dt, float(ratio.max()))
+
+
+def test_wide_case_table_covers_the_cluster_split():
+    """At 132 SMs: cluster sizes 1, 2, 4 and 8, one of size 1 over several blocks; a range boundary inside the falling and the
+    dominant patterns; B * heads > 1 with a split; a multi-block key range ending in a partial 32-key block."""
+    cases = sk.WIDE_CASES
+    cs = {s.name: sk.wide_cluster(s.Nq, s.Nk, s.B * s.heads, WIDE_SMS) for s in cases}
+    assert {1, 2, 4, 8} <= set(cs.values())
+    assert any(cs[s.name] == 1 and s.Nk > sk.WIDE_BNK for s in cases)
+    for mode in ("falling", "dominant"):
+        assert any(s.mode == mode and cs[s.name] > 1 for s in cases), mode
+    assert any(s.B * s.heads > 1 and cs[s.name] > 1 for s in cases)
+    assert any(s.Nk % sk.WIDE_BNK and s.Nk > sk.WIDE_BNK for s in cases)
+    assert all(s.D == sk.WIDE_D for s in cases) and {"bhnd", "bnhd"} <= {s.layout for s in cases}
+    # every range holds at least one block, and the ranges tile the blocks
+    for s in cases:
+        r = sk.wide_ranges(s.Nk, cs[s.name])
+        assert r[0][0] == 0 and r[-1][1] == -(-s.Nk // sk.WIDE_BNK) and all(t1 > t0 for t0, t1 in r)
+        assert all(a[1] == b[0] for a, b in zip(r, r[1:]))
+    for s in cases:                  # a case named for its cluster size has that size
+        named = [int(p[2:]) for p in s.name.split("_") if p.startswith("cs") and p[2:].isdigit()]
+        assert named in ([], [cs[s.name]]), (s.name, cs[s.name])
+    assert sk.wide_cluster(64, 4096, 1, 132) == 8 and sk.wide_cluster(64 * 132, 4096, 1, 132) == 1 and sk.wide_cluster(65, 65, 1, 132) == 2
+
+
 def test_sparse_attention_refuses_a_scale_that_is_not_positive_and_finite(cabi_lib):
     """The header documents scale > 0; the entry point refuses anything else before it touches the device."""
     from sige_b200 import _cabi
