@@ -69,7 +69,7 @@ class RecordingMixin:
                           dict(x=x, groups=groups, eps=eps, gamma=gamma, beta=beta, act=act, weight=weight, bias=bias, out=out))
 
     def prepare_attention(self, qkv_tokens, out_tokens, pdl):
-        return self._keep("attention", super().prepare_attention(qkv_tokens, out_tokens, pdl), dict(qkv=qkv_tokens, out=out_tokens))
+        return self._keep("attention", super().prepare_attention(qkv_tokens, out_tokens, pdl), dict(qkv=qkv_tokens, out=out_tokens, pdl=pdl))
 
     def prepare_sparse_attention(self, q, k, v, scale, out):
         return self._keep("sparse_attention", super().prepare_sparse_attention(q, k, v, scale, out), dict(q=q, k=k, v=v, scale=scale, out=out))
@@ -670,20 +670,31 @@ EXPECT = {"conv": conv_expect, "conv_in": conv_in_expect, "tail": tail_expect, "
 # ----------------------------------------------------------------------------------------------------------------------
 # the walk
 # ----------------------------------------------------------------------------------------------------------------------
-def _allowed(state: State, wants: List[Want]) -> Dict[Tuple[str, int], torch.Tensor]:
-    """Per storage: bool over its bytes, True where the launch may write."""
-    out: Dict[Tuple[str, int], torch.Tensor] = {}
+Masks = Dict[Tuple[str, int], torch.Tensor]
+
+
+def _allowed(state: State, wants: List[Want], free_only: bool = False) -> Masks:
+    """Per storage: bool over its bytes, True where the launch may write (free_only: only the elements it may leave with any
+    value)."""
+    out: Masks = {}
     for w in wants:
         t = w.tensor
         key = _key(t)
         assert key in state.storages, "%s: written tensor outside the step's state" % w.name
+        if free_only and w.free is None:
+            continue
         nb = state.storages[key].bytes.numel()
         es = t.element_size()
         elem = torch.zeros(nb // es, dtype=torch.bool, device=t.device)
-        elem.as_strided(t.shape, t.stride(), t.storage_offset())[w.written if w.free is None else (w.written | w.free)] = True
+        elem.as_strided(t.shape, t.stride(), t.storage_offset())[w.free if free_only else (w.written if w.free is None else (w.written | w.free))] = True
         byte = elem.view(-1, 1).expand(-1, es).reshape(-1)
         out[key] = byte if key not in out else (out[key] | byte)
     return out
+
+
+def _union(into: Masks, more: Masks) -> None:
+    for k, m in more.items():
+        into[k] = m.clone() if k not in into else (into[k] | m)
 
 
 @dataclass
@@ -729,9 +740,13 @@ def _sync(dev) -> None:
         torch.cuda.synchronize(dev)
 
 
-def _check_launch(state: State, kinds: Dict[str, KindStats], kind: str, label: str, wants: List[Want], fn, stream, dev) -> None:
-    """Snapshot the whole state, launch, synchronise: nothing outside the wanted elements changed, every wanted one in bound."""
+def _check_launch(state: State, kinds: Dict[str, KindStats], kind: str, label: str, wants: List[Want], fn, stream, dev,
+                  footprint: Masks, free: Masks) -> None:
+    """Snapshot the whole state, launch, synchronise: nothing outside the wanted elements changed, every wanted one in bound.
+    The bytes the launch may write join `footprint`, those it may leave with any value `free`."""
     allowed = _allowed(state, wants)
+    _union(footprint, allowed)
+    _union(free, _allowed(state, wants, free_only=True))
     snap = state.snapshot()
     fn(stream)
     _sync(dev)
@@ -764,6 +779,8 @@ def walk(step, program=None, model=None, state: Optional[State] = None) -> Dict[
     dev = step.dev
     stream = torch.cuda.current_stream(dev).cuda_stream if dev.type == "cuda" else 0
     kinds: Dict[str, KindStats] = {}
+    footprint: Masks = {}
+    free: Masks = {}
     eager = 0
     t0 = time.perf_counter()
     with torch.no_grad():
@@ -783,8 +800,9 @@ def walk(step, program=None, model=None, state: Optional[State] = None) -> Dict[
                 wants = sparse_attention_expect(rec, step.dtype, live_tokens(step, rec["q"]))
             else:
                 wants = EXPECT[kind](rec, step.dtype)
-            _check_launch(state, kinds, kind, label, wants, fn, stream, dev)
-    return {"kinds": kinds, "eager": eager, "seconds": time.perf_counter() - t0, "state_bytes": state.nbytes, "poisoned": poisoned}
+            _check_launch(state, kinds, kind, label, wants, fn, stream, dev, footprint, free)
+    return {"kinds": kinds, "eager": eager, "seconds": time.perf_counter() - t0, "state_bytes": state.nbytes, "poisoned": poisoned,
+            "footprint": footprint, "free": free}
 
 
 def walk_loads(step, model=None, state: Optional[State] = None) -> Dict[str, object]:
@@ -795,16 +813,62 @@ def walk_loads(step, model=None, state: Optional[State] = None) -> Dict[str, obj
     dev = step.dev
     stream = torch.cuda.current_stream(dev).cuda_stream if dev.type == "cuda" else 0
     kinds: Dict[str, KindStats] = {}
+    footprint: Masks = {}
+    free: Masks = {}
     t0 = time.perf_counter()
     with torch.no_grad():
         if run is not None:
             rec = step.ex.record_of("cache_load", run)
-            _check_launch(state, kinds, "cache_load", "cache_load launch 0 (cache_load)", cache_load_expect(rec, step.dtype), run, stream, dev)
+            _check_launch(state, kinds, "cache_load", "cache_load launch 0 (cache_load)", cache_load_expect(rec, step.dtype), run, stream, dev,
+                          footprint, free)
         for b in rest:
             b.restore()
         _sync(dev)
     return {"kinds": kinds, "eager": len(rest), "seconds": time.perf_counter() - t0, "state_bytes": state.nbytes,
-            "entries": 0 if run is None else len(step.ex.record_of("cache_load", run))}
+            "entries": 0 if run is None else len(step.ex.record_of("cache_load", run)), "footprint": footprint, "free": free}
+
+
+POISON = 0xFF                  # every byte: NaN in f16, bf16 and f32
+
+
+def poison(state: State, footprint: Masks) -> int:
+    """POISON into every byte of a program's write footprint (the union of its launches' `_allowed` masks, as `walk` returns
+    it).  A launch that reads a byte its program writes before the program has written it then reads NaN.  Returns the bytes
+    poisoned."""
+    n = 0
+    with torch.no_grad():
+        for key, m in footprint.items():
+            state.storages[key].bytes[m] = POISON
+            n += int(m.sum())
+    return n
+
+
+def differs_outside(state: State, snap, free: Masks) -> Optional[str]:
+    """Like State.differs, ignoring the bytes a launch may leave with any value (`free`: rows of padding tiles)."""
+    for k, s in state.storages.items():
+        d = s.bytes != snap[k]
+        if k in free:
+            d &= ~free[k]
+        if bool(d.any()):
+            return "%s (%d bytes differ, the first at byte %d)" % (s.name, int(d.sum()), int(d.nonzero()[0]))
+    return None
+
+
+def poisoned_walk(step, res, start, walked, program=None, model=None, state: Optional[State] = None, loads: bool = False):
+    """From `start`, the footprint of the first walk `res` poisoned (and, before a walk, the padding rows, as `walk` does): the
+    walk again (walk or walk_loads), which must meet every record and leave every byte outside the padding rows as the first walk left them
+    (`walked`).  Returns (the second walk's result, the poisoned state it started from, the state it ended in, bytes
+    poisoned)."""
+    state = state or State(step, model)
+    state.restore(start)
+    n = poison(state, res["footprint"])
+    if not loads:
+        poison_padding(step)
+    from_ = state.snapshot()
+    res2 = walk_loads(step, model=model, state=state) if loads else walk(step, program, model=model, state=state)
+    diff = differs_outside(state, walked, res["free"])
+    assert diff is None, "after its write footprint was poisoned (%d bytes), the walk ends differently: %s" % (n, diff)
+    return res2, from_, state.snapshot(), n
 
 
 def summary(tag: str, res) -> str:

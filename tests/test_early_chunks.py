@@ -4,6 +4,7 @@ import ctypes
 import os
 import sys
 
+import pytest
 import torch
 
 from conftest import REPO, golden
@@ -18,11 +19,11 @@ SKIP_CONV1 = ["n189.conv3x3", "n202.conv3x3", "n215.conv3x3", "n232.conv3x3", "n
               "n336.conv3x3", "n349.conv3x3"] + ["up.%d.block.%d.scatter_gather" % (u, b) for u in (2, 1, 0) for b in (0, 1, 2)]
 
 
-def test_ddpm256_step_marks_the_shortcut_and_skip_launches():
-    """Exactly the 20 fused-shortcut conv2s (bit 2) and the 18 up-path conv1s on cat([h, skip]) (bit 1) get a mask; no marked group
-    is written by the preceding step, which is always a tile conv; their predecessors, and only those, release early."""
+def _ddpm256(**opts):
     from test_fused_cpu import _prepared
 
+    import fused_step_contract as fsc
+    import pdl_hazards as ph
     from sige_b200.fused import FusedStep
     from sige_b200.workloads.ddpm import DDPMConfig
     from sim_executor import SimExecutor
@@ -30,35 +31,55 @@ def test_ddpm256_step_marks_the_shortcut_and_skip_launches():
     G = golden("ddpm256_golden.npz")
     model, x1, t = _prepared("intree", DDPMConfig(), float(G["ratio"][0]))
     with torch.no_grad():
-        step = FusedStep(model, x1, t, executor=SimExecutor())
+        return model, FusedStep(model, x1, t, executor=fsc.recording(ph.planned(SimExecutor))(), **opts)
+
+
+def test_ddpm256_step_marks_the_shortcut_and_skip_launches(cabi_lib):
+    """Exactly the 20 fused-shortcut conv2s (bit 2) and the 18 up-path conv1s on cat([h, skip]) (bit 1) get a mask, each after a
+    wgmma tile conv; their predecessors, and only those, release early; and no launch of the step reads, before its wait, a line
+    that a launch possibly running beside it writes (tests/pdl_hazards.py)."""
+    import pdl_hazards as ph
+
+    model, step = _ddpm256()
     assert len(step.fused) == 86
     marked = {f.name: f.spec.early for f in step.fused if f.spec.early}
     assert marked == {**{n: 4 for n in SHORTCUT_CONV2}, **{n: 2 for n in SKIP_CONV1}}
-    by_pos = {f.pos: f for f in step.fused}
     kinds = [k for k, _ in step.steps]
-    releasers = set()
+    es = {e.pos: e for e in ph.entries(step)}
     for f in step.fused:
-        if not f.spec.early:
-            continue
-        assert kinds[f.pos - 1] == "conv", "%s follows a %s step" % (f.name, kinds[f.pos - 1])
-        prev = by_pos[f.pos - 1].spec
-        written = {v.untyped_storage().data_ptr() for (v, _, _, _) in prev.aux}
-        if prev.dst is not None and prev.dst.has_raw:
-            written.add(prev.dst.raw.untyped_storage().data_ptr())
-        groups = [[t_] for t_, _ in f.spec.srcs] + [[]] * (2 - len(f.spec.srcs)) + [list(f.spec.shortcut[0]) if f.spec.shortcut else []]
-        for g, reads in enumerate(groups):
-            if (f.spec.early >> g) & 1:
-                assert reads and not any(r.untyped_storage().data_ptr() in written for r in reads), (f.name, g)
-        releasers.add(f.pos - 1)
-    assert {f.pos for f in step.fused if f.spec.early_release} == releasers
-    # after an attention core or a glue step nothing is marked
-    for f in step.fused:
-        if f.pos > 0 and kinds[f.pos - 1] != "conv":
-            assert f.spec.early == 0
+        if f.spec.early:
+            assert kinds[f.pos - 1] == "conv" and es[f.pos - 1].kernel == "wgmma", "%s follows a %s" % (f.name, es[f.pos - 1].kernel)
+    assert {f.pos for f in step.fused if f.spec.early_release} == {f.pos - 1 for f in step.fused if f.spec.early}
+    st = ph.verify(step, "ddpm256", model)["main then main"]
+    assert st.early == 2 * 38
     # without programmatic dependent launch there is nothing to overlap
-    with torch.no_grad():
-        plain = FusedStep(model, x1, t, executor=SimExecutor(), pdl=False)
+    _, plain = _ddpm256(pdl=False)
     assert not any(f.spec.early or f.spec.early_release for f in plain.fused)
+    assert not any(e.pdl for e in ph.entries(plain) if e.kernel in ("wgmma", "mma.sync"))
+
+
+def test_early_marks_that_ignore_what_the_predecessor_writes_are_rejected_by_name(cabi_lib, monkeypatch):
+    """`_early_masks` marking every group, `written` or not: each skip conv1 then reads h, which its predecessor writes, before
+    its wait."""
+    import pdl_hazards as ph
+    from sige_b200.fused import Lowering
+
+    def every_group(self):
+        self._conv_at = {fc.pos: fc for fc in self.fused}
+        for fc in self.fused:
+            s, prev = fc.spec, self._conv_at.get(fc.pos - 1)
+            if s.pdl and s.tc5 and prev is not None and prev.spec.pdl and prev.spec.tc5:
+                s.early = sum(1 << g for g, views in enumerate(ph.early_groups(s)) if views)
+                prev.spec.early_release = bool(s.early)
+
+    monkeypatch.setattr(Lowering, "_early_masks", every_group)
+    model, step = _ddpm256()
+    seq = ph.entries(step)
+    found = ph.hazards(seq, ph.storage_names(step, model))
+    for name in SKIP_CONV1:
+        assert any(h.startswith("main launch") and "(%s, wgmma) reads early group 0 src0 before its wait" % name in h for h in found), name
+    with pytest.raises(AssertionError, match=r"PDL hazards; the first: main launch \d+ \(.*, wgmma\) reads early group \d"):
+        ph.check(seq)
 
 
 def _desc(cin, cout, n_tiles, *, srcs=None, cin2=0, early=0, ksplit=0, res=64):

@@ -70,7 +70,11 @@ def _step(model, *args, step_dtype, executor_cls=None, **opts):
 
 
 def _walk_and_replay(step, tag, program=None, model=None, replays=True):
-    """(a) the walk, (c) every non-eager entry checked, (b) graph replay and eager run bitwise equal to the walk."""
+    """(a) the walk, (c) every non-eager entry checked, (b) graph replay and eager run bitwise equal to the walk; then (d) the walk
+    again from the start with the program's write footprint poisoned, which must end where the first walk ended outside the
+    padding rows, and (e) graph replay and eager run from that poisoned start bitwise equal to the poisoned walk.  The start
+    holds every intermediate a run on the same inputs left there, so only (d) and (e) see a launch that reads a byte before the
+    launch that writes it (in program order, or under programmatic dependent launch) has written it."""
     t0 = time.perf_counter()
     fsc.poison_padding(step)                 # (the walk poisons them too: replays start from the same padding rows)
     state = fsc.State(step, model)
@@ -83,15 +87,42 @@ def _walk_and_replay(step, tag, program=None, model=None, replays=True):
         # the sparse_update epilogue: its first call runs it and captures it, the second replays the captured graph
         runs = ([("replay", step.replay), ("run_eager", step.run_eager)] if program is None else
                 [("sparse_update (launches)", step.sparse_update), ("sparse_update (graph replay)", step.sparse_update)])
-        for name, run in runs:
-            state.restore(start)
-            torch.cuda.synchronize()
-            with torch.no_grad():
-                run()
-            torch.cuda.synchronize()
-            diff = state.differs(walked)
-            assert diff is None, "%s: %s leaves the state different from the synchronised walk: %s" % (tag, name, diff)
-    print(fsc.summary(tag, res) + "; %.2f s with replays" % (time.perf_counter() - t0))
+        _replay(state, start, walked, runs, tag, "the synchronised walk")
+    t1 = time.perf_counter()
+    res2, poisoned, walked2, n = fsc.poisoned_walk(step, res, start, walked, program, model=model, state=state)
+    fsc.checked_all(step, res2, program)
+    if replays:
+        runs = ([("replay", step.replay), ("run_eager", step.run_eager)] if program is None else
+                [("sparse_update (graph replay)", step.sparse_update), ("sparse_update (launches)", lambda: step._run(step.low.epilogue))])
+        _replay(state, poisoned, walked2, runs, tag + " (poisoned)", "the poisoned walk")
+    print(fsc.summary(tag, res) + "; %.2f s with replays; %d bytes poisoned, +%.2f s" % (time.perf_counter() - t0, n, time.perf_counter() - t1))
+    return res
+
+
+def _replay(state, start, walked, runs, tag, what):
+    for name, run in runs:
+        state.restore(start)
+        torch.cuda.synchronize()
+        with torch.no_grad():
+            run()
+        torch.cuda.synchronize()
+        diff = state.differs(walked)
+        assert diff is None, "%s: %s leaves the state different from %s: %s" % (tag, name, what, diff)
+
+
+def _walk_loads_and_replay(step, tag, model):
+    """walk_loads, then again from its write footprint poisoned, then `load_caches` from that poisoned start: bitwise equal to
+    the poisoned walk."""
+    t0 = time.perf_counter()
+    state = fsc.State(step, model)
+    start = state.snapshot()
+    res = fsc.walk_loads(step, model=model, state=state)
+    walked = state.snapshot()
+    t1 = time.perf_counter()
+    _, poisoned, walked2, n = fsc.poisoned_walk(step, res, start, walked, model=model, state=state, loads=True)
+    stream = torch.cuda.current_stream().cuda_stream
+    _replay(state, poisoned, walked2, [("load_caches", lambda: step.low.load_caches(stream))], tag + " (poisoned)", "the poisoned walk")
+    print(fsc.summary(tag, res) + "; %d bytes poisoned, +%.2f s" % (n, time.perf_counter() - t1))
     return res
 
 
@@ -326,8 +357,7 @@ def test_sd_decoder_step_meets_its_records_before_and_after_a_rebind(dtype):
     net.set_masks(downsample_mask(mask2, min_res=(4, 4), dilation=0))
     with torch.no_grad():
         assert step.rebind()
-    res = fsc.walk_loads(step, model=net)
-    print(fsc.summary("sd_decoder mini %s loads after rebind" % dtype, res))
+    _walk_loads_and_replay(step, "sd_decoder mini %s loads after rebind" % dtype, net)
     _sd_launches(step, _walk_and_replay(step, "sd_decoder mini %s after rebind" % dtype, model=net))
 
 
@@ -388,8 +418,7 @@ def test_cache_loads_meet_their_records_after_a_refresh_and_after_a_rebind():
         model((x0 * 0.7).to(DEV).half(), t)
         model.set_mode("sparse")
         assert step.refresh()
-    res = fsc.walk_loads(step, model=model)
-    print(fsc.summary("ddpm_small fp16 loads after refresh", res))
+    res = _walk_loads_and_replay(step, "ddpm_small fp16 loads after refresh", model)
     assert res["kinds"]["cache_load"].launches == 1
 
     import consumers
@@ -401,8 +430,7 @@ def test_cache_loads_meet_their_records_after_a_refresh_and_after_a_rebind():
     step = _step(net, consumers.gaugan_inputs("mini")[1].to(DEV), step_dtype=torch.float16)
     with torch.no_grad():
         assert step.rebind()
-    res = fsc.walk_loads(step, model=net)
-    print(fsc.summary("gaugan_spade mini fp16 loads after rebind", res))
+    res = _walk_loads_and_replay(step, "gaugan_spade mini fp16 loads after rebind", net)
     assert res["kinds"]["cache_load"].launches == 1
 
 
