@@ -259,7 +259,9 @@ typedef struct {
      * 0 (the reference's layout, sige/cuda/gather_kernel.cu:30): every image of the batch uses the same N tile origins.
      * 1: `idx` (and `sc_flags`) hold B*N entries, row b*N + i = tile i of image b — each edit has its own mask; lists shorter
      * than N are padded with SIGE_TILE_NONE origins (such a tile reads zeros and writes nothing).  Weights are read once for
-     * the whole batch.  Full-tensor source and destination only (no stacks).  A window source (src_pixel_stride) or a modulated
+     * the whole batch.  One side may be a tile stack of B*N rows, stack row b*N + i = list row b*N + i: a stack destination's
+     * SIGE_TILE_NONE rows write nothing to their stack rows; a stack source's row r is written to image r / N at that row's own
+     * origin, with the residual, scale and shift of that image.  Stack to stack is refused.  A window source (src_pixel_stride) or a modulated
      * one (modulation) takes per-image lists only with SIGE_CONV_PER_IMAGE_OPERANDS in `flags`. */
     int idx_per_image;
     /* ---- single source read as a channel window of a wider NHWC buffer ----
@@ -286,7 +288,7 @@ typedef struct {
 /* Use the wgmma / TMA kernel when the geometry allows (3x3 s1 on 6x6 tiles, 1x1 on 4x4 tiles,
  * Cout % 64 == 0); otherwise the mma.sync kernel runs. */
 #define SIGE_CONV_TC5 2
-/* `idx` is a fixed-capacity list (B == 1), or B of them (idx_per_image == 1): real tiles packed at the front of each list,
+/* `idx` is a fixed-capacity list (B == 1), or B of them (idx_per_image == 1, a stack on one side included): real tiles packed at the front of each list,
  * SIGE_TILE_NONE entries behind them, possibly whole CTAs' worth — CTAs made only of padding exit at once.  With per-image lists
  * the flag takes effect only when N is a multiple of the kernel's tiles per CTA (8 for the stride-1 geometries of either kernel,
  * 32 for the wgmma stride-2 one, the plan's tiles per CTA on the mma.sync kernel), so that no CTA holds tiles of two images.
@@ -311,7 +313,7 @@ typedef struct {
 /* A batch of INDEPENDENT EDITS (sige_tile_conv_t.flags and sige_separable_conv_t.flags): every operand of the launch holds B
  * images — the source or its window, gamma and beta of the modulation, the destinations — image b of each at b * H * W * (its
  * pixel stride), and the launch reads per-image tile lists: row b*N + i of `idx` is tile i of image b, a SIGE_TILE_NONE row reads
- * zeros and writes nothing.  sige_tile_conv: needs idx_per_image == 1 (and so full-tensor source and destination); it is what lets
+ * zeros and writes nothing.  sige_tile_conv: needs idx_per_image == 1 and full-tensor source and destination; it is what lets
  * a window or a modulated source take per-image lists.  sige_separable_conv: needs an NHWC buffer source and buffer destinations
  * (no stacks).  Both refuse the flag otherwise, before any CUDA call; SIGE_CONV_PADDED behaves as for per-image lists. */
 #define SIGE_CONV_PER_IMAGE_OPERANDS 128

@@ -376,7 +376,7 @@ tile_conv_mma_kernel(const __grid_constant__ ConvParams p) {
             hh += (p.offH + __ldg(p.idx + 2 * nn)) / p.stride;
             ww += (p.offW + __ldg(p.idx + 2 * nn + 1)) / p.stride;
             img = t / p.N;
-        } else if (p.idx && __ldg(p.idx + 2 * (t % p.N)) <= SIGE_TILE_NONE) {
+        } else if (p.idx && __ldg(p.idx + 2 * (p.idx_per_image ? t : t % p.N)) <= SIGE_TILE_NONE) {
             continue;                                  // a padding entry of the list writes nothing to its stack row
         }
         if (hh < 0 || hh >= p.dH || ww < 0 || ww >= p.dW) continue;
@@ -640,7 +640,7 @@ extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) {
         SIGE_REQUIRE(x.act == SIGE_ACT_IDENTITY || x.act == SIGE_ACT_SWISH || x.act == SIGE_ACT_RELU, "sige_tile_conv: aux %d unknown activation", i);
     }
 
-    SIGE_REQUIRE(!a->idx_per_image || (!a->src_is_stack && !a->dst_is_stack), "sige_tile_conv: per-image tile lists need full-tensor source and destination");
+    SIGE_REQUIRE(!a->idx_per_image || !a->src_is_stack || !a->dst_is_stack, "sige_tile_conv: per-image tile lists need a full-tensor source or destination (stack to stack is not supported)");
     SIGE_REQUIRE(a->n_src2 >= 0 && a->n_src2 <= 2, "sige_tile_conv: n_src2 must be 0, 1 or 2");
     if (a->n_src2 > 0) {
         int c2 = 0;
@@ -667,8 +667,9 @@ extern "C" int sige_tile_conv(const sige_tile_conv_t *a, sige_stream_t stream) {
     p.N = a->N;
     p.NT = a->B * a->N;
     p.idx_per_image = a->idx_per_image ? 1 : 0;
-    // (per-image lists: launch_cfg keeps the flag only when a list is a whole number of CTAs, see tile_conv_tc5.cu)
-    p.padded = ((a->flags & SIGE_CONV_PADDED) && a->idx && !a->src_is_stack && !a->dst_is_stack && (a->B == 1 || a->idx_per_image)) ? 1 : 0;
+    // (per-image lists, which may have a stack on one side: launch_cfg keeps the flag only when a list is a whole number of CTAs,
+    // see tile_conv_tc5.cu)
+    p.padded = ((a->flags & SIGE_CONV_PADDED) && a->idx && (a->idx_per_image || (!a->src_is_stack && !a->dst_is_stack && a->B == 1))) ? 1 : 0;
     p.R = a->R; p.S = a->S; p.RS = a->R * a->S;
     p.scale = a->scale; p.shift = a->shift; p.affine_bstride = a->affine_bstride; p.act = a->act;
     p.w = a->w_packed; p.bias = a->bias;

@@ -1382,7 +1382,8 @@ int tc5_launch(const sige_tile_conv_t *a, cudaStream_t st) {
     const bool s2 = !m && tc5_is_s2(a);
     // a CTA's first index row is row tile0 of `idx`: one list (B == 1), or per-image lists whose length is a whole number of CTAs
     // (no CTA then holds tiles of two images, so padding behind one image's tiles fills whole CTAs)
-    p.padded = ((a->flags & SIGE_CONV_PADDED) && a->idx && !a->src_is_stack && !a->dst_is_stack &&
+    // (per-image lists may have a stack on one side; the list's row tile0 is then also the CTA's first stack row)
+    p.padded = ((a->flags & SIGE_CONV_PADDED) && a->idx && (a->idx_per_image || (!a->src_is_stack && !a->dst_is_stack)) &&
                 (a->B == 1 || (a->idx_per_image && a->N % (s2 ? tc5::S2_TILES : tc5::TILES) == 0))) ? 1 : 0;
     const tc5::Plan pl = tc5::decide(p.NT, p.Cin, p.C0, p.Cout, p.taps, p.Cin2, p.early, a->ksplit, s2);
     p.ksplit = pl.ksplit;

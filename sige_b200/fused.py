@@ -554,6 +554,12 @@ class CudaExecutor:
         (SIGE_CONV_PER_IMAGE_OPERANDS)?  Then the GauGAN generators' SPADE layers lower for a batch as for one edit."""
         return True
 
+    def per_image_stacks_supported(self) -> bool:
+        """Can a tile conv of a batch of edits read per-edit lists with a tile stack on one side (sige_tile_conv_t.idx_per_image:
+        stack row b*N + i is list row b*N + i)?  Then SIGEAttnBlock's q conv and proj_out, and the sparse attention between
+        them, lower for a batch as for one edit."""
+        return True
+
     def prepare_writeback(self, entries) -> Callable[[int], None]:
         """One `sige_tile_writeback` over (src buffer, module cache, tile list, off, stride, output tile) entries."""
         return self.ops.tile_writeback_launcher(entries)
@@ -956,6 +962,8 @@ class Lowering:
         self.batch_slots = ok is not None and ok()
         ok = getattr(executor, "per_image_operands_supported", None)
         self.per_image_ops = self.batch_slots and ok is not None and ok()
+        ok = getattr(executor, "per_image_stacks_supported", None)
+        self.per_image_stacks = self.batch_slots and ok is not None and ok()
         self.module_names = module_names or {}
         self.pdl, self.tc5, self.producer_preop, self.fuse_shortcut = pdl, tc5, producer_preop, fuse_shortcut
         self.fused_attention, self.sparse_stem, self.ksplit = fused_attention, sparse_stem, ksplit
@@ -1154,7 +1162,7 @@ class Lowering:
         reads channels [c0, c1) of its single plain source (the spec holds that channel slice of the buffer)."""
         if stack_src is not None:            # rows are b*N + i (reference sige/cuda/gather_kernel.cu:30)
             B = dst.shape[0] if (dst is not None and idx is not None) else 1
-            n = int(stack_src.shape[0]) // B
+            n = int(stack_src.shape[0]) // (B if tile_img is None else 1)     # (per-image lists: one list row per stack row)
             assert idx is None or int(idx.shape[0]) == n, name
         else:
             B, n = segs[0][0].shape[0], int(idx.shape[0])
@@ -2026,6 +2034,8 @@ class Lowering:
         segs, pre, hw, idx, block, off, stack_src, timg = self.tile_conv_args(co)
         if stack_src is not None and gather is not None:      # a materialised stack scattered through `gather`'s tile set
             idx, off = co.src.slot.buf if co.src.slot is not None else gather.active_indices.to(self.dev), int(gather.offset[0])
+            if co.src.slot is not None:
+                timg = co.src.slot.tile_img        # (a batch: the slot's per-edit lists, one per E * cap stack row)
         self.emit_conv(name or ("n%d" % node.index), segs, pre, hw, idx, block, co.weight, co.bias, co.stride, off, dst, residual=residual,
                        shortcut=shortcut, stack_src=stack_src, tile_img=timg, cin_pad=co.cin_pad, epilogue=co.act, window=self._window_of(co))
 
@@ -2561,11 +2571,15 @@ class Lowering:
         Recognised at the first bmm, with every later node of the chain checked on the tape; then ONE `sige_sparse_attention`
         launch reads the q stack (written by the q conv's launch over the fixed-capacity tile list) and the k / v buffers in place
         (token stride C) and writes the NHWC tile stack that proj_out reads — padding tiles' rows are computed and never scattered.
+        A batch of E independent edits records every tile as a batch row of its own (b = tiles) against k[tile_images] /
+        v[tile_images], its edit's maps; it lowers, when the executor takes per-edit lists with a tile stack on one side
+        (`per_image_stacks_supported`), to the q conv over the slot's per-edit lists into an [E * cap] stack, one launch at B = E
+        (queries cap * bs * bs tokens of each edit's stack rows, keys and values its maps) and proj_out from that stack.
         Anything else keeps the recorded calls."""
         qa, kb = node.args[0], node.args[1]
-        if not (isinstance(qa, LazyTensor) and isinstance(kb, LazyTensor) and qa.dim() == 3 and kb.dim() == 3 and qa.shape[0] == 1):
+        if not (isinstance(qa, LazyTensor) and isinstance(kb, LazyTensor) and qa.dim() == 3 and kb.dim() == 3):
             return False
-        # queries: reshape(1, tiles * bs * bs, c) <- permute(0, 1, 3, 2) <- reshape(1, tiles, c, bs * bs) <- 1x1 conv on the tiles
+        # queries: reshape(b, tiles / b * bs * bs, c) <- permute(0, 1, 3, 2) <- reshape(b, tiles / b, c, bs * bs) <- 1x1 conv on the tiles
         q3 = qa
         p3 = q3.node.args[0] if q3.node is not None and q3.node.name in ("reshape", "view") else None
         r4 = p3.node.args[0] if isinstance(p3, LazyTensor) and p3.node is not None and p3.node.name == "permute" else None
@@ -2575,19 +2589,31 @@ class Lowering:
                 and co.stride == 1 and co.act is None and co.cin_pad == 0 and all(self.n_uses(t) == 1 for t in (q3, p3, r4, qc))):
             return False
         g = co.src.gather
+        timg = getattr(g, "tile_images", None)
+        if timg is not None and not self.per_image_stacks:
+            return False
         bs = int(g.block_size[0])
         nt, C = int(qc.shape[0]), int(qc.shape[1])
-        if (tuple(g.block_size) != (bs, bs) or tuple(qc.shape[2:]) != (bs, bs) or tuple(r4.shape) != (1, nt, C, bs * bs)
-                or tuple(int(d) for d in p3.node.args[1:]) != (0, 1, 3, 2) or tuple(q3.shape) != (1, nt * bs * bs, C)
-                or getattr(g, "tile_images", None) is not None or int(g.active_indices.shape[0]) != nt or nt == 0):
+        b = 1 if timg is None else nt            # bmm batch rows: the one image, or every tile of a batch of edits
+        per = nt // b
+        if (tuple(g.block_size) != (bs, bs) or tuple(qc.shape[2:]) != (bs, bs) or tuple(r4.shape) != (b, per, C, bs * bs)
+                or tuple(int(d) for d in p3.node.args[1:]) != (0, 1, 3, 2) or tuple(q3.shape) != (b, per * bs * bs, C)
+                or int(g.active_indices.shape[0]) != nt or nt == 0):
             return False
+        E = 1 if timg is None else int(g.num_edits)
 
-        def full_tokens(t):          # reshape(1, c, h * w) of a plain single-buffer map
+        def full_tokens(t):          # reshape(b, c, h * w) of a plain single-buffer map of E images (a batch: indexed by tile_images)
             if not (t.node is not None and t.node.name in ("reshape", "view") and self.n_uses(t) == 1):
                 return None
-            f = self.sym(t.node.args[0])
+            m = t.node.args[0]
+            if timg is not None:
+                if not (isinstance(m, LazyTensor) and m.node is not None and m.node.name == "__getitem__" and self.n_uses(m) == 1
+                        and len(m.node.args) == 2 and m.node.args[1] is timg and not m.node.kwargs):
+                    return None
+                m = m.node.args[0]
+            f = self.sym(m)
             buf = f.single if isinstance(f, Full) else None
-            if buf is None or tuple(buf.shape[:2]) != (1, C) or tuple(t.shape) != (1, C, buf.shape[2] * buf.shape[3]):
+            if buf is None or tuple(buf.shape[:2]) != (E, C) or tuple(t.shape) != (b, C, buf.shape[2] * buf.shape[3]):
                 return None
             return buf
 
@@ -2603,24 +2629,27 @@ class Lowering:
         bmm2 = self._sole_consumer(pt.outs[0], ("bmm",)) if pt is not None and tuple(int(d) for d in pt.args[1:]) == (0, 2, 1) else None
         vbuf = full_tokens(bmm2.args[0]) if bmm2 is not None and bmm2.args[1] is pt.outs[0] else None
         o5 = self._sole_consumer(bmm2.outs[0], ("reshape", "view")) if vbuf is not None else None
-        o5p = self._sole_consumer(o5.outs[0], ("permute",)) if o5 is not None and tuple(o5.outs[0].shape) == (1, C, nt, bs, bs) else None
+        o5p = self._sole_consumer(o5.outs[0], ("permute",)) if o5 is not None and tuple(o5.outs[0].shape) == (b, C, per, bs, bs) else None
         o4 = (self._sole_consumer(o5p.outs[0], ("reshape", "view"))
               if o5p is not None and tuple(int(d) for d in o5p.args[1:]) == (0, 2, 1, 3, 4) else None)
         if (o4 is None or tuple(o4.outs[0].shape) != (nt, C, bs, bs) or kbuf is None or tuple(vbuf.shape) != tuple(kbuf.shape)
                 or not (float(scale) > 0 and self.ex.sparse_attention_supported(C))):
             return False
-        # q: the conv's launch over the fixed-capacity list writes a capacity-row NHWC stack
-        segs, pre, hw, idx, block, off, stack_src, timg = self.tile_conv_args(co)
+        # q: the conv's launch over the fixed-capacity list(s) writes a capacity-row NHWC stack (E * cap rows for a batch)
+        segs, pre, hw, idx, block, off, stack_src, qimg = self.tile_conv_args(co)
         sl = self.slots.get(id(g.active_indices))
-        if stack_src is not None or timg is not None or sl is None or idx is not sl.buf or segs[0][0].shape[0] != 1:
+        if (stack_src is not None or sl is None or idx is not sl.buf or segs[0][0].shape[0] != E or sl.E != E
+                or (qimg is None) != (timg is None)):
             return False
-        cap = int(idx.shape[0])
-        q_st = torch.empty((cap, C, bs, bs), dtype=self.dtype, device=self.dev, memory_format=torch.channels_last)
-        self.emit_conv("n%d.q_stack" % co.node.index, segs, pre, hw, idx, block, co.weight, co.bias, co.stride, off, None, dst_stack=q_st)
+        rows = int(idx.shape[0])
+        # (zeros: the rows of padding tiles, which the q conv never writes, hold finite values for the attention to compute on)
+        q_st = torch.empty((rows, C, bs, bs), dtype=self.dtype, device=self.dev, memory_format=torch.channels_last).zero_()
+        self.emit_conv("n%d.q_stack" % co.node.index, segs, pre, hw, idx, block, co.weight, co.bias, co.stride, off, None, dst_stack=q_st,
+                       tile_img=qimg)
         o_st = torch.empty_like(q_st)
 
-        def tokens(t):               # [1, 1, tokens, C] view of an NHWC map or stack
-            return t.permute(0, 2, 3, 1).reshape(1, -1, C).unsqueeze(1)
+        def tokens(t):               # [E, 1, tokens, C] view of an NHWC map or stack of E images (a stack: its rows in edit order)
+            return t.permute(0, 2, 3, 1).reshape(E, -1, C).unsqueeze(1)
 
         for buf in (kbuf, vbuf):
             buf.readers.append(None)

@@ -112,6 +112,9 @@ class SIGEAttnBlock(SIGEModule):
         v = self.v_scatter(self.v(h))
         b = x.size(0)
         c = q.shape[1]
+        timg = self.gather.tile_images if sparse else None
+        if timg is not None:  # a batch of independent edits: each tile is a batch row of its own, against its edit's keys and values
+            k, v, b = k[timg], v[timg], q.shape[0]
         if sparse:            # [b * tiles, c, bs, bs] -> [b, tiles * bs * bs, c]: tile-major, then pixel order
             q = q.reshape(b, -1, c, self.block_size * self.block_size).permute(0, 1, 3, 2).reshape(b, -1, c)
         else:
@@ -188,6 +191,11 @@ def build_sd_decoder(size: str = "mini") -> SIGEDecoder:
     return init_deterministic(SIGEDecoder(**SIZES[size]), seed=31).eval()
 
 
+def _latent_mask(mask: torch.Tensor, f: int) -> torch.Tensor:
+    res = mask.shape[0]
+    return mask.view(res // f, f, res // f, f).any(3).any(1)
+
+
 def sd_decoder_inputs(size: str = "mini", seed: int = 4):
     """(z0, z1, mask): the original latent, the edited one and the edit mask at IMAGE resolution.  full: BASELINE.json's
     centred 15 % square of the 512 x 512 image; mini: a 10 x 14 rectangle of the 32 x 32 image.  z1 differs from z0 on the
@@ -204,9 +212,32 @@ def sd_decoder_inputs(size: str = "mini", seed: int = 4):
         mask[lo:lo + side, lo:lo + side] = True
     else:
         mask[9:19, 13:27] = True
-    latent_mask = mask.view(res // f, f, res // f, f).any(3).any(1)
-    z1 = z0 + torch.from_numpy(rng.standard_normal(tuple(z0.shape)).astype(np.float32)) * latent_mask
+    z1 = z0 + torch.from_numpy(rng.standard_normal(tuple(z0.shape)).astype(np.float32)) * _latent_mask(mask, f)
     return z0, z1, mask
+
+
+# Edits 1, 2, ... of sd_decoder_edits as (top, left, height, width) fractions of the image: a smaller one, one along the left border,
+# one in the bottom-right corner (cycled for more edits).
+_OTHER_EDITS = ((0.62, 0.12, 0.19, 0.19), (0.25, 0.0, 0.44, 0.16), (0.8, 0.75, 0.2, 0.25))
+
+
+def sd_decoder_edits(size: str = "mini", E: int = 3, seed: int = 4):
+    """(z0, z1s, masks): E INDEPENDENT EDITS of one latent z0 — z1s [E, 4, h, w], masks [E, H, W] at image resolution.  Edit 0 is
+    sd_decoder_inputs' (z1, mask); the others have other sizes and places, one of them on the image border.  Edit e's latent
+    differs from z0 on the latent pixels its mask touches."""
+    z0, z1, mask = sd_decoder_inputs(size, seed)
+    res = mask.shape[0]
+    f = res // z0.shape[2]
+    rng = np.random.default_rng(seed + 1)
+    z1s, masks = [z1], [mask]
+    for e in range(1, E):
+        top, left, h, w = _OTHER_EDITS[(e - 1) % len(_OTHER_EDITS)]
+        m = torch.zeros(res, res, dtype=torch.bool)
+        y0, x0 = int(top * res), int(left * res)
+        m[y0:y0 + max(1, int(round(h * res))), x0:x0 + max(1, int(round(w * res)))] = True
+        masks.append(m)
+        z1s.append(z0 + torch.from_numpy(rng.standard_normal(tuple(z0.shape)).astype(np.float32)) * _latent_mask(m, f))
+    return z0, torch.cat(z1s, 0), torch.stack(masks, 0)
 
 
 def run_sd_decoder(net, downsample_mask, size: str = "mini", device="cpu", fused=None):

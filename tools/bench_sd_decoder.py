@@ -14,6 +14,15 @@ events):
 Then the next edit (a second, smaller mask): the wall time from `set_masks` / `set_masks_async` to the synchronised end of the step
 that follows, against a recompile (set_fused + the first call), three times each.  Prints the launch mix of both compiled steps,
 the GPU's name, power limit and SM clock read in the same run, and one JSON line.
+
+    python tools/bench_sd_decoder.py --size full --edits E
+
+E independent edits of the latent (sd_decoder_edits: edit 0 is the one above, the others smaller, larger, on the border), arms
+alternated as above:
+  batched      ONE compiled fp16 step over the batch of E edits (per-edit tile lists, headroom 0.5)
+  singles      E compiled single-edit fp16 steps, one after another
+Then the next batch (edits E .. 2E-1, each list within the first batch's capacities) installed through `set_masks` and through
+`set_masks_async`, against a recompile, as above.
 """
 from __future__ import annotations
 
@@ -38,7 +47,10 @@ def main():
     ap.add_argument("--size", default="full", choices=["full", "mini"])
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--edits", type=int, default=1, help="E > 1: a batch of E independent edits in one step, against E single steps")
     args = ap.parse_args()
+    if args.edits > 1:
+        return batched(args)
 
     import torch
 
@@ -147,6 +159,105 @@ def main():
         "fused_core_recorded": mix(recorded),
         "core_recorded_vs_fused_rel_diff": err,
         "sparse_attention_launches": tokens,
+        "steps": args.steps,
+    }
+    print(json.dumps(out))
+
+
+def _timed(arms, steps, warmup, flush):
+    import torch
+
+    times = {k: [] for k in arms}
+    for i in range(warmup + steps):
+        for name, fn in arms.items():
+            flush.zero_()
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            fn()
+            b.record()
+            torch.cuda.synchronize()
+            if i >= warmup:
+                times[name].append(a.elapsed_time(b))
+    return times
+
+
+def batched(args):
+    import torch
+
+    from sige.utils import downsample_mask
+    from sige_b200.masks import stack_mask_pyramids
+    from sige_b200.workloads import sd_decoder as SD
+
+    assert torch.cuda.is_available(), "bench_sd_decoder needs a GPU"
+    torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
+    dev = torch.device("cuda:0")
+    E = args.edits
+    net = SD.build_sd_decoder(args.size).to(dev)
+    z0, z1s, masks = (t.to(dev) for t in SD.sd_decoder_edits(args.size, 2 * E))
+    pyrs = [downsample_mask(m, min_res=(4, 4), dilation=0) for m in masks]
+    A, B = list(range(E)), list(range(E, 2 * E))
+    batch_a, batch_b = (stack_mask_pyramids([pyrs[e] for e in ids]) for ids in (A, B))
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
+    with torch.no_grad():
+        net.set_mode("full")
+        net(z0)
+        net.set_mode("sparse")
+        singles = []
+        for e in A:
+            net.set_fused(True, dtype=torch.float16)
+            net.set_masks(pyrs[e])
+            o = net(z1s[e:e + 1]).clone()
+            singles.append((net.fused_step, o))
+        net.set_fused(True, dtype=torch.float16, headroom=0.5)
+        net.set_masks(batch_a)
+        out = net(z1s[A]).clone()
+        step = net.fused_step
+        x_a = z1s[A]
+        err = max(float((out[i:i + 1].float() - o.float()).abs().max() / o.float().abs().max()) for i, (_, o) in enumerate(singles))
+
+        def one_batch():
+            step(x_a)
+
+        def one_by_one():
+            for e, (s, _) in enumerate(singles):
+                s(z1s[e:e + 1])
+
+        times = _timed({"batched": one_batch, "singles": one_by_one}, args.steps, args.warmup, flush)
+
+        nxt = {"set_masks": [], "set_masks_async": [], "recompile": []}
+        in_place = True
+        for _ in range(3):
+            for how in nxt:
+                net.set_fused(True, dtype=torch.float16, headroom=0.5)
+                net.set_masks(batch_a)
+                net(x_a)
+                step = net.fused_step
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                if how == "set_masks":
+                    net.set_masks(batch_b)
+                elif how == "set_masks_async":
+                    net.set_masks_async(batch_b)
+                else:
+                    net.set_fused(True, dtype=torch.float16, headroom=0.5)
+                    net.set_masks(batch_b)
+                net(z1s[B])
+                torch.cuda.synchronize()
+                nxt[how].append((time.perf_counter() - t0) * 1e3)
+                if how != "recompile":
+                    in_place = in_place and net.fused_step is step and net.masks_async_ok()
+    caps = sorted({sl.cap for sl in step.low.slots.values()})
+    out = {
+        "workload": "sd_decoder_%s_batch_of_%d" % (args.size, E),
+        "edits": [int(m.sum()) for m in masks[:E]],
+        "gpu": gpu_info(),
+        "ms_median": {k: statistics.median(v) for k, v in times.items()},
+        "ms_min": {k: min(v) for k, v in times.items()},
+        "batched_vs_singles_max_rel_diff": err,
+        "next_batch_ms_median": {k: statistics.median(v) for k, v in nxt.items()},
+        "next_batch_in_place": in_place,
+        "tile_list_capacities": caps,
+        "batched_steps": dict(Counter(k for k, _ in step.steps)),
         "steps": args.steps,
     }
     print(json.dumps(out))
