@@ -324,22 +324,36 @@ __global__ void __launch_bounds__(1024) gn_finalize_kernel(const float *__restri
 // ------------------------------------------------------------------------------------------
 // conv_out: y = conv3x3(act(x*scale+shift)), C -> Cout <= 8, output NCHW.
 // CTA = 8 x 32 output pixels, one warp per output row.  The (8+2) x (32+2) halo is transformed ONCE into shared
-// memory (row pitch C*2+16 bytes -> conflict-free ldmatrix), then the conv is an implicit GEMM on the legacy tensor
+// memory (row pitch cc*2+16 bytes -> conflict-free ldmatrix), then the conv is an implicit GEMM on the legacy tensor
 // path: M = 16 consecutive pixels of the row, N = 8 (Cout zero-padded), K = 9*C, mma.sync.m16n8k16; the A fragment of
 // tap (ky,kx) is a set of ldmatrix row pointers into the halo tile shifted by (ky,kx).
+// The halo holds cc channels at a time (cc divides C): all of them when they fit beside the weights, else the halo is
+// filled and consumed once per chunk of cc channels (the Stable Diffusion VAE encoder's 512-channel conv_out), with the
+// accumulators carried across chunks.  With cc == C the MMA order is the single-fill order.
 // ------------------------------------------------------------------------------------------
 constexpr int CO_TH = 8, CO_TW = 32;
+
+static size_t conv_out_smem(int C, int cc) {
+    return (((size_t)(CO_TH + 2) * (CO_TW + 2) * (cc * 2 + 16) + 15) & ~(size_t)15) + (size_t)8 * (9 * C * 2 + 16);
+}
+
+// Channels per halo fill: the largest multiple of 16 that divides C and fits in shared memory beside the weights (0: none).
+static int conv_out_chunk(int C) {
+    for (int cc = C; cc >= 16; cc -= 16)
+        if (C % cc == 0 && conv_out_smem(C, cc) <= 227 * 1024) return cc;
+    return 0;
+}
 
 template <typename T>
 __global__ void __launch_bounds__(CO_TH * 32) conv_out_kernel(const T *__restrict__ x, const float *__restrict__ scale,
                                                                 const float *__restrict__ shift, int act, const T *__restrict__ w,
                                                                 const T *__restrict__ bias, T *__restrict__ out, int B, int H, int W,
-                                                                int C, int Cout) {
+                                                                int C, int Cout, int cc) {
     extern __shared__ __align__(16) unsigned char smraw[];
-    const int pitch = C * 2 + 16;
+    const int pitch = cc * 2 + 16;
     const int HP = CO_TH + 2, WP = CO_TW + 2;
     const int K = 9 * C, wpitch = K * 2 + 16;                                 // bytes per weight row (odd number of 16-byte units)
-    unsigned char *tile = smraw;                                             // [HP*WP][pitch]
+    unsigned char *tile = smraw;                                             // [HP*WP][pitch]: channels c0 .. c0+cc-1
     unsigned char *wsm = smraw + ((HP * WP * pitch + 15) & ~15);             // [8][wpitch]: B operand, row n = output channel
     const int b = blockIdx.z, ty0 = blockIdx.y * CO_TH, tx0 = blockIdx.x * CO_TW;
     {
@@ -362,86 +376,89 @@ __global__ void __launch_bounds__(CO_TH * 32) conv_out_kernel(const T *__restric
             }
         }
     }
-    const int CV = C / 8;
+    const int CV = cc / 8;
     const bool pre = scale || shift || act != SIGE_ACT_IDENTITY;
     pdl_release();
     pdl_acquire();                 // the weights above are constants; x, scale and shift come from the preceding kernels
-    if (blockDim.x % CV == 0) {
-        // every thread keeps ONE channel octet for all its pixels: its 8 (scale, shift) pairs live in registers and the
-        // pixel walk is a fixed stride (the pre-op — 11 M SiLU evaluations per 256x256x128 step — is this kernel's cost)
-        const int cv = threadIdx.x % CV, pstep = blockDim.x / CV;
-        float sc[8], sh[8];
-#pragma unroll
-        for (int z = 0; z < 8; ++z) {
-            sc[z] = scale ? __ldg(scale + (long long)b * C + cv * 8 + z) : 1.f;
-            sh[z] = shift ? __ldg(shift + (long long)b * C + cv * 8 + z) : 0.f;
-        }
-        // loads are issued in batches of HB before any is consumed: one DRAM round trip per batch instead of per pixel
-        constexpr int HB = 8;
-        for (int pp0 = threadIdx.x / CV; pp0 < HP * WP; pp0 += pstep * HB) {
-            uint4 v[HB];
-            bool ok[HB];
-#pragma unroll
-            for (int j = 0; j < HB; ++j) {
-                const int pp = pp0 + j * pstep;
-                const int py = pp / WP, px = pp - py * WP;
-                const int hh = ty0 + py - 1, ww = tx0 + px - 1;
-                ok[j] = pp < HP * WP && hh >= 0 && hh < H && ww >= 0 && ww < W;
-                v[j] = make_uint4(0, 0, 0, 0);
-                if (ok[j]) v[j] = __ldg(reinterpret_cast<const uint4 *>(x + (((long long)b * H + hh) * W + ww) * C + cv * 8));
-            }
-#pragma unroll
-            for (int j = 0; j < HB; ++j) {
-                const int pp = pp0 + j * pstep;
-                if (pp >= HP * WP) break;
-                if (pre && ok[j]) {
-                    T *el = reinterpret_cast<T *>(&v[j]);
-#pragma unroll
-                    for (int z = 0; z < 8; ++z) el[z] = DT<T>::from_f(activate<true>(act, fmaf(DT<T>::to_f(el[z]), sc[z], sh[z])));
-                }
-                *reinterpret_cast<uint4 *>(tile + pp * pitch + cv * 16) = v[j];   // zero padding AFTER the pre-op
-            }
-        }
-    } else {
-        for (int e = threadIdx.x; e < HP * WP * CV; e += blockDim.x) {
-            const int cv = e % CV, pp = e / CV;
-            const int py = pp / WP, px = pp - py * WP;
-            const int hh = ty0 + py - 1, ww = tx0 + px - 1;
-            uint4 v = make_uint4(0, 0, 0, 0);
-            if (hh >= 0 && hh < H && ww >= 0 && ww < W) {
-                v = __ldg(reinterpret_cast<const uint4 *>(x + (((long long)b * H + hh) * W + ww) * C + cv * 8));
-                if (pre) {
-                    T *el = reinterpret_cast<T *>(&v);
-#pragma unroll
-                    for (int z = 0; z < 8; ++z) {
-                        const int c = cv * 8 + z;
-                        float f = DT<T>::to_f(el[z]);
-                        f = fmaf(f, scale ? scale[(long long)b * C + c] : 1.f, shift ? shift[(long long)b * C + c] : 0.f);
-                        el[z] = DT<T>::from_f(activate<true>(act, f));
-                    }
-                }
-            }
-            *reinterpret_cast<uint4 *>(tile + pp * pitch + cv * 16) = v;   // zero padding AFTER the pre-op
-        }
-    }
-    __syncthreads();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;            // warp = output row inside the tile
     float acc[2][4] = {{0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f}};
-    const uint32_t tbase = smem_u32(tile), wbase = smem_u32(wsm);
-    const int a_row = lane & 15, a_khalf = lane >> 4;                      // ldmatrix.x4: 16 pixel rows x {k-lo, k-hi}
-    const int b_row = lane & 7, b_khalf = (lane >> 3) & 1;                 // ldmatrix.x2: 8 channel rows x {k-lo, k-hi}
-    for (int tap = 0; tap < 9; ++tap) {
-        const int ky = tap / 3, kx = tap - 3 * ky;
-        const uint32_t arow0 = tbase + ((warp + ky) * WP + kx + a_row) * pitch + a_khalf * 16;
-        const uint32_t brow = wbase + b_row * wpitch + (tap * C) * 2 + b_khalf * 16;
-        for (int kk = 0; kk < C / 16; ++kk) {
-            uint32_t b0, b1;
-            asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0,%1}, [%2];\n" : "=r"(b0), "=r"(b1) : "r"(brow + kk * 32));
+    for (int c0 = 0; c0 < C; c0 += cc) {
+        if (c0) __syncthreads();       // every warp is done with the previous chunk's halo
+        if (blockDim.x % CV == 0) {
+            // every thread keeps ONE channel octet for all its pixels: its 8 (scale, shift) pairs live in registers and the
+            // pixel walk is a fixed stride (the pre-op — 11 M SiLU evaluations per 256x256x128 step — is this kernel's cost)
+            const int cv = threadIdx.x % CV, pstep = blockDim.x / CV;
+            float sc[8], sh[8];
 #pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                uint32_t a[4];
-                ldmatrix_x4(arow0 + i * 16 * pitch + kk * 32, a[0], a[1], a[2], a[3]);
-                mma_m16n8k16<T>(acc[i], a, b0, b1);
+            for (int z = 0; z < 8; ++z) {
+                sc[z] = scale ? __ldg(scale + (long long)b * C + c0 + cv * 8 + z) : 1.f;
+                sh[z] = shift ? __ldg(shift + (long long)b * C + c0 + cv * 8 + z) : 0.f;
+            }
+            // loads are issued in batches of HB before any is consumed: one DRAM round trip per batch instead of per pixel
+            constexpr int HB = 8;
+            for (int pp0 = threadIdx.x / CV; pp0 < HP * WP; pp0 += pstep * HB) {
+                uint4 v[HB];
+                bool ok[HB];
+#pragma unroll
+                for (int j = 0; j < HB; ++j) {
+                    const int pp = pp0 + j * pstep;
+                    const int py = pp / WP, px = pp - py * WP;
+                    const int hh = ty0 + py - 1, ww = tx0 + px - 1;
+                    ok[j] = pp < HP * WP && hh >= 0 && hh < H && ww >= 0 && ww < W;
+                    v[j] = make_uint4(0, 0, 0, 0);
+                    if (ok[j]) v[j] = __ldg(reinterpret_cast<const uint4 *>(x + (((long long)b * H + hh) * W + ww) * C + c0 + cv * 8));
+                }
+#pragma unroll
+                for (int j = 0; j < HB; ++j) {
+                    const int pp = pp0 + j * pstep;
+                    if (pp >= HP * WP) break;
+                    if (pre && ok[j]) {
+                        T *el = reinterpret_cast<T *>(&v[j]);
+#pragma unroll
+                        for (int z = 0; z < 8; ++z) el[z] = DT<T>::from_f(activate<true>(act, fmaf(DT<T>::to_f(el[z]), sc[z], sh[z])));
+                    }
+                    *reinterpret_cast<uint4 *>(tile + pp * pitch + cv * 16) = v[j];   // zero padding AFTER the pre-op
+                }
+            }
+        } else {
+            for (int e = threadIdx.x; e < HP * WP * CV; e += blockDim.x) {
+                const int cv = e % CV, pp = e / CV;
+                const int py = pp / WP, px = pp - py * WP;
+                const int hh = ty0 + py - 1, ww = tx0 + px - 1;
+                uint4 v = make_uint4(0, 0, 0, 0);
+                if (hh >= 0 && hh < H && ww >= 0 && ww < W) {
+                    v = __ldg(reinterpret_cast<const uint4 *>(x + (((long long)b * H + hh) * W + ww) * C + c0 + cv * 8));
+                    if (pre) {
+                        T *el = reinterpret_cast<T *>(&v);
+#pragma unroll
+                        for (int z = 0; z < 8; ++z) {
+                            const int c = c0 + cv * 8 + z;
+                            float f = DT<T>::to_f(el[z]);
+                            f = fmaf(f, scale ? scale[(long long)b * C + c] : 1.f, shift ? shift[(long long)b * C + c] : 0.f);
+                            el[z] = DT<T>::from_f(activate<true>(act, f));
+                        }
+                    }
+                }
+                *reinterpret_cast<uint4 *>(tile + pp * pitch + cv * 16) = v;   // zero padding AFTER the pre-op
+            }
+        }
+        __syncthreads();
+        const uint32_t tbase = smem_u32(tile), wbase = smem_u32(wsm);
+        const int a_row = lane & 15, a_khalf = lane >> 4;                      // ldmatrix.x4: 16 pixel rows x {k-lo, k-hi}
+        const int b_row = lane & 7, b_khalf = (lane >> 3) & 1;                 // ldmatrix.x2: 8 channel rows x {k-lo, k-hi}
+        for (int tap = 0; tap < 9; ++tap) {
+            const int ky = tap / 3, kx = tap - 3 * ky;
+            const uint32_t arow0 = tbase + ((warp + ky) * WP + kx + a_row) * pitch + a_khalf * 16;
+            const uint32_t brow = wbase + b_row * wpitch + (tap * C + c0) * 2 + b_khalf * 16;
+            for (int kk = 0; kk < cc / 16; ++kk) {
+                uint32_t b0, b1;
+                asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0,%1}, [%2];\n" : "=r"(b0), "=r"(b1) : "r"(brow + kk * 32));
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    uint32_t a[4];
+                    ldmatrix_x4(arow0 + i * 16 * pitch + kk * 32, a[0], a[1], a[2], a[3]);
+                    mma_m16n8k16<T>(acc[i], a, b0, b1);
+                }
             }
         }
     }
@@ -594,16 +611,16 @@ int sige_conv_out_nhwc(const void *x, const float *scale, const float *shift, in
     SIGE_REQUIRE(B > 0 && H > 0 && W > 0 && C > 0 && C % 16 == 0 && Cout >= 1 && Cout <= 8, "sige_conv_out_nhwc: needs C %% 16 == 0 and Cout <= 8");
     SIGE_REQUIRE(act == SIGE_ACT_IDENTITY || act == SIGE_ACT_SWISH, "sige_conv_out_nhwc: unknown activation %d", act);
     SIGE_REQUIRE(((uintptr_t)x & 15) == 0, "sige_conv_out_nhwc: input not 16-byte aligned");
-    const int pitch = C * 2 + 16;
-    const size_t smem = (((size_t)(CO_TH + 2) * (CO_TW + 2) * pitch + 15) & ~(size_t)15) + (size_t)8 * (9 * C * 2 + 16);
-    SIGE_REQUIRE(smem <= 227 * 1024, "sige_conv_out_nhwc: %d channels do not fit in shared memory", C);
+    const int cc = conv_out_chunk(C);
+    SIGE_REQUIRE(cc > 0, "sige_conv_out_nhwc: %d channels do not fit in shared memory", C);
+    const size_t smem = conv_out_smem(C, cc);
     dim3 grid((W + CO_TW - 1) / CO_TW, (H + CO_TH - 1) / CO_TH, B);
     cudaStream_t st = (cudaStream_t)stream;
 #define SIGE_CO(T)                                                                                                        \
     do {                                                                                                                  \
         cudaFuncSetAttribute(conv_out_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);                  \
         (void)launch_ex(conv_out_kernel<T>, grid, dim3(CO_TH * 32), smem, st, true, dim3(1, 1, 1), (const T *)x, scale, shift, act,  \
-                        (const T *)w, (const T *)bias, (T *)out, B, H, W, C, Cout);                                               \
+                        (const T *)w, (const T *)bias, (T *)out, B, H, W, C, Cout, cc);                                               \
     } while (0)
     switch (dtype) {
         case SIGE_F16: SIGE_CO(__half); break;

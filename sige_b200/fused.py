@@ -508,10 +508,12 @@ class CudaExecutor:
         return self.ops.attention_tokens_supported(n_tokens, channels, self.dtype)
 
     def tail_supported(self, channels: int, cout: int) -> bool:
-        """sige_conv_out_nhwc stages a 10 x 34 pixel halo tile and the weights of all channels in shared memory (<= 227 KB)."""
-        pitch = channels * 2 + 16
-        smem = ((10 * 34 * pitch + 15) & ~15) + 8 * (9 * channels * 2 + 16)      # (CO_TH + 2) x (CO_TW + 2) = 10 x 34 pixels
-        return cout <= 8 and channels % 16 == 0 and channels <= 1024 and smem <= 227 * 1024
+        """sige_conv_out_nhwc stages the weights of all channels and a 10 x 34 pixel halo tile in shared memory (<= 227 KB); the
+        halo holds cc channels at a time, cc a multiple of 16 that divides the channels (all of them when they fit)."""
+        weights = 8 * (9 * channels * 2 + 16)
+        fits = any(channels % cc == 0 and ((10 * 34 * (cc * 2 + 16) + 15) & ~15) + weights <= 227 * 1024   # (CO_TH + 2) x (CO_TW + 2)
+                   for cc in range(16, channels + 1, 16))
+        return cout <= 8 and channels % 16 == 0 and channels <= 1024 and fits
 
     def prepare_attention(self, qkv_tokens: torch.Tensor, out_tokens: torch.Tensor, pdl: bool):
         ops = self.ops

@@ -1,12 +1,14 @@
-"""Time the Stable Diffusion VAE decoder's sparse step on one GPU.
+"""Time the Stable Diffusion VAE decoder's (or encoder's) sparse step on one GPU.
 
-    python tools/bench_sd_decoder.py [--size full|mini] [--steps 20] [--warmup 5]
+    python tools/bench_sd_decoder.py [--model decoder|encoder] [--size full|mini] [--steps 20] [--warmup 5]
 
-Workload: sige_b200/workloads/sd_decoder.py — "full" is the first-stage decoder of stable-diffusion/configs/sige.yaml, z 4 x 64 x 64
--> 512 x 512, with BASELINE.json's centred 15 % square edit and the SDEdit runner's mask pyramid (min_res 4 x 4, dilation 0).
+Workload: sige_b200/workloads/sd_decoder.py (the default) — "full" is the first-stage decoder of stable-diffusion/configs/sige.yaml,
+z 4 x 64 x 64 -> 512 x 512 — or, with --model encoder, sige_b200/workloads/sd_encoder.py — the first-stage encoder of the same
+config, image 3 x 512 x 512 -> moments 8 x 64 x 64 — with BASELINE.json's centred 15 % square edit and the SDEdit runner's mask
+pyramid (min_res 4 x 4, dilation 0).
 Arms, alternated step by step in one process (CUDA events around each call, an L2 flush (256 MiB write) between calls outside the
 events):
-  dense        the decoder's full (dense) pass, fp32, on the original latent
+  dense        the model's full (dense) pass, fp32, on the original input
   modules      the sparse pass through the eager fp32 operator modules
   fused        the compiled fused fp16 step (CUDA graph)
   fused_core_recorded   the same step with the mid block's attention core left to its recorded torch calls (an executor without
@@ -15,9 +17,9 @@ Then the next edit (a second, smaller mask): the wall time from `set_masks` / `s
 that follows, against a recompile (set_fused + the first call), three times each.  Prints the launch mix of both compiled steps,
 the GPU's name, power limit and SM clock read in the same run, and one JSON line.
 
-    python tools/bench_sd_decoder.py --size full --edits E
+    python tools/bench_sd_decoder.py [--model decoder|encoder] --size full --edits E
 
-E independent edits of the latent (sd_decoder_edits: edit 0 is the one above, the others smaller, larger, on the border), arms
+E independent edits of the input (sd_decoder_edits / sd_encoder_edits: edit 0 is the one above, the others smaller, larger, on the border), arms
 alternated as above:
   batched      ONE compiled fp16 step over the batch of E edits (per-edit tile lists, headroom 0.5)
   singles      E compiled single-edit fp16 steps, one after another
@@ -42,8 +44,20 @@ sys.path.insert(0, os.path.join(REPO, "tools"))
 from bench_gaugan_gc import gpu_info  # noqa: E402
 
 
+def _workload(model):
+    """(build, inputs, edits) of the model: build(size) -> net, inputs(size) -> (x0, x1, mask), edits(size, E) -> (x0, x1s, masks)."""
+    if model == "encoder":
+        from sige_b200.workloads import sd_encoder as SE
+
+        return SE.build_sd_encoder, SE.sd_encoder_inputs, SE.sd_encoder_edits
+    from sige_b200.workloads import sd_decoder as SD
+
+    return SD.build_sd_decoder, SD.sd_decoder_inputs, SD.sd_decoder_edits
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--model", default="decoder", choices=["decoder", "encoder"])
     ap.add_argument("--size", default="full", choices=["full", "mini"])
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
@@ -56,13 +70,13 @@ def main():
 
     from sige.utils import downsample_mask
     from sige_b200.fused import CudaExecutor, FusedStep
-    from sige_b200.workloads import sd_decoder as SD
 
     assert torch.cuda.is_available(), "bench_sd_decoder needs a GPU"
     torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
     dev = torch.device("cuda:0")
-    net = SD.build_sd_decoder(args.size).to(dev)
-    z0, z1, mask = (t.to(dev) for t in SD.sd_decoder_inputs(args.size))
+    build, inputs, _ = _workload(args.model)
+    net = build(args.size).to(dev)
+    z0, z1, mask = (t.to(dev) for t in inputs(args.size))
     res = mask.shape[0]
     mask2 = torch.zeros_like(mask)
     lo = res // 2 - res // 8
@@ -148,7 +162,7 @@ def main():
 
     tokens = int(step.low.sparse_attention_calls)
     out = {
-        "workload": "sd_decoder_%s" % args.size,
+        "workload": "sd_%s_%s" % (args.model, args.size),
         "edit": "centred 15 %% square of the %d x %d image, min_res 4 x 4, dilation 0" % (res, res),
         "gpu": gpu_info(),
         "ms_median": {k: statistics.median(v) for k, v in times.items()},
@@ -186,14 +200,14 @@ def batched(args):
 
     from sige.utils import downsample_mask
     from sige_b200.masks import stack_mask_pyramids
-    from sige_b200.workloads import sd_decoder as SD
 
     assert torch.cuda.is_available(), "bench_sd_decoder needs a GPU"
     torch.backends.cudnn.allow_tf32 = torch.backends.cuda.matmul.allow_tf32 = False
     dev = torch.device("cuda:0")
     E = args.edits
-    net = SD.build_sd_decoder(args.size).to(dev)
-    z0, z1s, masks = (t.to(dev) for t in SD.sd_decoder_edits(args.size, 2 * E))
+    build, _, edits = _workload(args.model)
+    net = build(args.size).to(dev)
+    z0, z1s, masks = (t.to(dev) for t in edits(args.size, 2 * E))
     pyrs = [downsample_mask(m, min_res=(4, 4), dilation=0) for m in masks]
     A, B = list(range(E)), list(range(E, 2 * E))
     batch_a, batch_b = (stack_mask_pyramids([pyrs[e] for e in ids]) for ids in (A, B))
@@ -248,7 +262,7 @@ def batched(args):
                     in_place = in_place and net.fused_step is step and net.masks_async_ok()
     caps = sorted({sl.cap for sl in step.low.slots.values()})
     out = {
-        "workload": "sd_decoder_%s_batch_of_%d" % (args.size, E),
+        "workload": "sd_%s_%s_batch_of_%d" % (args.model, args.size, E),
         "edits": [int(m.sum()) for m in masks[:E]],
         "gpu": gpu_info(),
         "ms_median": {k: statistics.median(v) for k, v in times.items()},
